@@ -1,4 +1,4 @@
-"""B200-native DaNet inference hot path (HRNet IUV estimator -> part regressors -> SMPL LBS ->
+"""H100-native DaNet inference hot path (HRNet IUV estimator -> part regressors -> SMPL LBS ->
 IUV rasteriser) behind the reference's call surface.  See DESIGN.md."""
 __version__ = "0.1.0"
 

@@ -77,7 +77,6 @@ SIGNATURES = {
     "danet_conv_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),
     "danet_conv_tc_group": (c_int, [c_int, ctypes.POINTER(ConvProblem), c_p]),
     "danet_conv_tc_config": (c_int, [c_int, ctypes.POINTER(ConvDesc), c_p, c_p]),
-    "danet_conv_tc_set_profile_buffer": (c_int, [c_p]),
     "danet_act_split": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_act_merge": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_nchw_to_nhwc": (c_int, [c_int, c_int, c_int, c_int, c_p, ctypes.POINTER(Act), c_p]),
@@ -113,7 +112,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 "danet_b200: %s not found -- build it with `python __graft_entry__.py` "
-                "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+                "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)          # AttributeError if the symbol is not exported

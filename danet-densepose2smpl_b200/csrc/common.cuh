@@ -1,4 +1,4 @@
-// Shared helpers for libdanet_b200.so (sm_100a only).
+// Shared helpers for libdanet_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

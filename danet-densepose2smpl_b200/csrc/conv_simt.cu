@@ -1,5 +1,5 @@
 // fp32 implicit-GEMM convolution on the FMA pipe (NHWC) -- the exact-parity path of the
-// network half and the fallback for shapes the tcgen05 kernel does not take.
+// network half and the fallback for shapes the wgmma kernel does not take.
 // Replaces nn.Conv2d (+ folded BatchNorm2d + ReLU + residual add) of models/module/hr_module.py,
 // models/module/res_module.py; grouped convolutions (res_module.py:335-342,500-535) are expressed
 // as `wsets` weight sets over the (batch,part)-flattened image axis (see include/danet_b200.h).

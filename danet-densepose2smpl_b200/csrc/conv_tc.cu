@@ -1,35 +1,39 @@
-// tcgen05 implicit-GEMM convolution engine for sm_100a, second generation.
+// wgmma implicit-GEMM convolution engine for sm_90a (Hopper).
 // The tensor-core path of models/module/hr_module.py:161-179,334-378 + res_module.py:27-97,281-390,393-535
 // convolutions (conv + folded BN + residual + ReLU): 1x1 / 3x3 / 7x7, stride 1 or 2, weight sets (the
 // reference's grouped convolutions over the (batch, part)-flattened image axis).
 //
 // Numerics.  Activations and weights are SPLIT-FP16: v = hi + lo with hi = rn_f16(v), lo = rn_f16(v - hi)
 // (22 significant bits, fp16 exponent range; plain fp32 numbers below 6e-5 keep an absolute error <= 3e-8).
-// "exact" mode issues three MMAs per K step, hi*hi + hi*lo + lo*hi, into one fp32 TMEM accumulator
-// (the dropped lo*lo term is 2^-22 relative): fp32-grade results from the fp16 tensor pipe, which is what
-// lets the default path meet the reference's fp32 outputs to 1e-4.  "fast" mode issues hi*hi only.
+// "exact" mode issues three products per K step, hi*hi + hi*lo + lo*hi, in fp32 accumulators (the dropped lo*lo
+// term is 2^-22 relative): fp32-grade results from the fp16 tensor pipe, which is what lets the default path meet
+// the reference's fp32 outputs to 1e-4.  "fast" mode issues hi*hi only.
 //
 // Structure (one persistent CTA per SM, warp-specialised, up to kMaxProb independent convolutions -- e.g. the
 // parallel branches of one HRNet stage -- in ONE launch over a concatenated tile space):
 //   A (activations): fp16 NHWC planes in HBM.  One TMA tensor-map load (cp.async.bulk.tensor.4d, SWIZZLE_128B/64B/32B,
 //       out-of-bounds zero fill = the convolution's padding, elementStrides = 2 for the parity planes of a
-//       stride-2 convolution) brings the input HALO of a tile -- (16+k-1) x (8*S+k-1) pixels x <= 64 channels --
+//       stride-2 convolution) brings the input HALO of a tile -- (16+k-1) x (8+k-1) pixels x <= 64 channels --
 //       into shared memory, one 128/64/32-byte row per pixel.  Eight consecutive MMA rows are eight consecutive
 //       pixels of one halo row, the next 8-row group is the next image row (SBO = halo pitch), so every filter
 //       tap is just a different descriptor start address: an input element crosses L2->SM ~1.3x, not 9x.
-//       S = 1 or 2 sub-tiles of 16 x 8 output pixels share one halo (256 pixels per pipeline step).
 //   B (weights): pre-packed once (danet_conv_tc_pack) into the swizzled shared-memory image of every
 //       (N tile, channel chunk, parity plane, tap group[, hi/lo]) block; streamed with 1-D cp.async.bulk.
-//   MMA: one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (M = 128, K = 16); accumulators in TMEM,
-//       two 256-column halves used alternately (a tile that needs more than 256 columns takes both).
-//       exact mode with 2*N <= 256: the hi and lo weight rows are concatenated along N, so hi*[hi|lo] is ONE
-//       MMA of width 2N (the A operand is fetched once) and the epilogue adds the two column ranges.
-//   MMA issue order (exact mode): N tiles above 64 channels (one accumulator chain per CTA) issue, per weight block, all
-//       hi*[hi|lo] MMAs and then all lo*hi MMAs (two same-shape chains); the other layers alternate per K step.
-//   Epilogue: 8 warps, row-per-thread (tcgen05.ld.32x32b.x16: lane = pixel, 16 channels per load); registers initialised
-//       with bias + residual, every K segment added in fp32 round-to-nearest, ReLU, output as split-fp16 planes and/or fp32.
+//   MMA: two consumer warpgroups, each owning 64 of the tile's 128 output pixels (8 image rows x 8 columns), issue
+//       wgmma.mma_async m64nNk16 (N = the tile's output channels) with fp32 accumulators in registers.
+//       exact mode: the hi and lo weight rows are concatenated along N, so hi*[hi|lo] is ONE MMA of width 2N whose
+//       second half lands in a separate small-term accumulator; lo*hi joins the small terms.  Per weight block all
+//       hi*[hi|lo] MMAs are issued first, then all lo*hi MMAs (two same-shape chains).
+//   K segments (exact mode): the tensor core's fp32 accumulation truncates, which biases long chains; after every
+//       lseg main-chain MMAs the accumulators are added in fp32 round-to-nearest to a running sum that starts at
+//       bias + residual.
+//   Epilogue: each consumer thread holds 2 pixels x 2 consecutive channels per 8-channel group; ReLU, output as
+//       split-fp16 planes and/or fp32.
+//   One producer warp: a single thread runs the tile scheduler and issues every TMA / bulk copy in the order the
+//       consumers use them.
 //   Launch: programmatic dependent launch; every mbarrier wait is bounded (traps instead of hanging).
 #include "common.cuh"
+#include "wgmma_f16.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <mutex>
@@ -40,15 +44,15 @@ namespace danet {
 namespace tc {
 
 constexpr int kTileH = 16, kTileW = 8;
-constexpr int kEpiWarps = 8;
-constexpr int kWarpA = 8, kWarpB = 9, kWarpMma = 10;   // the MMA issuer is the highest warp id (issue priority)
-constexpr int kThreads = 11 * 32;
-constexpr int kNumEpi = kEpiWarps * 32;
+constexpr int kConsumers = 2;                          // consumer warpgroups: 64 pixels (8 tile rows) each
+constexpr int kWarpProd = 4 * kConsumers;              // the producer warp follows the consumer warpgroups
+constexpr int kThreads = (kWarpProd + 1) * 32;
+constexpr int kNtMaxExact = 64, kNtMaxFast = 256;      // output channels per N tile: bounded by the register accumulators
 constexpr int kMaxAStages = 8, kMaxBStages = 8;
-constexpr int kSmemMax = 227 * 1024;                   // opt-in dynamic shared memory per CTA on sm_100
+constexpr int kSmemMax = 227 * 1024;                   // opt-in dynamic shared memory per CTA on sm_90
 constexpr int kSmemFixed = 2048;                       // barriers + 1024-byte alignment slack
 constexpr int kSchedDepth = 4, kSchedAhead = 2, kSchedStatic = 3;
-constexpr int kSchedConsumers = 2 + kEpiWarps;         // B producer, MMA warp, one lane per epilogue warp
+constexpr int kSchedConsumers = 4 * kConsumers;        // lane 0 of every consumer warp
 constexpr int kPackHeader = 1024;                      // packed weights start with a header: float[0] = 2^s applied to the weights, float[1] = 2^-s
 
 struct alignas(64) Prob {
@@ -57,21 +61,14 @@ struct alignas(64) Prob {
     const float* res_f; const __half* res_hi; const __half* res_lo;
     float* y_f; __half* y_hi; __half* y_lo;
     int N, H, W, Cin, Cout, Ho, Wo, ks, stride, pad, relu, wsets, exact;
-    int S;                               // sub-tiles (16 x 8 output pixels each) per pipeline step
     int npa;                             // active parity planes (1 for stride 1, up to 4 for stride 2)
     int SWB, KCH, nchunks;               // swizzle bytes per pixel row, channels per chunk, chunks
     int TG;                              // filter taps per weight block
     int NT, ntn;                         // output channels per N tile, N tiles
-    int nconcat;                         // exact mode: hi and lo weight rows share one block (one MMA of width 2*NT)
-    int ACC;                             // accumulator columns per sub-tile
-    int mo;                              // MMA issue order inside a weight block: 1 = all hi*[hi|lo] MMAs, then all lo*hi MMAs (two
-                                         // same-shape accumulate chains); 0 = alternating per K step.  A function of the layer's
-                                         // channel count alone, so that an image's bits do not depend on the batch it is in
-    int big;                             // S*ACC > 256: the tile takes both accumulator halves
     int nstack, hs, box_h;               // small maps: nstack images share one tile; image n's rows start at group n*hs
                                          // (hs = H + pad: the zero rows between images are the TMA out-of-bounds fill)
-    int lseg, nseg;                      // K segmentation: close a segment after a weight block once it holds >= lseg
-                                         // main-chain MMAs; nseg segments per tile (1 in fast mode)
+    int lseg;                            // K segmentation: close a segment after a weight block once it holds >= lseg
+                                         // main-chain MMAs (exact mode)
     int par_py[4], par_px[4], ntap[4], ngrp[4], stage_bytes[4], sbo_a[4];
     int tapoff16[4][16];                 // smem offset (16-byte units) of each tap's shifted view inside the plane
     int tapidx[4][16];                   // original filter tap index r*ks+s (weight packing)
@@ -86,19 +83,16 @@ struct alignas(64) Prob {
 constexpr int kMaxProb = 6;
 struct ArgsN {
     int nprob, total_tiles, na_stages, a_slot_bytes, nb_stages, b_slot_bytes;
-    int variant, pad_;                   // bring-up knock-outs (DANET_TC_VARIANT): 1 no stores, 2 no residual/bias loads, 4 no MMAs
-    long long* prof;                     // bring-up: per-role wait cycles of CTA 0 (danet_conv_tc_set_profile_buffer), else NULL
     unsigned* sched;                     // [2]: dynamic tile counter, finished-CTA counter (self-resetting); NULL = static round-robin
     Prob p[kMaxProb];
 };
 
 static unsigned long long magic40(int d) { return (1ull << 40) / (unsigned long long)d + 1ull; }
-static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
 
 // ---------------------------------------------------------------------------------------------
 // host: geometry of one problem (everything but the shared-memory ring sizes, which belong to the launch)
 // ---------------------------------------------------------------------------------------------
-static bool make_prob(const danet_conv_desc* d, int S_req, Prob* g) {
+static bool make_prob(const danet_conv_desc* d, Prob* g) {
     if (!(d->stride == 1 || d->stride == 2) || !(d->ksize == 1 || d->ksize == 3 || d->ksize == 7) || d->pad != d->ksize / 2) return false;
     if (d->Cin % 8 != 0 || d->Cout % 8 != 0 || d->H < 1 || d->W < 1 || d->N < 1 || d->wsets < 1) return false;
     g->N = d->N; g->H = d->H; g->W = d->W; g->Cin = d->Cin; g->Cout = d->Cout; g->ks = d->ksize;
@@ -107,39 +101,12 @@ static bool make_prob(const danet_conv_desc* d, int S_req, Prob* g) {
     g->Ho = (d->H + 2 * d->pad - d->ksize) / d->stride + 1;
     g->Wo = (d->W + 2 * d->pad - d->ksize) / d->stride + 1;
     if (g->Ho < 1 || g->Wo < 1) return false;
-    // N tiling / accumulators
-    // exact mode: N tiles of <= 128 channels, so that the hi and lo weight rows of a tap form ONE operand of 2*NT <= 256
-    // rows (hi*[hi|lo] is one MMA) and the small terms get their own accumulator columns [NT, 2*NT)
+    // N tiling: equal tiles of a multiple of 16 channels, at most kNtMax* (exact mode keeps three register
+    // accumulators per output -- main, small terms, running sum -- so its tiles are narrower)
     const int np = (d->Cout + 15) / 16 * 16;
-    const int ntmax = env_int(g->exact ? "DANET_TC_NTMAX_EXACT" : "DANET_TC_NTMAX_FAST", g->exact ? 128 : 256);
+    const int ntmax = g->exact ? kNtMaxExact : kNtMaxFast;
     g->ntn = (np + ntmax - 1) / ntmax;
     g->NT = ((np + g->ntn - 1) / g->ntn + 15) / 16 * 16;
-    // (experiment, off: measured 25.65 vs 24.79 ms/step) exact mode, k >= 3: cap a tap of [hi|lo] weight rows at 24 KB: the weight ring
-    // keeps its depth and the layer can share a launch with the wide-halo branches (384-channel 7x7 maps: NT 128 -> 96)
-    if (g->exact && d->ksize >= 3 && 2 * g->NT * 128 > 24 * 1024 && env_int("DANET_TC_NTRULE", 0)) {
-        g->ntn += 1;
-        g->NT = ((np + g->ntn - 1) / g->ntn + 15) / 16 * 16;
-    }
-    g->nconcat = g->exact;
-    g->ACC = g->NT * (g->nconcat ? 2 : 1);
-    // Exact-mode N tiles of more than 64 channels never pair sub-tiles (2 * ACC > 256 columns), whatever the batch: one
-    // accumulator chain per CTA.  Alternating the two MMA shapes per K step then makes every MMA wait for the previous
-    // one on the shared columns [NT, 2 NT) (measured: 1.3-1.8x the operand model); issued as two same-shape chains per
-    // weight block they stream like a plain GEMM main loop (192-ch 14x14: 63 -> 51 us, 384-ch 7x7: 66 -> 52 us, step
-    // 23.3 -> 21.3 ms).  Layers that MAY pair sub-tiles keep the alternating order in every tile -- the order of the fp32
-    // sums must not depend on S, which depends on the batch size (profiles/r02_mma_order.txt).
-    g->mo = (g->exact && 2 * g->ACC > 256 && env_int("DANET_TC_MMAORDER", 1)) ? 1 : 0;
-    int S = S_req;
-    if (g->Wo <= kTileW) S = 1;
-    if (g->exact && S * g->ACC > 256) S = 1;        // segmented accumulation wants two accumulator stages
-    if (S * g->ACC > 512) S = 1;
-    // sub-tile pairs only pay when the image is wide enough that few pairs are half empty and there are tiles to spare
-    {
-        const long long tiles2 = (long long)d->N * ((g->Ho + kTileH - 1) / kTileH) * ((g->Wo + 2 * kTileW - 1) / (2 * kTileW)) * g->ntn;
-        if (S == 2 && tiles2 < 2 * 148) S = 1;
-    }
-    g->S = S;
-    g->big = S * g->ACC > 256 ? 1 : 0;
     // parity decomposition: a stride-2 convolution is the sum over the input parities (py,px) of dense
     // stride-1 sub-convolutions; each parity plane is one TMA box with elementStrides = 2
     g->npa = 0;
@@ -157,13 +124,13 @@ static bool make_prob(const danet_conv_desc* d, int S_req, Prob* g) {
             tr_max = tr > tr_max ? tr : tr_max; tc_max = tcn > tc_max ? tcn : tc_max;
         }
     // every parity plane is loaded with the box of the largest one (one tensor map per input plane)
-    const int Hb = kTileH + tr_max - 1, Wb = kTileW * S + tc_max - 1;
+    const int Hb = kTileH + tr_max - 1, Wb = kTileW + tc_max - 1;
     // Small maps (H + pad <= 8): several images share the 16 row groups of a tile.  Image n of the tile is loaded by its
     // own TMA box [(H + 2 pad) rows] at row offset n * (H + pad): the bottom halo of one image and the top halo of the
     // next are the same shared-memory rows, both filled with out-of-bounds zeros.  Row groups that fall on those rows
     // produce garbage outputs the epilogue never stores.  Needs one weight set (consecutive images share weights).
     g->nstack = 1; g->hs = kTileH; g->box_h = Hb;
-    if (d->stride == 1 && d->wsets == 1 && d->H + d->pad <= kTileH / 2 && env_int("DANET_TC_STACK", 1)) {
+    if (d->stride == 1 && d->wsets == 1 && d->H + d->pad <= kTileH / 2) {
         g->hs = d->H + d->pad;
         g->nstack = kTileH / g->hs;
         g->box_h = d->H + 2 * d->pad;
@@ -172,15 +139,13 @@ static bool make_prob(const danet_conv_desc* d, int S_req, Prob* g) {
     int swb = 128;
     const int c16 = (d->Cin + 15) / 16 * 16;
     while (swb > 32 && swb / 2 >= 2 * c16) swb /= 2;
-    swb = env_int("DANET_TC_SWB", swb);
     g->SWB = swb; g->KCH = swb / 2;
     g->nchunks = (d->Cin + g->KCH - 1) / g->KCH;
-    g->rows_blk = g->NT * (g->nconcat ? 2 : 1);
+    g->rows_blk = g->NT * (g->exact ? 2 : 1);
     g->tap_bytes = g->rows_blk * swb;
     int tg = max_ntap;
-    // weight block size: larger blocks mean fewer barrier round trips (fast mode: +7 %, measured); exact mode keeps two
-    // more ring slots instead
-    while (tg > 1 && tg * g->tap_bytes > env_int("DANET_TC_TGKB", g->exact ? 24 : 48) * 1024) --tg;
+    // weight block size: larger blocks mean fewer barrier round trips; exact mode keeps more ring slots instead
+    while (tg > 1 && tg * g->tap_bytes > (g->exact ? 24 : 48) * 1024) --tg;
     g->TG = tg;
     g->b_block_bytes = (tg * g->tap_bytes + 1023) / 1024 * 1024;
     g->bpc = 0;
@@ -199,31 +164,9 @@ static bool make_prob(const danet_conv_desc* d, int S_req, Prob* g) {
         }
     }
     g->nblk = g->nchunks * g->bpc;
-    // K segmentation (exact mode): the tensor core accumulates with truncation, which biases long chains; a tile's K loop
-    // is cut after a weight block once >= lseg MMAs went into the main accumulator, and the epilogue sums the segments
-    // in fp32 round-to-nearest.  Needs all units of a warp in registers (<= 4) and two accumulator stages.
-    g->lseg = 1 << 30; g->nseg = 1;
-    {
-        const int gph0 = (g->NT / 16 + 1) / 2;
-        if (g->exact && !g->big && g->S * gph0 <= 4) {
-            g->lseg = env_int("DANET_TC_LSEG", 8);
-            int cnt = 0, nseg = 0;
-            for (int c = 0; c < g->nchunks; ++c) {
-                const int kreal = (d->Cin - c * g->KCH + 15) / 16, kmma = g->KCH / 16;
-                const int kv = kreal < kmma ? kreal : kmma;
-                for (int a = 0; a < g->npa; ++a)
-                    for (int t = 0; t < g->ngrp[a]; ++t) {
-                        const int ntk = g->ntap[a] - t * g->TG < g->TG ? g->ntap[a] - t * g->TG : g->TG;
-                        cnt += ntk * kv;
-                        const bool last = c == g->nchunks - 1 && a == g->npa - 1 && t == g->ngrp[a] - 1;
-                        if (last || cnt >= g->lseg) { ++nseg; cnt = 0; }
-                    }
-            }
-            g->nseg = nseg;
-        }
-    }
+    g->lseg = g->exact ? 8 : (1 << 30);
     g->blocks_per_set = (long long)g->ntn * g->nblk;
-    g->tiles_w = (g->Wo + kTileW * S - 1) / (kTileW * S); g->tiles_h = (g->Ho + kTileH - 1) / kTileH;
+    g->tiles_w = (g->Wo + kTileW - 1) / kTileW; g->tiles_h = (g->Ho + kTileH - 1) / kTileH;
     const long long tiles = (long long)((d->N + g->nstack - 1) / g->nstack) * g->tiles_h * g->tiles_w * g->ntn;
     if (tiles >= (1 << 24) || g->wsets >= (1 << 16)) return false;
     if ((long long)d->N * g->Ho * g->Wo * d->Cout >= (1LL << 31) || (long long)d->N * d->H * d->W * d->Cin >= (1LL << 31)) return false;   // 32-bit element offsets
@@ -233,7 +176,7 @@ static bool make_prob(const danet_conv_desc* d, int S_req, Prob* g) {
 }
 static int max_stage_bytes(const Prob& g) { int m = 0; for (int a = 0; a < g.npa; ++a) m = g.stage_bytes[a] > m ? g.stage_bytes[a] : m; return m; }
 
-// ring sizes of a launch over n problems; false if they cannot fit even with S = 1 everywhere
+// ring sizes of a launch over n problems; false if they cannot fit
 static bool plan_rings(ArgsN* a) {
     int amax = 0, bmax = 0, need_a = 2;
     for (int i = 0; i < a->nprob; ++i) {
@@ -244,10 +187,9 @@ static bool plan_rings(ArgsN* a) {
     }
     a->a_slot_bytes = (amax + 1023) / 1024 * 1024;
     a->b_slot_bytes = (bmax + 1023) / 1024 * 1024;
-    int nb = env_int("DANET_TC_NB", 3);
+    int nb = 3;
     int na = (kSmemMax - kSmemFixed - nb * a->b_slot_bytes) / a->a_slot_bytes;
     if (na < need_a) { nb = 2; na = (kSmemMax - kSmemFixed - nb * a->b_slot_bytes) / a->a_slot_bytes; }
-    if (na < (need_a == 4 ? 2 : 2)) return false;
     if (na < need_a) return false;
     if (na > kMaxAStages) na = kMaxAStages;
     // spend what is left on deeper weight prefetch
@@ -269,8 +211,7 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// one out-of-line copy: the bounded polling loop is ~40 SASS instructions and there are ~30 wait sites; inlined (and
-// unrolled by the compiler) they made the kernel 101 KB of code and the instruction cache hit rate 78 % (ncu)
+// one out-of-line copy: the bounded polling loop is ~40 SASS instructions and there are many wait sites
 __device__ __noinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t done = 0;
 #pragma unroll 1
@@ -283,13 +224,6 @@ __device__ __noinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         if (done) return;
     }
     __trap();                                        // bounded wait: never hang the device
-}
-// bring-up instrumentation: a wait that adds its duration to *acc when profiling is on
-__device__ __forceinline__ void mbar_wait_t(uint32_t bar, uint32_t parity, bool on, long long* acc) {
-    if (!on) { mbar_wait(bar, parity); return; }
-    const long long t0 = clock64();
-    mbar_wait(bar, parity);
-    *acc += clock64() - t0;
 }
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -306,42 +240,22 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
 // previous kernel wrote (activations, residual) or still reads (our output may be its input) is touched before pdl_wait()
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// 32 lanes x 32 bits, 16 columns: thread i of the warp receives TMEM lane (base lane + i), columns 0..15
-__device__ __forceinline__ void tc_ld32x32_x16_nowait(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads across wgmma.wait_group
+template <int NV> __device__ __forceinline__ void reg_fence(float* d) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < NV; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// K-major swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, version 1).
-// layout_type: SWIZZLE_128B = 2, SWIZZLE_64B = 4, SWIZZLE_32B = 6; LBO is unused for swizzled K-major.
-// The hardware derives the swizzle phase from the absolute shared-memory address, so a start address that is
-// only row-aligned (a filter tap shifted by a few pixels) needs no base_offset (verified on B200, round 1).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
+// K-major swizzled shared-memory matrix descriptor of wgmma: start address and SBO (the stride between 8-row groups)
+// in 16-byte units, LBO unused for swizzled K-major layouts, swizzle mode in bits 62-63 (128B = 1, 64B = 2, 32B = 3).
+// The swizzle phase follows the absolute shared-memory address (the TMA writes the same pattern), so a start
+// address that is only row-aligned (a filter tap shifted by a few pixels) needs no base offset.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t swb) {
+    const uint32_t mode = swb == 128 ? 1u : (swb == 64 ? 2u : 3u);
     const uint32_t lo = ((saddr >> 4) & 0x3FFFu) | (1u << 16);
-    const uint32_t hi = ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (layout_type << 29);
+    const uint32_t hi = ((sbo_bytes >> 4) & 0x3FFFu) | (mode << 30);
     return ((uint64_t)hi << 32) | lo;
 }
 // physical offset of logical byte offset `off` inside a 1024-byte-aligned swizzled region
@@ -367,24 +281,41 @@ __device__ __forceinline__ TileCoord decode_tile(const Prob& g, int t) {
     return c;
 }
 
+// One MMA of runtime width n (a multiple of 16, <= NMAX): accumulator columns [0, n/2) in lo, [n/2, n) in hi.
+template <int NMAX>
+__device__ __forceinline__ void mma_n(int n, float* lo, float* hi, uint64_t a, uint64_t b, uint32_t acc) {
+#define DANET_WG_CASE(N) case N: if (N <= NMAX) Wgmma<(N <= NMAX ? N : 16)>::mma(lo, hi, a, b, acc); break;
+    switch (n) {
+        DANET_WG_CASE(16) DANET_WG_CASE(32) DANET_WG_CASE(48) DANET_WG_CASE(64) DANET_WG_CASE(80) DANET_WG_CASE(96)
+        DANET_WG_CASE(112) DANET_WG_CASE(128) DANET_WG_CASE(144) DANET_WG_CASE(160) DANET_WG_CASE(176) DANET_WG_CASE(192)
+        DANET_WG_CASE(208) DANET_WG_CASE(224) DANET_WG_CASE(240) DANET_WG_CASE(256)
+        default: break;
+    }
+#undef DANET_WG_CASE
+}
+// the plain accumulator of width n: registers d[0, n/2) (the column split point moves with n)
+template <int NMAX>
+__device__ __forceinline__ void mma_plain(int n, float* d, uint64_t a, uint64_t b, uint32_t acc) {
+#define DANET_WG_CASE(N) case N: if (N <= NMAX) Wgmma<(N <= NMAX ? N : 16)>::mma(d, d + (N <= NMAX ? N : 16) / 4, a, b, acc); break;
+    switch (n) {
+        DANET_WG_CASE(16) DANET_WG_CASE(32) DANET_WG_CASE(48) DANET_WG_CASE(64) DANET_WG_CASE(80) DANET_WG_CASE(96)
+        DANET_WG_CASE(112) DANET_WG_CASE(128) DANET_WG_CASE(144) DANET_WG_CASE(160) DANET_WG_CASE(176) DANET_WG_CASE(192)
+        DANET_WG_CASE(208) DANET_WG_CASE(224) DANET_WG_CASE(240) DANET_WG_CASE(256)
+        default: break;
+    }
+#undef DANET_WG_CASE
+}
+
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
-// PROF: bring-up instrumentation (per-role wait cycles); a separate instantiation so that the production kernel carries
-// none of its code
-// 256-bit global stores (sm_100: STG.E.ENL2.256): p must be 32-byte aligned
-__device__ __forceinline__ void st_global_v8(float* p, const float* v) {
-    asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]),
-                 "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
-}
-
-// EX: precision mode fixed at compile time (1 = every problem of the launch is exact, 0 = every problem is fast, -1 = read
-// it per problem).  The mode-specific instantiations drop the other mode's branches from every role's loop: this kernel
-// is sensitive to its instruction footprint (three knock-out branches were worth 2 % of the step).
-// RESF: some problem of the launch adds an fp32 residual view (else that path is not compiled in).
-template <bool PROF, int EX, bool RESF>
+// EX: precision mode fixed at compile time (1: every problem of the launch is exact, 0: every problem is fast).
+// NV: fp32 accumulator registers per thread and array (a 64 x NT warpgroup tile holds NT / 2 per thread).
+template <int EX>
 __global__ void __launch_bounds__(kThreads, 1)
 k_conv_tc(const __grid_constant__ ArgsN a) {
+    constexpr int NTMAX = EX ? kNtMaxExact : kNtMaxFast;
+    constexpr int NV = NTMAX / 2;
     extern __shared__ __align__(1024) uint8_t smem[];
     const uint32_t sbase = (smem_u32(smem) + 1023u) & ~1023u;          // swizzle atoms need 1024-byte alignment
     const uint32_t sA = sbase;
@@ -393,41 +324,26 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
     // barrier map (8 bytes each)
     const uint32_t bar_a_full = sBar, bar_a_empty = sBar + 8 * kMaxAStages;
     const uint32_t bar_b_full = sBar + 16 * kMaxAStages, bar_b_empty = bar_b_full + 8 * kMaxBStages;
-    const uint32_t bar_acc_full = bar_b_empty + 8 * kMaxBStages, bar_acc_empty = bar_acc_full + 16;
-    const uint32_t tmem_slot_addr = bar_acc_empty + 16;
-    // dynamic tile scheduler: a ring of kSchedDepth tile indices published by the A producer (it takes them from a
-    // global atomic counter, heaviest problems first) and read by the other roles
+    // dynamic tile scheduler: a ring of kSchedDepth tile indices published by the producer (it takes them from a
+    // global atomic counter, heaviest problems first) and read by the consumer warps
     const uint32_t bar_sched_full = sBar + 512, bar_sched_empty = sBar + 512 + 8 * kSchedDepth, sched_ring = sBar + 512 + 16 * kSchedDepth;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; ++i) { mbar_init(bar_acc_full + 8 * i, 1); mbar_init(bar_acc_empty + 8 * i, kNumEpi); }
-        for (int i = 0; i < a.na_stages; ++i) { mbar_init(bar_a_full + 8 * i, 1); mbar_init(bar_a_empty + 8 * i, 1); }
-        for (int i = 0; i < a.nb_stages; ++i) { mbar_init(bar_b_full + 8 * i, 1); mbar_init(bar_b_empty + 8 * i, 1); }
+        for (int i = 0; i < a.na_stages; ++i) { mbar_init(bar_a_full + 8 * i, 1); mbar_init(bar_a_empty + 8 * i, kConsumers); }
+        for (int i = 0; i < a.nb_stages; ++i) { mbar_init(bar_b_full + 8 * i, 1); mbar_init(bar_b_empty + 8 * i, kConsumers); }
         for (int i = 0; i < kSchedDepth; ++i) { mbar_init(bar_sched_full + 8 * i, 1); mbar_init(bar_sched_empty + 8 * i, kSchedConsumers); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == kWarpA && lane < a.nprob) { tma_prefetch_desc(&a.p[lane].tm[0]); if (EX < 0 ? a.p[lane].exact : EX) tma_prefetch_desc(&a.p[lane].tm[1]); }
-    if (warp == kWarpMma) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot_addr), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
+    if (warp == kWarpProd && lane < a.nprob) { tma_prefetch_desc(&a.p[lane].tm[0]); if (EX) tma_prefetch_desc(&a.p[lane].tm[1]); }
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot_addr));
     pdl_launch_dependents();            // the next launch may fill SMs as our CTAs retire
 
-    if (warp == kWarpA) {
-        // ================= A producer: one TMA box per (plane, channel chunk, parity plane) =================
+    if (warp == kWarpProd) {
+        // ================= producer: tile scheduler + every TMA / bulk copy, in consumption order =================
         if (lane == 0) {
-            int as = 0; uint32_t aph = 0;
-            int pi = 0;
-            const bool pon = PROF && a.prof != nullptr && blockIdx.x == 0;
-            long long pw = 0; const long long pt0 = clock64();
-            // Tile scheduler: this thread publishes tile indices kSchedAhead tiles ahead of its own loads, so that the
-            // weight producer can prefetch for the coming tiles while the MMAs work on the current one.  The first
+            int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
+            // Tile scheduler: this thread publishes tile indices kSchedAhead tiles ahead of its own loads.  The first
             // kSchedStatic tiles of a CTA are its round-robin share (no atomic latency at start-up), later ones come
             // from the global counter (heaviest problems first): greedy list scheduling over heterogeneous tiles.
             int pub = 0; bool ended = false;
@@ -447,15 +363,18 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
                 asm volatile("ld.shared.s32 %0, [%1];" : "=r"(tile) : "r"(sched_ring + 4 * (seq & (kSchedDepth - 1))) : "memory");
                 if (tile >= a.total_tiles) break;
                 if (seq == 0) pdl_wait();                            // activations come from the previous kernel
-                pi = 0;
+                int pi = 0;
                 while (tile >= a.p[pi].tile_base + a.p[pi].tile_count) ++pi;
                 const Prob& P = a.p[pi];
                 const TileCoord tc = decode_tile(P, tile - P.tile_base);
-                const int h0 = tc.th * kTileH * P.stride - P.pad, w0 = tc.tw * kTileW * P.S * P.stride - P.pad;
+                const int h0 = tc.th * kTileH * P.stride - P.pad, w0 = tc.tw * kTileW * P.stride - P.pad;
+                const int ws = tc.img - mdiv(tc.img, P.m_ws) * P.wsets;
+                const uint8_t* src = P.wpk + kPackHeader + ((long long)ws * P.blocks_per_set + (long long)tc.nt * P.nblk) * P.b_block_bytes;
+                int b = 0;
                 for (int c = 0; c < P.nchunks; ++c)
-                    for (int slot = 0; slot < P.npa; ++slot)
-                        for (int pl = 0; pl <= (EX < 0 ? P.exact : EX); ++pl) {
-                            mbar_wait_t(bar_a_empty + 8 * as, ((aph >> as) & 1u) ^ 1u, pon, &pw);
+                    for (int slot = 0; slot < P.npa; ++slot) {
+                        for (int pl = 0; pl <= EX; ++pl) {
+                            mbar_wait(bar_a_empty + 8 * as, ((aph >> as) & 1u) ^ 1u);
                             if (P.nstack > 1) {
                                 const uint32_t box_bytes = (uint32_t)(P.box_h * P.sbo_a[slot]);
                                 mbar_expect_tx(bar_a_full + 8 * as, box_bytes * P.nstack);
@@ -463,407 +382,223 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
                                     tma_load_4d(sA + as * a.a_slot_bytes + n * P.hs * P.sbo_a[slot], &P.tm[pl], c * P.KCH, w0, -P.pad,
                                                 tc.img * P.nstack + n, bar_a_full + 8 * as);
                             } else {
-                            mbar_expect_tx(bar_a_full + 8 * as, (uint32_t)P.stage_bytes[slot]);
-                            tma_load_4d(sA + as * a.a_slot_bytes, &P.tm[pl], c * P.KCH, w0 + P.par_px[slot], h0 + P.par_py[slot],
-                                        tc.img, bar_a_full + 8 * as);
+                                mbar_expect_tx(bar_a_full + 8 * as, (uint32_t)P.stage_bytes[slot]);
+                                tma_load_4d(sA + as * a.a_slot_bytes, &P.tm[pl], c * P.KCH, w0 + P.par_px[slot], h0 + P.par_py[slot],
+                                            tc.img, bar_a_full + 8 * as);
                             }
                             aph ^= 1u << as;
                             if (++as == a.na_stages) as = 0;
                         }
+                        for (int t = 0; t < P.ngrp[slot]; ++t, ++b) {
+                            mbar_wait(bar_b_empty + 8 * bs, ((bph >> bs) & 1u) ^ 1u);
+                            mbar_expect_tx(bar_b_full + 8 * bs, (uint32_t)P.b_block_bytes);
+                            bulk_g2s(sB + bs * a.b_slot_bytes, src + (long long)b * P.b_block_bytes, (uint32_t)P.b_block_bytes, bar_b_full + 8 * bs);
+                            bph ^= 1u << bs;
+                            if (++bs == a.nb_stages) bs = 0;
+                        }
+                    }
             }
-            if (pon) { a.prof[0] = clock64() - pt0; a.prof[1] = pw; }
         }
-    } else if (warp == kWarpB) {
-        // ================= B producer: bulk copies of pre-packed weight blocks =================
-        if (lane == 0) {
-            int bs = 0; uint32_t bph = 0;
-            int pi = 0;
-            const bool pon = PROF && a.prof != nullptr && blockIdx.x == 0;
-            long long pw = 0, ps = 0; const long long pt0 = clock64();
-            for (int seq = 0;; ++seq) {
-                const long long ts0 = pon ? clock64() : 0;
-                const int tile = sched_next(bar_sched_full, bar_sched_empty, sched_ring, seq);
-                if (pon) ps += clock64() - ts0;
-                if (tile >= a.total_tiles) break;
-                pi = 0;
-                while (tile >= a.p[pi].tile_base + a.p[pi].tile_count) ++pi;
-                const Prob& P = a.p[pi];
-                const TileCoord tc = decode_tile(P, tile - P.tile_base);
-                const int ws = tc.img - mdiv(tc.img, P.m_ws) * P.wsets;
-                const uint8_t* src = P.wpk + kPackHeader + ((long long)ws * P.blocks_per_set + (long long)tc.nt * P.nblk) * P.b_block_bytes;
-                for (int b = 0; b < P.nblk; ++b) {
-                    mbar_wait_t(bar_b_empty + 8 * bs, ((bph >> bs) & 1u) ^ 1u, pon, &pw);
-                    mbar_expect_tx(bar_b_full + 8 * bs, (uint32_t)P.b_block_bytes);
-                    bulk_g2s(sB + bs * a.b_slot_bytes, src + (long long)b * P.b_block_bytes, (uint32_t)P.b_block_bytes, bar_b_full + 8 * bs);
-                    bph ^= 1u << bs;
-                    if (++bs == a.nb_stages) bs = 0;
-                }
-            }
-            if (pon) { a.prof[2] = clock64() - pt0; a.prof[3] = pw; a.prof[4] = ps; }
-        }
-    } else if (warp == kWarpMma) {
-        // ================= MMA issuer =================
-        // The whole warp runs the loop (warp-uniform control flow keeps descriptors in uniform registers); one
-        // elected lane issues the tcgen05 instructions.
-        int as = 0, bs = 0; uint32_t aph = 0, bph = 0, eph = 0; int tog = 0;
-        int pi = 0;
-        const bool pon = PROF && a.prof != nullptr && blockIdx.x == 0;
-        long long pwa = 0, pwb = 0, pwe = 0, pws = 0; const long long pt0 = clock64();
+    } else {
+        // ================= consumer warpgroups: wgmma main loop + epilogue =================
+        const int wg = warp >> 2, w4 = warp & 3;
+        const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
+        // accumulator fragment of m64nNk16: this thread owns tile rows prow0, prow0 + 1 at column pcol, and channels
+        // 8 j + cq, 8 j + cq + 1 of every 8-channel group j (registers 4 j + 2 r + {0, 1} for row prow0 + r)
+        const int prow0 = 8 * wg + 2 * w4, pcol = lane >> 2, cq = 2 * (lane & 3);
+        float m[NV];                      // main accumulator (fast mode: the only one)
+        float s[EX ? NV : 1];             // exact: small terms hi*lo + lo*hi
+        float sum[EX ? NV : 1];           // exact: bias + residual + every closed K segment, fp32 round-to-nearest
+        int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
+        pdl_wait();                                              // residual reads / output writes
         for (int seq = 0;; ++seq) {
             int tile = 0;
-            const long long ts0 = pon ? clock64() : 0;
             if (lane == 0) tile = sched_next(bar_sched_full, bar_sched_empty, sched_ring, seq);
             tile = __shfl_sync(0xffffffffu, tile, 0);
-            if (pon) pws += clock64() - ts0;
             if (tile >= a.total_tiles) break;
-            pi = 0;
+            int pi = 0;
             while (tile >= a.p[pi].tile_base + a.p[pi].tile_count) ++pi;
             const Prob& P = a.p[pi];
             const TileCoord tc = decode_tile(P, tile - P.tile_base);
-            const int exact = EX < 0 ? P.exact : EX, big = EX == 1 ? 0 : P.big;      // exact mode never takes both accumulator halves
-            const int lseg = P.lseg, nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
-            // the second sub-tile of the last tile column may lie wholly outside the image: its MMAs are skipped
-            const bool S2 = P.S == 2 && (tc.tw * 2 + 1) * kTileW < P.Wo;
-            const uint32_t ACC = (uint32_t)P.ACC, NT = (uint32_t)P.NT;
-            // kind::f16, A/B = F16 (format 0), D = F32, both K-major, N>>3 at bit 17, M>>4 at bit 24
-            const uint32_t idesc1 = (1u << 4) | ((uint32_t)(NT >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t idesc2 = (1u << 4) | ((uint32_t)((2 * NT) >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t ltype = SWB == 128 ? 2u : (SWB == 64 ? 4u : 6u);
-            const uint64_t bd0 = make_desc(0, 8 * SWB, ltype);
+            const int NT = P.NT, Cout = P.Cout, Wo = P.Wo, Ho = P.Ho;
+            const int nj = NT >> 3;                               // 8-channel groups of the tile
+            const int cw = Cout - tc.nt * NT;                     // channels of this N tile that exist (multiple of 8)
+            // this thread's two output pixels: tile row prow of image tc.img, or (stacked small maps) row prow % hs of image
+            // tc.img * nstack + prow / hs -- rows hs-pad.. of a stacked image are the shared zero rows (no output)
+            uint32_t eoff[2]; int boff[2]; bool ok[2];
+            const int ow = tc.tw * kTileW + pcol;
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int prow = prow0 + r;
+                int oh = tc.th * kTileH + prow, img = tc.img;
+                bool row_ok = oh < Ho;
+                if (P.nstack > 1) {
+                    const int n = prow / P.hs;
+                    oh = prow - n * P.hs; img = tc.img * P.nstack + n;
+                    row_ok = oh < Ho && n < P.nstack && img < P.N;
+                }
+                ok[r] = row_ok && ow < Wo;
+                eoff[r] = ((uint32_t)(img * Ho + oh) * Wo + ow) * Cout + tc.nt * NT + cq;
+                boff[r] = (img - mdiv(img, P.m_ws) * P.wsets) * Cout + tc.nt * NT + cq;
+            }
+            // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
+            // residual enter the sum times 2^s and the result leaves it times 2^-s -- exact in fp32
+            const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
+            // bias + residual of this thread's outputs, times 2^s, into v (the exact mode's running sum starts there;
+            // fast mode adds it to the accumulator after the main loop)
+            auto init = [&](float* v, bool add) {
+#pragma unroll
+                for (int j = 0; j < NV / 4; ++j) {
+                    if (j >= nj) break;
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        float2 t = make_float2(0.f, 0.f);
+                        if (8 * j < cw) {
+                            if (P.bias) t = __ldg(reinterpret_cast<const float2*>(P.bias + boff[r] + 8 * j));
+                            if (ok[r]) {
+                                if (P.res_f) {
+                                    const float2 q = __ldg(reinterpret_cast<const float2*>(P.res_f + eoff[r] + 8 * j));
+                                    t.x += q.x; t.y += q.y;
+                                } else if (P.res_hi) {
+                                    const float2 q = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_hi + eoff[r] + 8 * j)));
+                                    t.x += q.x; t.y += q.y;
+                                    if (P.res_lo) {
+                                        const float2 q2 = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_lo + eoff[r] + 8 * j)));
+                                        t.x += q2.x; t.y += q2.y;
+                                    }
+                                }
+                            }
+                        }
+                        if (add) { v[4 * j + 2 * r] += t.x * wsc.x; v[4 * j + 2 * r + 1] += t.y * wsc.x; }
+                        else { v[4 * j + 2 * r] = t.x * wsc.x; v[4 * j + 2 * r + 1] = t.y * wsc.x; }
+                    }
+                }
+            };
+            if constexpr (EX) init(sum, false);
+            const int nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
             const int kmma = P.KCH / 16;                          // K = 16 halves (32 bytes) per MMA
             const uint32_t tap16 = P.tap_bytes >> 4;
-            const uint32_t sub16 = (uint32_t)(kTileW * SWB) >> 4;
-            bool need_acc = true;                                 // next MMA opens a K segment: take an accumulator stage
-            uint32_t acc = 0, d_base = 0;
-            int cs = 0, seg_cnt = 0;
+            const uint64_t bd0 = make_desc(0, 8 * SWB, SWB);
+            uint32_t acc = 0;
+            int seg_cnt = 0;
             for (int c = 0; c < nchunks; ++c) {
                 const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
                 const int kv = kreal < kmma ? kreal : kmma;       // K steps wholly beyond Cin are not issued
                 for (int slot = 0; slot < npa; ++slot) {
                     const int as_hi = as;
-                    mbar_wait_t(bar_a_full + 8 * as, (aph >> as) & 1u, pon, &pwa);
+                    mbar_wait(bar_a_full + 8 * as, (aph >> as) & 1u);
                     aph ^= 1u << as; if (++as == a.na_stages) as = 0;
                     int as_lo = as_hi;
-                    if (exact) {
+                    if (EX) {
                         as_lo = as;
-                        mbar_wait_t(bar_a_full + 8 * as, (aph >> as) & 1u, pon, &pwa);
+                        mbar_wait(bar_a_full + 8 * as, (aph >> as) & 1u);
                         aph ^= 1u << as; if (++as == a.na_stages) as = 0;
                     }
-                    tc_fence_after();
-                    const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a[slot], ltype);
+                    // this warpgroup's 8 tile rows start 8 halo rows further down for the second warpgroup
+                    const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB) + ((uint32_t)(wg * 8 * P.sbo_a[slot]) >> 4);
                     const uint64_t ad_hi = ad0 + ((sA + as_hi * a.a_slot_bytes) >> 4);
                     const uint64_t ad_lo = ad0 + ((sA + as_lo * a.a_slot_bytes) >> 4);
                     const int ngrp = P.ngrp[slot], ntap = P.ntap[slot];
                     for (int tg = 0; tg < ngrp; ++tg) {
                         const int k0 = tg * TG;
                         const int ntk = min(TG, ntap - k0);
-                        if (need_acc) {
-                            if (big) {
-                                mbar_wait_t(bar_acc_empty, (eph & 1u) ^ 1u, pon, &pwe); mbar_wait_t(bar_acc_empty + 8, ((eph >> 1) & 1u) ^ 1u, pon, &pwe);
-                                eph ^= 3u; cs = 0;
-                            } else {
-                                cs = tog; tog ^= 1;
-                                mbar_wait_t(bar_acc_empty + 8 * cs, ((eph >> cs) & 1u) ^ 1u, pon, &pwe);
-                                eph ^= 1u << cs;
-                            }
-                            tc_fence_after();
-                            d_base = tmem_base + cs * 256;
-                            acc = 0; need_acc = false; seg_cnt = 0;
-                        }
-                        mbar_wait_t(bar_b_full + 8 * bs, (bph >> bs) & 1u, pon, &pwb);
-                        tc_fence_after();
+                        mbar_wait(bar_b_full + 8 * bs, (bph >> bs) & 1u);
                         const uint64_t bd = bd0 + ((sB + bs * a.b_slot_bytes) >> 4);
-                        if (elect_one()) {
-                            if (EX != 0 && exact && P.mo) {
-                                // one accumulator chain per CTA (N tiles of 96 / 128 channels, see make_prob): two same-shape
-                                // chains per weight block; the sums are the same products in another order
-                                const int nt_ = (PROF && (a.variant & 4)) ? 0 : ntk;
-                                for (int tt = 0; tt < nt_; ++tt) {
-                                    const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                                    for (int kk = 0; kk < kv; ++kk) {
-                                        tc_mma_f16(d_base, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, idesc2, acc);
-                                        acc = 1;
-                                    }
-                                }
-                                for (int tt = 0; tt < nt_; ++tt) {
-                                    const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                                    for (int kk = 0; kk < kv; ++kk)
-                                        tc_mma_f16(d_base + NT, ad_lo + toff + 2 * kk, bd + tt * tap16 + 2 * kk, idesc1, 1u);
-                                }
-                            } else
-                            for (int tt = 0; tt < ((PROF && (a.variant & 4)) ? 0 : ntk); ++tt) {
+                        wg_fence();
+                        if constexpr (EX) {
+                            // hi * [hi | lo]: main chain in m, small terms in s; then lo * hi into s
+                            #pragma unroll 1
+                            for (int tt = 0; tt < ntk; ++tt) {
                                 const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
+                                #pragma unroll 1
                                 for (int kk = 0; kk < kv; ++kk) {
-                                    const uint64_t bdk = bd + tt * tap16 + 2 * kk;
-                                    const uint64_t adh = ad_hi + toff + 2 * kk, adl = ad_lo + toff + 2 * kk;
-                                    if (!exact) {
-                                        tc_mma_f16(d_base, adh, bdk, idesc1, acc);
-                                        if (S2) tc_mma_f16(d_base + ACC, adh + sub16, bdk, idesc1, acc);
-                                    } else {
-                                        // hi * [hi | lo]: main chain in columns [0, NT), small terms in [NT, 2 NT);
-                                        // lo * hi joins the small terms
-                                        tc_mma_f16(d_base, adh, bdk, idesc2, acc);
-                                        if (S2) tc_mma_f16(d_base + ACC, adh + sub16, bdk, idesc2, acc);
-                                        tc_mma_f16(d_base + NT, adl, bdk, idesc1, 1u);
-                                        if (S2) tc_mma_f16(d_base + ACC + NT, adl + sub16, bdk, idesc1, 1u);
-                                    }
+                                    mma_n<2 * NTMAX>(2 * NT, m, s, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
                                     acc = 1;
                                 }
                             }
-                            tc_commit(bar_b_empty + 8 * bs);
+                            #pragma unroll 1
+                            for (int tt = 0; tt < ntk; ++tt) {
+                                const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
+                                #pragma unroll 1
+                                for (int kk = 0; kk < kv; ++kk)
+                                    mma_plain<NTMAX>(NT, s, ad_lo + toff + 2 * kk, bd + tt * tap16 + 2 * kk, 1u);
+                            }
+                        } else {
+                            #pragma unroll 1
+                            for (int tt = 0; tt < ntk; ++tt) {
+                                const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
+                                #pragma unroll 1
+                                for (int kk = 0; kk < kv; ++kk) {
+                                    mma_plain<NTMAX>(NT, m, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
+                                    acc = 1;
+                                }
+                            }
                         }
-                        __syncwarp();
-                        acc = 1;
+                        wg_commit();
+                        wg_wait_all();
+                        reg_fence<NV>(m);
+                        if (leader) mbar_arrive(bar_b_empty + 8 * bs);
                         bph ^= 1u << bs; if (++bs == a.nb_stages) bs = 0;
-                        seg_cnt += ntk * kv;
-                        const bool last = c == nchunks - 1 && slot == npa - 1 && tg == ngrp - 1;
-                        if (last || seg_cnt >= lseg) {            // close the K segment: hand the accumulator to the epilogue
-                            if (elect_one()) tc_commit(bar_acc_full + 8 * cs);
-                            __syncwarp();
-                            need_acc = true;
+                        if constexpr (EX) {
+                            reg_fence<NV>(s);
+                            seg_cnt += ntk * kv;
+                            const bool last = c == nchunks - 1 && slot == npa - 1 && tg == ngrp - 1;
+                            if (last || seg_cnt >= P.lseg) {              // close the K segment
+#pragma unroll
+                                for (int j = 0; j < NV; ++j) {
+                                    if (j >= 4 * nj) break;
+                                    sum[j] += m[j];
+                                    sum[j] += s[j];
+                                }
+                                acc = 0; seg_cnt = 0;
+                            }
                         }
                     }
-                    if (elect_one()) {
-                        tc_commit(bar_a_empty + 8 * as_hi);
-                        if (exact) tc_commit(bar_a_empty + 8 * as_lo);
+                    if (leader) {
+                        mbar_arrive(bar_a_empty + 8 * as_hi);
+                        if (EX) mbar_arrive(bar_a_empty + 8 * as_lo);
                     }
-                    __syncwarp();
                 }
             }
-        }
-        if (pon && lane == 0) { a.prof[5] = clock64() - pt0; a.prof[6] = pwa; a.prof[7] = pwb; a.prof[8] = pwe; a.prof[9] = pws; }
-    } else {
-        // ================= epilogue: TMEM -> (+ bias, residual) -> ReLU -> global =================
-        // Row-per-thread mapping (tcgen05.ld 32x32b.x16): lane i of a warp owns TMEM lane 32q+i = output pixel
-        // (tile row 4q + i/8, column i%8) and receives 16 consecutive output channels per load: every global access
-        // is a 16-byte vector of one pixel.  A "unit" = (sub-tile, 16-column group); the two warps of a TMEM lane
-        // quarter take alternate groups.  Per batch of <= 4 units the register accumulators are INITIALISED with
-        // bias + residual (all their global loads are issued before the accumulator wait, one latency exposure per
-        // tile, under the MMAs of the same tile), then every K segment of the tile is added from TMEM in fp32
-        // (round-to-nearest: the tensor core's own accumulation truncates, so long K chains are cut into segments),
-        // then ReLU, split into hi/lo fp16 planes and stored.
-        const int q = warp & 3;                                  // TMEM lane quarter this warp may access
-        const int half = warp >> 2;                              // 0/1: which 16-column groups this warp owns
-        const int prow = 4 * q + (lane >> 3), pcol = lane & 7;    // this thread's pixel inside the sub-tile
-        uint32_t fph = 0; int tog = 0;
-        int pi = 0;
-        const bool do_store = !(PROF && (a.variant & 1));          // knock-outs live in the profiling instantiation only
-        const bool pon = PROF && a.prof != nullptr && blockIdx.x == 0 && warp == 0 && lane == 0;
-        long long pwf = 0, pws = 0, pinit = 0, pseg = 0, pst = 0; const long long pt0 = clock64();
-        pdl_wait();                                              // residual reads / output writes
-        for (int seq = 0;; ++seq) {
-            int tile = 0;
-            const long long ts0 = pon ? clock64() : 0;
-            if (lane == 0) tile = sched_next(bar_sched_full, bar_sched_empty, sched_ring, seq);
-            tile = __shfl_sync(0xffffffffu, tile, 0);
-            if (pon) pws += clock64() - ts0;
-            if (tile >= a.total_tiles) break;
-            pi = 0;
-            while (tile >= a.p[pi].tile_base + a.p[pi].tile_count) ++pi;
-            const Prob& P = a.p[pi];
-            const TileCoord tc = decode_tile(P, tile - P.tile_base);
-            const int NT = P.NT, ACC = P.ACC, S = P.S, nseg = P.nseg, relu = P.relu;
-            const int nconcat = EX < 0 ? P.nconcat : EX, big = EX == 1 ? 0 : P.big;
-            const int Cout = P.Cout, Wo = P.Wo, Ho = P.Ho;
-            const float* __restrict__ bias = P.bias;
-            const float* __restrict__ res_f = (!RESF || (PROF && (a.variant & 2))) ? nullptr : P.res_f;
-            const __half* __restrict__ res_hi = (PROF && (a.variant & 2)) ? nullptr : P.res_hi;
-            const __half* __restrict__ res_lo = P.res_lo;
+            if constexpr (!EX) init(m, true);
+            const float* v = EX ? sum : m;
+            // ReLU, split, store
+            const int relu = P.relu;
             float* __restrict__ y_f = P.y_f; __half* __restrict__ y_hi = P.y_hi; __half* __restrict__ y_lo = P.y_lo;
-            // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
-            // residual enter the accumulator times 2^s and the sum leaves it times 2^-s -- exact in fp32
-            const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
-            const int ngroups = NT >> 4;
-            const int gph = (ngroups - half + 1) >> 1;            // groups this warp owns per sub-tile
-            const int nunits = S * gph;
-            const int cw = Cout - tc.nt * NT;                     // channels of this N tile that exist (multiple of 8)
-            // this thread's output row: tile row prow of image tc.img, or (stacked small maps) row prow % hs of image
-            // tc.img * nstack + prow / hs -- rows hs-pad.. of a stacked image are the shared zero rows (no output)
-            int oh = tc.th * kTileH + prow, img = tc.img;
-            bool row_ok = oh < Ho;
-            if (P.nstack > 1) {
-                const int n = prow / P.hs;
-                oh = prow - n * P.hs; img = tc.img * P.nstack + n;
-                row_ok = oh < Ho && n < P.nstack && img < P.N;
-            }
-            const int boff = (img - mdiv(img, P.m_ws) * P.wsets) * Cout + tc.nt * NT;
-            const uint32_t rowbase = (uint32_t)(img * Ho + oh) * Wo;
-            const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16);
-            int cs_first = 0;
-            for (int u0 = 0; u0 < (nunits > 0 ? nunits : 1); u0 += 4) {
-                const long long ti0 = pon ? clock64() : 0;
-                float acc[4][16];
-                uint32_t eoff[4]; int cou[4]; bool okp[4];
 #pragma unroll
-                for (int uu = 0; uu < 4; ++uu) {
-                    const int u = u0 + uu;
-                    const int s = u / gph, grp = half + 2 * (u - s * gph);
-                    const int ow = (tc.tw * S + s) * kTileW + pcol;
-                    cou[uu] = grp * 16;
-                    okp[uu] = u < nunits && row_ok && ow < Wo;
-                    eoff[uu] = (rowbase + ow) * Cout + tc.nt * NT + grp * 16;
-                    // accumulator <- bias
+            for (int j = 0; j < NV / 4; ++j) {
+                if (j >= nj) break;
+                if (8 * j >= cw) continue;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int co = grp * 16 + 8 * h;
-                        const bool ch_ok = u < nunits && co < cw;
-                        float4 b0 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = b0;
-                        if (bias && ch_ok) { b0 = __ldg(reinterpret_cast<const float4*>(bias + boff + co)); b1 = __ldg(reinterpret_cast<const float4*>(bias + boff + co + 4)); }
-                        float* ac = &acc[uu][8 * h];
-                        ac[0] = b0.x; ac[1] = b0.y; ac[2] = b0.z; ac[3] = b0.w; ac[4] = b1.x; ac[5] = b1.y; ac[6] = b1.z; ac[7] = b1.w;
-                    }
-                }
-                // + residual: all the 16-byte loads of one plane are issued back to back (8 in flight per lane) before the
-                // first use -- one memory round trip per plane instead of one per load (measured: the per-load form cost
-                // 6K cycles per tile and made the MMA warp wait for accumulator stages)
-                if (res_f) {
-#pragma unroll
-                    for (int hp = 0; hp < 2; ++hp) {                  // two passes of 4 x 16 bytes per unit half
-                        float4 r[4][2];
-#pragma unroll
-                        for (int uu = 0; uu < 4; ++uu)
-#pragma unroll
-                            for (int k = 0; k < 2; ++k) {
-                                r[uu][k] = make_float4(0.f, 0.f, 0.f, 0.f);
-                                if (okp[uu] && cou[uu] + 8 * hp < cw) r[uu][k] = __ldg(reinterpret_cast<const float4*>(res_f + eoff[uu] + 8 * hp + 4 * k));
-                            }
-#pragma unroll
-                        for (int uu = 0; uu < 4; ++uu) {
-                            float* ac = &acc[uu][8 * hp];
-                            ac[0] += r[uu][0].x; ac[1] += r[uu][0].y; ac[2] += r[uu][0].z; ac[3] += r[uu][0].w;
-                            ac[4] += r[uu][1].x; ac[5] += r[uu][1].y; ac[6] += r[uu][1].z; ac[7] += r[uu][1].w;
-                        }
-                    }
-                } else if (res_hi) {
-#pragma unroll
-                    for (int pl = 0; pl < 2; ++pl) {
-                        const __half* __restrict__ rp = pl == 0 ? res_hi : res_lo;
-                        if (rp == nullptr) break;
-                        uint4 r[4][2];
-#pragma unroll
-                        for (int uu = 0; uu < 4; ++uu)
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                r[uu][h] = make_uint4(0u, 0u, 0u, 0u);
-                                if (okp[uu] && cou[uu] + 8 * h < cw) r[uu][h] = __ldg(reinterpret_cast<const uint4*>(rp + eoff[uu] + 8 * h));
-                            }
-#pragma unroll
-                        for (int uu = 0; uu < 4; ++uu)
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                float* ac = &acc[uu][8 * h];
-                                float2 t;
-                                t = h2_to_f2(r[uu][h].x); ac[0] += t.x; ac[1] += t.y; t = h2_to_f2(r[uu][h].y); ac[2] += t.x; ac[3] += t.y;
-                                t = h2_to_f2(r[uu][h].z); ac[4] += t.x; ac[5] += t.y; t = h2_to_f2(r[uu][h].w); ac[6] += t.x; ac[7] += t.y;
-                            }
-                    }
-                }
-#pragma unroll
-                for (int uu = 0; uu < 4; ++uu)
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) acc[uu][j] *= wsc.x;
-                if (pon) pinit += clock64() - ti0;
-                // add every K segment of the tile from TMEM (a multi-batch tile has a single segment)
-                for (int seg = 0; seg < nseg; ++seg) {
-                    const long long tg0 = pon ? clock64() : 0;
-                    long long wseg = 0;
-                    int cs = cs_first;
-                    if (u0 == 0) {
-                        cs = 0;
-                        if (!big) { cs = tog; tog ^= 1; }
-                        mbar_wait_t(bar_acc_full + 8 * cs, (fph >> cs) & 1u, pon, &wseg);
-                        fph ^= 1u << cs;
-                        tc_fence_after();
-                        cs_first = cs;
-                    }
-                    // TMEM -> registers two units at a time (32 temporaries), main range then small-term range
-                    const int nrange = nconcat ? 2 : 1;
-                    for (int rg = 0; rg < nrange; ++rg) {
-#pragma unroll
-                        for (int up = 0; up < 4; up += 2) {
-                            if (u0 + up >= nunits) break;
-                            float v[2][16];
-#pragma unroll
-                            for (int w2 = 0; w2 < 2; ++w2) {
-                                const int u = u0 + up + w2;
-                                if (u < nunits) {
-                                    const int s = u / gph, grp = half + 2 * (u - s * gph);
-                                    tc_ld32x32_x16_nowait(tlane + cs * 256 + s * ACC + rg * NT + grp * 16, v[w2]);
-                                }
-                            }
-                            tc_wait_ld();
-#pragma unroll
-                            for (int w2 = 0; w2 < 2; ++w2)
-                                if (u0 + up + w2 < nunits) {
-#pragma unroll
-                                    for (int j = 0; j < 16; ++j) acc[up + w2][j] += v[w2][j];
-                                }
-                        }
-                    }
-                    if (u0 + 4 >= nunits) {                      // last batch: the accumulator stage is free again
-                        tc_fence_before();
-                        if (big) { mbar_arrive(bar_acc_empty); mbar_arrive(bar_acc_empty + 8); }
-                        else mbar_arrive(bar_acc_empty + 8 * cs);
-                    }
-                    if (pon) { pwf += wseg; pseg += clock64() - tg0 - wseg; }
-                }
-                const long long tst0 = pon ? clock64() : 0;
-                // ReLU, split, store.  The fp32 view goes out in 256-bit stores (STG.E.ENL2.256, one full 32-byte sector per
-                // lane; channel offsets are multiples of 8 floats): measured 2x on the store phase of the SMPL blend-shape
-                // GEMM.  The fp16 planes stay with 16-byte stores: 256-bit stores were 10 % slower on the DRAM-write-bound
-                // 1x1 layers (tools/tc_layers.py, profiles/r02_epilogue_store_width.txt).
-#pragma unroll
-                for (int uu = 0; uu < 4; ++uu) {
-                    if (!(okp[uu] && do_store)) continue;
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (cou[uu] + 8 * h >= cw) continue;
-                        float* ac = &acc[uu][8 * h];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) ac[j] *= wsc.y;
-                        if (relu) {
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) ac[j] = fmaxf(ac[j], 0.f);
-                        }
-                        const uint32_t e = eoff[uu] + 8 * h;
-                        if (y_f) st_global_v8(y_f + e, ac);
-                        if (y_hi) {
-                            uint4 hv;
-                            hv.x = pack_h2_rn(ac[0], ac[1]); hv.y = pack_h2_rn(ac[2], ac[3]);
-                            hv.z = pack_h2_rn(ac[4], ac[5]); hv.w = pack_h2_rn(ac[6], ac[7]);
-                            *reinterpret_cast<uint4*>(y_hi + e) = hv;
-                            if (y_lo) {
-                                float2 t; uint4 lv;
-                                t = h2_to_f2(hv.x); lv.x = pack_h2_rn(ac[0] - t.x, ac[1] - t.y);
-                                t = h2_to_f2(hv.y); lv.y = pack_h2_rn(ac[2] - t.x, ac[3] - t.y);
-                                t = h2_to_f2(hv.z); lv.z = pack_h2_rn(ac[4] - t.x, ac[5] - t.y);
-                                t = h2_to_f2(hv.w); lv.w = pack_h2_rn(ac[6] - t.x, ac[7] - t.y);
-                                *reinterpret_cast<uint4*>(y_lo + e) = lv;
-                            }
+                for (int r = 0; r < 2; ++r) {
+                    if (!ok[r]) continue;
+                    float x0 = v[4 * j + 2 * r] * wsc.y, x1 = v[4 * j + 2 * r + 1] * wsc.y;
+                    if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                    const uint32_t e = eoff[r] + 8 * j;
+                    if (y_f) *reinterpret_cast<float2*>(y_f + e) = make_float2(x0, x1);
+                    if (y_hi) {
+                        const uint32_t hv = pack_h2_rn(x0, x1);
+                        *reinterpret_cast<uint32_t*>(y_hi + e) = hv;
+                        if (y_lo) {
+                            const float2 t = h2_to_f2(hv);
+                            *reinterpret_cast<uint32_t*>(y_lo + e) = pack_h2_rn(x0 - t.x, x1 - t.y);
                         }
                     }
                 }
-                if (pon) pst += clock64() - tst0;
             }
         }
-        if (pon) { a.prof[10] = clock64() - pt0; a.prof[11] = pwf; a.prof[12] = pws; a.prof[13] = pinit; a.prof[14] = pseg; a.prof[15] = pst; }
     }
-    tc_fence_before();
     __syncthreads();
     if (threadIdx.x == 0 && a.sched) {
         // the last CTA to finish re-arms the scheduler for the next launch (or graph replay) that uses this slot
         __threadfence();
         if (atomicAdd(a.sched + 1, 1u) == gridDim.x - 1) { a.sched[0] = 0u; a.sched[1] = 0u; __threadfence(); }
     }
-    if (warp == kWarpMma) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    }
 }
 
 // weight packing: SIMT layout [wsets][ks*ks*Cin][Cout] fp32 -> swizzled smem-image blocks of split fp16.
 // block (ws, nt, chunk, parity plane, tap group[, plane]) = [TG taps][rows][SWB bytes]; rows = output channels
-// (nconcat: NT hi rows then NT lo rows; wsplit: a hi block followed by a lo block)
+// (exact mode: NT hi rows then NT lo rows)
 __global__ void k_absmax(long long n, const float* __restrict__ w, unsigned* __restrict__ out) {
     unsigned m = 0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -893,7 +628,7 @@ __global__ void k_pack(const Prob g, const float* __restrict__ w, __half* __rest
     if (tt < g.TG) {
         const uint32_t r = loff - tt * g.tap_bytes;
         int n = r / g.SWB; const int kk = (r % g.SWB) / 2;
-        if (g.nconcat && n >= g.NT) { n -= g.NT; want_lo = 1; }
+        if (g.exact && n >= g.NT) { n -= g.NT; want_lo = 1; }
         int bi = (int)(blk % g.bpc); blk /= g.bpc;
         int slot = 0, base = 0;
         for (;;) { const int nb = g.ngrp[slot]; if (bi < base + nb || slot + 1 >= g.npa) break; base += nb; ++slot; }
@@ -970,34 +705,24 @@ static int encode_x(const Prob& g, const void* base, CUtensorMap* tm) {
 
 }  // namespace tc
 
-static long long* g_tc_prof = nullptr;
 static int g_sm_count[64];
 static unsigned* g_sched[64];              // per device: kSchedSlots x {tile counter, done counter}, zero-initialised, self-resetting
 static unsigned g_sched_seq[64];
 constexpr int kSchedSlots = 1024;
 static std::mutex g_tc_mu;
 static unsigned long long g_tc_devs = 0;
-static bool g_use_pdl = true;
 
-// geometry of every problem + the shared-memory rings of the launch (sub-tile pairs are given up, largest halo first,
-// until the rings fit)
+// geometry of every problem + the shared-memory rings of the launch
 static int configure_group(int n, const danet_conv_desc* const* descs, tc::ArgsN* a) {
     using namespace tc;
     DANET_CHECK(n >= 1 && n <= kMaxProb, "danet_conv_tc_group: 1..%d problems per launch (got %d)", kMaxProb, n);
     memset(a, 0, sizeof(*a));
     a->nprob = n;
-    int S_req[kMaxProb];
-    const int s_env = env_int("DANET_TC_S", 2);
-    for (int i = 0; i < n; ++i) S_req[i] = s_env;
-    for (int attempt = 0;; ++attempt) {
-        for (int i = 0; i < n; ++i)
-            if (!make_prob(descs[i], S_req[i], &a->p[i])) { set_error("danet_conv_tc_group: problem %d has an unsupported shape", i); return -1; }
-        if (plan_rings(a)) break;
-        int worst = -1, wb = 0;
-        for (int i = 0; i < n; ++i) if (a->p[i].S > 1 && max_stage_bytes(a->p[i]) > wb) { wb = max_stage_bytes(a->p[i]); worst = i; }
-        DANET_CHECK(worst >= 0 && attempt < 2 * kMaxProb, "danet_conv_tc_group: shared-memory plan does not fit");
-        S_req[worst] = 1;
-    }
+    for (int i = 0; i < n; ++i)
+        if (!make_prob(descs[i], &a->p[i])) { set_error("danet_conv_tc_group: problem %d has an unsupported shape", i); return -1; }
+    for (int i = 1; i < n; ++i)
+        DANET_CHECK(a->p[i].exact == a->p[0].exact, "danet_conv_tc_group: exact and fast problems cannot share a launch");
+    DANET_CHECK(plan_rings(a), "danet_conv_tc_group: shared-memory plan does not fit");
     return 0;
 }
 
@@ -1018,7 +743,7 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         const Prob& P = a.p[i];
         int taps = 0;
         for (int s2 = 0; s2 < P.npa; ++s2) taps += P.ntap[s2];
-        tcost[i] = (double)P.S * taps * ((P.Cin + 15) / 16) * (P.exact ? 2.0 : 1.0) * (128 + P.NT * (P.exact ? 1.5 : 1.0));
+        tcost[i] = (double)taps * ((P.Cin + 15) / 16) * (P.exact ? 2.0 : 1.0) * (128 + P.NT * (P.exact ? 1.5 : 1.0));
         order[i] = i;
     }
     for (int i = 1; i < n; ++i)
@@ -1045,8 +770,6 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         DANET_CHECK(base < (1 << 24), "danet_conv_tc_group: too many tiles");
     }
     a.total_tiles = base;
-    a.variant = env_int("DANET_TC_VARIANT", 0);
-    a.prof = g_tc_prof;
     int dev = 0;
     DANET_CUDA(cudaGetDevice(&dev));
     DANET_CHECK(dev >= 0 && dev < 64, "conv_tc: device ordinal %d out of range", dev);
@@ -1054,40 +777,27 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         std::lock_guard<std::mutex> lk(g_tc_mu);
         if (first_use_on_current_device(&g_tc_devs) != 0) {          // function attributes are per device
             DANET_CUDA(cudaDeviceGetAttribute(&g_sm_count[dev], cudaDevAttrMultiProcessorCount, dev));
-            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<false, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<false, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<false, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<false, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<true, -1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-            g_use_pdl = env_int("DANET_TC_PDL", 1) != 0;
+            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
             DANET_CUDA(cudaMalloc((void**)&g_sched[dev], kSchedSlots * 2 * sizeof(unsigned)));
             DANET_CUDA(cudaMemset(g_sched[dev], 0, kSchedSlots * 2 * sizeof(unsigned)));
         }
         // every launch takes the next counter pair (a CUDA graph keeps the one it captured: the kernel re-arms it)
-        a.sched = env_int("DANET_TC_DYNAMIC", 1) ? g_sched[dev] + 2 * (g_sched_seq[dev]++ % kSchedSlots) : nullptr;
+        a.sched = g_sched[dev] + 2 * (g_sched_seq[dev]++ % kSchedSlots);
     }
     const int smem_bytes = kSmemFixed + a.na_stages * a.a_slot_bytes + a.nb_stages * a.b_slot_bytes;
     const int cap = g_sm_count[dev];
     const int grid = a.total_tiles < cap ? a.total_tiles : cap;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem_bytes < 120 * 1024 ? 120 * 1024 : smem_bytes;      // one CTA per SM (TMEM: 512 columns each)
+    cfg.dynamicSmemBytes = smem_bytes;
     cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = g_use_pdl ? 1 : 0;
-    int n_exact = 0, n_big = 0, n_resf = 0;
-    for (int i = 0; i < a.nprob; ++i) { n_exact += a.p[i].exact; n_big += a.p[i].big; n_resf += a.p[i].res_f != nullptr; }
-    if (a.prof || a.variant || (n_exact != 0 && (n_exact != a.nprob || n_big != 0))) {
-        DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<true, -1, true>, a));      // instrumentation / knock-outs / mixed modes: the generic instantiation
-    } else if (n_exact) {
-        if (n_resf) { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<false, 1, true>, a)); }
-        else { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<false, 1, false>, a)); }
-    } else {
-        if (n_resf) { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<false, 0, true>, a)); }
-        else { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<false, 0, false>, a)); }
-    }
+    cfg.attrs = at; cfg.numAttrs = 1;
+    if (a.p[0].exact) { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<1>, a)); }
+    else { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<0>, a)); }
     DANET_LAUNCH_CHECK();
     return 0;
 }
@@ -1096,32 +806,25 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
 
 using namespace danet;
 
-// bring-up instrumentation: device buffer of 16 int64 written by CTA 0 of every following launch (NULL = off):
-// [0] A-producer total, [1] its a_empty waits; [2] B-producer total, [3] b_empty waits, [4] scheduler waits;
-// [5] MMA warp total, [6] a_full, [7] b_full, [8] acc_empty, [9] scheduler waits;
-// [10] epilogue warp 0 total, [11] acc_full waits, [12] scheduler waits, [13] bias/residual init, [14] TMEM segments, [15] stores
-extern "C" int danet_conv_tc_set_profile_buffer(void* dev_buf) { g_tc_prof = (long long*)dev_buf; return 0; }
-
 extern "C" int danet_conv_tc_supported(const danet_conv_desc* d) {
     tc::Prob g;
-    if (!d || !tc::make_prob(d, 2, &g)) return 0;
+    if (!d || !tc::make_prob(d, &g)) return 0;
     tc::ArgsN* a = new tc::ArgsN();
     a->nprob = 1; a->p[0] = g;
-    bool ok = tc::plan_rings(a);
-    if (!ok && tc::make_prob(d, 1, &g)) { a->p[0] = g; ok = tc::plan_rings(a); }
+    const bool ok = tc::plan_rings(a);
     delete a;
     return ok ? 1 : 0;
 }
 
 extern "C" int64_t danet_conv_tc_packed_bytes(const danet_conv_desc* d) {
     tc::Prob g;
-    if (!d || !tc::make_prob(d, 1, &g)) return 0;
+    if (!d || !tc::make_prob(d, &g)) return 0;
     return tc::kPackHeader + (int64_t)d->wsets * g.blocks_per_set * g.b_block_bytes;
 }
 
 extern "C" int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream) {
     tc::Prob g;
-    DANET_CHECK(d && tc::make_prob(d, 1, &g), "danet_conv_tc_pack: shape not supported by the tcgen05 path");
+    DANET_CHECK(d && tc::make_prob(d, &g), "danet_conv_tc_pack: shape not supported by the tensor-core path");
     DANET_CHECK(w_simt && w_packed, "danet_conv_tc_pack: null pointer");
     // power-of-two scale that brings the largest |w| into [2^13, 2^14): the lo halves (2^-11 of the value) of all but
     // the tiniest weights are then normal fp16 numbers and the split keeps its 22 bits
@@ -1130,7 +833,7 @@ extern "C" int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt,
     DANET_CUDA(cudaMalloc((void**)&d_max, 4));
     DANET_CUDA(cudaMemsetAsync(d_max, 0, 4, st));
     const long long nw = (long long)d->wsets * d->ksize * d->ksize * d->Cin * d->Cout;
-    tc::k_absmax<<<148, 256, 0, st>>>(nw, w_simt, d_max);
+    tc::k_absmax<<<132, 256, 0, st>>>(nw, w_simt, d_max);
     unsigned h_max = 0;
     DANET_CUDA(cudaMemcpyAsync(&h_max, d_max, 4, cudaMemcpyDeviceToHost, st));
     DANET_CUDA(cudaStreamSynchronize(st));
@@ -1157,7 +860,7 @@ extern "C" int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int
     tc::ArgsN* a = new tc::ArgsN();
     const int rc = configure_group(n, dp, a);
     if (rc == 0) {
-        for (int i = 0; i < n; ++i) subtiles[i] = a->p[i].S;
+        for (int i = 0; i < n; ++i) subtiles[i] = 1;
         stages[0] = a->na_stages; stages[1] = a->nb_stages;
     }
     delete a;

@@ -1,4 +1,4 @@
-// Fused SMPL layer for sm_100a: pose front-ends (rot-mat / axis-angle / rot6d), 24-joint
+// Fused SMPL layer for sm_90a: pose front-ends (rot-mat / axis-angle / rot6d), 24-joint
 // kinematic chain, blend shapes + pose correctives + linear blend skinning for 6890 vertices,
 // and the vertex-regressed joints (extra 9, H36M 17, 21 picked vertices) -> 49-joint output.
 //
@@ -7,9 +7,9 @@
 //  * small batches (B < kGemmMinB): everything fp32 SIMT in one fused kernel (below);
 //  * large batches: the blend-shape + pose-corrective contraction  v_posed[B, 20670] = template +
 //    [pose_feature | betas][B, 224] x [posedirs ; shapedirs][224, 20670]  is a genuine GEMM (4.5 MMAC per body,
-//    88 % of the layer's arithmetic) and runs on the tcgen05 engine of conv_tc.cu as a 1x1 "convolution" whose
+//    88 % of the layer's arithmetic) and runs on the wgmma engine of conv_tc.cu as a 1x1 "convolution" whose
 //    pixels are the bodies (exact mode: split-fp16 operands, 3 MMAs, fp32 accumulation -> fp32-grade), in chunks
-//    of kGemmChunk bodies so that the fp32 v_posed chunk (85 MB) stays in the 126 MB L2 until the skinning
+//    of kGemmChunk bodies so that the fp32 v_posed chunk (42 MB) stays in the 50 MB L2 until the skinning
 //    kernel (the same k_smpl_verts, phase 1 replaced by a coalesced load) has consumed it.
 // Fused SIMT route, three launches per forward:
 //   k_smpl_pose    one warp per body, lane = joint: rotations, rest joints (linear in beta, precomputed
@@ -33,7 +33,7 @@ constexpr int kPF = 208;                // padded pose-feature length (207 -> 20
 constexpr int kMaxBetas = 16;
 constexpr int kGF = 224;                // GEMM route: feature row = 207 pose features | 0 | betas (<= 16) at 208..
 constexpr int kGemmMinB = 512;          // batches at least this large take the tensor-core GEMM route
-constexpr int kGemmChunk = 1024;        // bodies per GEMM + skinning round (fp32 v_posed chunk = 85 MB, L2-resident)
+constexpr int kGemmChunk = 512;         // bodies per GEMM + skinning round (fp32 v_posed chunk = 42 MB, L2-resident)
 
 struct SmplView {
     int nv, ntiles, nvpad, npad, nbetas;
@@ -987,7 +987,7 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
     (void)G;
     DANET_LAUNCH_CHECK();
     int nb = bodies_per_cta;
-    if (nb <= 0) nb = B >= 32 ? 8 : (B >= 4 ? 4 : (B >= 2 ? 2 : 1));      // 8 is the measured optimum on B200 (tools/lbs_sweep.py)
+    if (nb <= 0) nb = B >= 32 ? 8 : (B >= 4 ? 4 : (B >= 2 ? 2 : 1));      // tools/lbs_sweep.py sweeps it
     const size_t smem = (size_t)nb * (kPF + kJ * 12 + kTileC + kMaxBetas) * sizeof(float);
 #define DANET_LBS_LAUNCH(NBV, Bc, off, VP)                                                          \
     do {                                                                                            \

@@ -183,7 +183,7 @@ extern "C" int danet_body_uv_losses(int32_t N, int32_t C, int32_t Cann, int32_t 
     const long long total = (long long)N * HW;
     DANET_CHECK((total + 63) / 64 < (1LL << 31), "body_uv_losses: too many pixels");
     // few pixels (the global heads of a 16-image batch: 50 K): smaller blocks, so that every SM gets several
-    const int bt = total >= 148LL * 2048 * 2 ? 256 : (total >= 148LL * 2048 / 2 ? 128 : 64);
+    const int bt = total >= 132LL * 2048 * 2 ? 256 : (total >= 132LL * 2048 / 2 ? 128 : 64);
     const int blocks = (int)((total + bt - 1) / bt);
     LossArgs a;
     a.N = N; a.C = C; a.Cann = Cann; a.HW = HW; a.pred_stride = pred_stride; a.map_stride = map_stride;

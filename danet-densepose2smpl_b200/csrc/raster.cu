@@ -1,4 +1,4 @@
-// IUV rasteriser for sm_100a.  Replaces utils/renderer.py:207-298 (IUV_Renderer.verts2uvimg /
+// IUV rasteriser for sm_90a.  Replaces utils/renderer.py:207-298 (IUV_Renderer.verts2uvimg /
 // camera_matrix) and the third-party neural_renderer forward pass behind it (projection,
 // vertices_to_faces, forward_face_index_map kernels, texture sampling, vertical flip), and
 // optionally fuses utils/iuvmap.py:103-151 (iuv_img2map) into the resolve pass.

@@ -97,7 +97,7 @@ class DaNet(nn.Module):
         if cfg:
             self.cfg.update(cfg)
         self.width = width or self.cfg["WIDTH"]
-        # conv_algo: 'auto' / 'tc' = tcgen05 tensor-core convolutions (sm_100a), 'simt' = fp32 FMA kernels (an
+        # conv_algo: 'auto' / 'tc' = wgmma tensor-core convolutions (sm_90a), 'simt' = fp32 FMA kernels (an
         # independent fp32 check path).  precision (tensor-core path): 'exact' = split-fp16 operands, three MMAs per
         # K step, fp32-grade results (the reference computes in fp32; this is the default and what parity is
         # stated for); 'fast' = single fp16 pass (~1e-3 on para), about twice the throughput.

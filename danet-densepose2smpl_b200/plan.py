@@ -67,8 +67,8 @@ class CudaOps(object):
         return c
 
     def tc_capable(self):
-        """The tcgen05 kernels are sm_100a code: compute capability 10.x only."""
-        return torch.cuda.get_device_capability(self.device)[0] == 10
+        """The wgmma kernels are sm_90a code: compute capability 9.0 only."""
+        return torch.cuda.get_device_capability(self.device) == (9, 0)
 
     def conv_tc_supported(self, d):
         return bool(self.lib.danet_conv_tc_supported(ctypes.byref(self._desc(d))))
@@ -283,7 +283,7 @@ class Plan(object):
         self.conv_algo, self.precision = conv_algo, precision
         self.tc = conv_algo == "tc"
         if self.tc and hasattr(self.ops, "tc_capable") and not self.ops.tc_capable():
-            raise RuntimeError("danet_b200: the tensor-core path is sm_100a code; device %s is not compute capability 10.x" % device)
+            raise RuntimeError("danet_b200: the tensor-core path is sm_90a code; device %s is not compute capability 9.0" % device)
         self.P = self.ops.planes(precision) if self.tc else 0          # fp16 planes per activation (0: fp32 buffers only)
         self.group_convs = group_convs and self.tc
         self.keep_all = keep_all                      # debugging: no buffer reuse, every intermediate stays readable

@@ -1,4 +1,4 @@
-/* libdanet_b200.so -- C ABI of the B200-native DaNet inference hot path.
+/* libdanet_b200.so -- C ABI of the H100-native DaNet inference hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  Every entry point replaces one piece of the
  * reference's Python/ATen path (file:line of the reference cited per function).  Conventions:
@@ -152,7 +152,7 @@ int danet_iuv_img2map(int32_t B, int32_t S, const float* img, float* maps_u, flo
  * every view that is present.
  * ------------------------------------------------------------------------------------------ */
 enum { DANET_CONV_SIMT = 0,            /* fp32 FMA implicit GEMM (independent fp32 check path)      */
-       DANET_CONV_TC = 1 };            /* tcgen05 tensor-core implicit GEMM (danet_conv_tc_group)   */
+       DANET_CONV_TC = 1 };            /* wgmma tensor-core implicit GEMM (danet_conv_tc_group)     */
 
 typedef struct {
     int32_t N, H, W, Cin;              /* input  [N,H,W,Cin]                                      */
@@ -198,13 +198,10 @@ int danet_conv_tc_group(int32_t n, const danet_conv_problem* problems, danet_str
  * member, so a host may use this to keep a dominant problem from losing its sub-tile pair to a small companion. */
 int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* subtiles, int32_t* stages);
 /* bytes / packing helper: converts the SIMT layout above into the swizzled shared-memory image blocks of
- * split-fp16 weights the tcgen05 kernel bulk-copies (device -> device, once at load). */
+ * split-fp16 weights the wgmma kernel bulk-copies (device -> device, once at load). */
 int64_t danet_conv_tc_packed_bytes(const danet_conv_desc* d);
 int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
 int danet_conv_tc_supported(const danet_conv_desc* d);
-/* bring-up instrumentation: 16 x int64 device buffer receiving per-role cycle counters of CTA 0 of
- * every following tensor-core launch (NULL = off; layout in csrc/conv_tc.cu) */
-int danet_conv_tc_set_profile_buffer(void* dev_buf);
 /* fp32 -> split-fp16 planes (lo may be NULL) and back (lo may be NULL); n elements */
 int danet_act_split(int64_t n, const float* x, void* hi, void* lo, danet_stream_t stream);
 int danet_act_merge(int64_t n, const void* hi, const void* lo, float* y, danet_stream_t stream);

@@ -53,7 +53,7 @@ def hostlib(tmp_path_factory):
         pytest.skip("nvcc not available")
     out = str(tmp_path_factory.mktemp("losses_host") / "liblosses_host.so")
     csrc = os.path.join(ROOT, "danet-densepose2smpl_b200", "csrc")
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O2", "-std=c++17", "-Xcompiler", "-fPIC",
+    subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "-Xcompiler", "-fPIC",
                            "-DDANET_LOSSES_HOST_CHECK", "-shared", os.path.join(csrc, "losses.cu"), os.path.join(csrc, "api.cu"),
                            "-o", out])
     lib = ctypes.CDLL(out)

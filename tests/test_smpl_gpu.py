@@ -41,7 +41,7 @@ def test_smpl_axis_angle(smpl_model, B):
 
 @pytest.mark.parametrize("B", [517, 1100])
 def test_smpl_large_batch_tensor_core_route(smpl_model, B):
-    """B >= 512: the blend-shape + pose-corrective contraction runs as a split-fp16 exact-mode GEMM on the tcgen05
+    """B >= 512: the blend-shape + pose-corrective contraction runs as a split-fp16 exact-mode GEMM on the wgmma
     engine (chunks of 1024 bodies; 517 / 1100 are ragged against the 8-body rows, the 128-row tiles and the chunk),
     followed by the skinning phases.  Same 1e-4 bar; bodies_per_cta = -1 forces the fused fp32 kernel for comparison."""
     import danet_b200

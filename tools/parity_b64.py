@@ -15,4 +15,4 @@ dev = torch.device("cuda:0")
 net = danet_b200.build_synthetic_danet(width=48, seed=0, device=dev, conv_algo=algo, precision=prec)
 p = bench.parity_block(net, dev, 48, 64)
 p.pop("note", None)
-print(algo, prec, "LSEG=%s" % os.environ.get("DANET_TC_LSEG", "default"), json.dumps(p))
+print(algo, prec, json.dumps(p))
