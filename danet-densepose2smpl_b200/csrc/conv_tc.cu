@@ -21,9 +21,11 @@
 //       (N tile, channel chunk, parity plane, tap group[, hi/lo]) block; streamed with 1-D cp.async.bulk.
 //   MMA: two consumer warpgroups, each owning 64 of the tile's 128 output pixels (8 image rows x 8 columns), issue
 //       wgmma.mma_async m64nNk16 (N = the tile's output channels) with fp32 accumulators in registers.
-//       exact mode: the hi and lo weight rows are concatenated along N, so hi*[hi|lo] is ONE MMA of width 2N whose
-//       second half lands in a separate small-term accumulator; lo*hi joins the small terms.  Per weight block all
-//       hi*[hi|lo] MMAs are issued first, then all lo*hi MMAs (two same-shape chains).
+//       exact mode: the lo and hi weight rows are concatenated along N, so hi*[lo|hi] is ONE MMA of width 2N whose
+//       first half lands in a separate small-term accumulator; lo*hi joins the small terms.  Per weight block all
+//       hi*[lo|hi] MMAs are issued first, then all lo*hi MMAs (two same-shape chains).
+//       Every MMA has a compile-time width (one tile body per N tile width); a warpgroup commits one group per
+//       weight block and waits only for the block before it, so the MMAs of consecutive blocks stay in flight.
 //   K segments (exact mode): the tensor core's fp32 accumulation truncates, which biases long chains; after every
 //       lseg main-chain MMAs the accumulators are added in fp32 round-to-nearest to a running sum that starts at
 //       bias + residual.
@@ -208,6 +210,11 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// arrive only where pred holds, as one predicated instruction: an `if (leader)` branch between wgmmas looks divergent
+// to ptxas, which then serialises them
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar), "r"((uint32_t)pred) : "memory");
+}
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -281,41 +288,253 @@ __device__ __forceinline__ TileCoord decode_tile(const Prob& g, int t) {
     return c;
 }
 
-// One MMA of runtime width n (a multiple of 16, <= NMAX): accumulator columns [0, n/2) in lo, [n/2, n) in hi.
-template <int NMAX>
-__device__ __forceinline__ void mma_n(int n, float* lo, float* hi, uint64_t a, uint64_t b, uint32_t acc) {
-#define DANET_WG_CASE(N) case N: if (N <= NMAX) Wgmma<(N <= NMAX ? N : 16)>::mma(lo, hi, a, b, acc); break;
-    switch (n) {
-        DANET_WG_CASE(16) DANET_WG_CASE(32) DANET_WG_CASE(48) DANET_WG_CASE(64) DANET_WG_CASE(80) DANET_WG_CASE(96)
-        DANET_WG_CASE(112) DANET_WG_CASE(128) DANET_WG_CASE(144) DANET_WG_CASE(160) DANET_WG_CASE(176) DANET_WG_CASE(192)
-        DANET_WG_CASE(208) DANET_WG_CASE(224) DANET_WG_CASE(240) DANET_WG_CASE(256)
-        default: break;
+// Consumer-side wait: inlined, so that no call sits between wgmmas in flight (a call makes ptxas serialise them).
+// Still bounded: traps instead of hanging.
+__device__ __forceinline__ void mbar_wait_inl(uint32_t bar, uint32_t parity) {
+    uint32_t done = 0;
+#pragma unroll 1
+    for (uint32_t it = 0; it < (1u << 22); ++it) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+        if (done) return;
     }
-#undef DANET_WG_CASE
+    __trap();
 }
-// the plain accumulator of width n: registers d[0, n/2) (the column split point moves with n)
-template <int NMAX>
-__device__ __forceinline__ void mma_plain(int n, float* d, uint64_t a, uint64_t b, uint32_t acc) {
-#define DANET_WG_CASE(N) case N: if (N <= NMAX) Wgmma<(N <= NMAX ? N : 16)>::mma(d, d + (N <= NMAX ? N : 16) / 4, a, b, acc); break;
-    switch (n) {
-        DANET_WG_CASE(16) DANET_WG_CASE(32) DANET_WG_CASE(48) DANET_WG_CASE(64) DANET_WG_CASE(80) DANET_WG_CASE(96)
-        DANET_WG_CASE(112) DANET_WG_CASE(128) DANET_WG_CASE(144) DANET_WG_CASE(160) DANET_WG_CASE(176) DANET_WG_CASE(192)
-        DANET_WG_CASE(208) DANET_WG_CASE(224) DANET_WG_CASE(240) DANET_WG_CASE(256)
-        default: break;
+__device__ __forceinline__ void wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+// ring positions of one consumer warpgroup (every consumer walks the A and B rings in the producer's order)
+struct Ring { int as, bs; uint32_t aph, bph; };
+// shared-memory addresses of the rings and their barriers
+struct Smem { uint32_t sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty; };
+
+// ---------------------------------------------------------------------------------------------
+// one consumer warpgroup's share of one tile, at a compile-time N tile width
+// ---------------------------------------------------------------------------------------------
+// EX: exact (1) or fast (0).  NT: the problem's N tile width (P.NT).  Every wgmma has a fixed width and a fixed
+// accumulator set, so ptxas keeps them in flight: one commit group per weight block, and the warpgroup waits only
+// for the block before it (wait_group 1) -- that block's B slot (and its A slots at the end of a parity plane) is
+// freed once the next block's MMAs are issued.  An exact-mode K segment close drains the chain (wait_group 0).
+template <int EX, int NT>
+__device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, const TileCoord tc, const Smem S, Ring& R,
+                                             int wg, int w4, int lane, bool leader, float* accs, float* sum) {
+    constexpr int NV = NT / 2;            // fp32 accumulator registers per thread and set (64 x NT warpgroup tile)
+    constexpr int nj = NT / 8;            // 8-channel groups of the tile
+    // accumulator fragment of m64nNk16: this thread owns tile rows prow0, prow0 + 1 at column pcol, and channels
+    // 8 j + cq, 8 j + cq + 1 of every 8-channel group j (registers 4 j + 2 r + {0, 1} for row prow0 + r)
+    const int prow0 = 8 * wg + 2 * w4, pcol = lane >> 2, cq = 2 * (lane & 3);
+    float* s = accs;                      // exact: small terms hi*lo + lo*hi
+    float* m = EX ? accs + NV : accs;     // main accumulator (fast mode: the only one)
+    const int Cout = P.Cout, Wo = P.Wo, Ho = P.Ho;
+    const int cw = Cout - tc.nt * NT;     // channels of this N tile that exist (multiple of 8)
+    // this thread's two output pixels: tile row prow of image tc.img, or (stacked small maps) row prow % hs of image
+    // tc.img * nstack + prow / hs -- rows hs-pad.. of a stacked image are the shared zero rows (no output)
+    uint32_t eoff[2]; int boff[2]; bool ok[2];
+    const int ow = tc.tw * kTileW + pcol;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int prow = prow0 + r;
+        int oh = tc.th * kTileH + prow, img = tc.img;
+        bool row_ok = oh < Ho;
+        if (P.nstack > 1) {
+            const int n = prow / P.hs;
+            oh = prow - n * P.hs; img = tc.img * P.nstack + n;
+            row_ok = oh < Ho && n < P.nstack && img < P.N;
+        }
+        ok[r] = row_ok && ow < Wo;
+        eoff[r] = ((uint32_t)(img * Ho + oh) * Wo + ow) * Cout + tc.nt * NT + cq;
+        boff[r] = (img - mdiv(img, P.m_ws) * P.wsets) * Cout + tc.nt * NT + cq;
     }
-#undef DANET_WG_CASE
+    // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
+    // residual enter the sum times 2^s and the result leaves it times 2^-s -- exact in fp32
+    const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
+    // bias + residual of this thread's outputs (channel group j, row r); they enter the sum times 2^s
+    auto init_term = [&](int j, int r) {
+        float2 t = make_float2(0.f, 0.f);
+        if (8 * j < cw) {
+            if (P.bias) t = __ldg(reinterpret_cast<const float2*>(P.bias + boff[r] + 8 * j));
+            if (ok[r]) {
+                if (P.res_f) {
+                    const float2 q = __ldg(reinterpret_cast<const float2*>(P.res_f + eoff[r] + 8 * j));
+                    t.x += q.x; t.y += q.y;
+                } else if (P.res_hi) {
+                    const float2 q = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_hi + eoff[r] + 8 * j)));
+                    t.x += q.x; t.y += q.y;
+                    if (P.res_lo) {
+                        const float2 q2 = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_lo + eoff[r] + 8 * j)));
+                        t.x += q2.x; t.y += q2.y;
+                    }
+                }
+            }
+        }
+        return t;
+    };
+    if constexpr (EX) {                   // the exact mode's running sum starts at bias + residual
+#pragma unroll
+        for (int j = 0; j < nj; ++j)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const float2 t = init_term(j, r);
+                sum[4 * j + 2 * r] = t.x * wsc.x; sum[4 * j + 2 * r + 1] = t.y * wsc.x;
+            }
+    }
+    const int nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
+    const int kmma = P.KCH / 16;                          // K = 16 halves (32 bytes) per MMA
+    const uint32_t tap16 = P.tap_bytes >> 4;
+    const uint32_t hi16 = EX ? (NT * SWB) >> 4 : 0;       // exact: the hi weight rows follow the NT lo rows
+    const uint64_t bd0 = make_desc(0, 8 * SWB, SWB);
+    uint32_t acc = 0;
+    int seg_cnt = 0;
+    // ring slots whose MMAs may still be in flight: freed once a later wait covers them (-1: none)
+    int pend_b = -1, pend_ahi = -1, pend_alo = -1;
+    auto release_pending = [&]() {
+        mbar_arrive_if(S.bar_b_empty + 8 * pend_b, leader && pend_b >= 0);
+        mbar_arrive_if(S.bar_a_empty + 8 * pend_ahi, leader && pend_ahi >= 0);
+        if (EX) mbar_arrive_if(S.bar_a_empty + 8 * pend_alo, leader && pend_alo >= 0);
+        pend_b = pend_ahi = pend_alo = -1;
+    };
+    for (int c = 0; c < nchunks; ++c) {
+        const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
+        const int kv = kreal < kmma ? kreal : kmma;       // K steps wholly beyond Cin are not issued
+        for (int slot = 0; slot < npa; ++slot) {
+            const int as_hi = R.as;
+            mbar_wait_inl(S.bar_a_full + 8 * R.as, (R.aph >> R.as) & 1u);
+            R.aph ^= 1u << R.as; if (++R.as == a.na_stages) R.as = 0;
+            int as_lo = as_hi;
+            if (EX) {
+                as_lo = R.as;
+                mbar_wait_inl(S.bar_a_full + 8 * R.as, (R.aph >> R.as) & 1u);
+                R.aph ^= 1u << R.as; if (++R.as == a.na_stages) R.as = 0;
+            }
+            // this warpgroup's 8 tile rows start 8 halo rows further down for the second warpgroup
+            const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB) + ((uint32_t)(wg * 8 * P.sbo_a[slot]) >> 4);
+            const uint64_t ad_hi = ad0 + ((S.sA + as_hi * a.a_slot_bytes) >> 4);
+            const uint64_t ad_lo = ad0 + ((S.sA + as_lo * a.a_slot_bytes) >> 4);
+            const int ngrp = P.ngrp[slot], ntap = P.ntap[slot];
+            for (int tg = 0; tg < ngrp; ++tg) {
+                const int k0 = tg * TG;
+                const int ntk = min(TG, ntap - k0);
+                const int bs = R.bs;
+                mbar_wait_inl(S.bar_b_full + 8 * bs, (R.bph >> bs) & 1u);
+                R.bph ^= 1u << bs; if (++R.bs == a.nb_stages) R.bs = 0;
+                const uint64_t bd = bd0 + ((S.sB + bs * a.b_slot_bytes) >> 4);
+                wg_fence();
+                if constexpr (EX) {
+                    // hi * [lo | hi]: small terms in s, main chain in m; then lo * hi into s.  The instruction's
+                    // accumulator is (s, m) in that order: ptxas keeps the wgmmas in flight only if the lo * hi
+                    // accumulator s is the start of the wide one, not its second half.
+                    #pragma unroll 1
+                    for (int tt = 0; tt < ntk; ++tt) {
+                        const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
+                        #pragma unroll
+                        for (int kk = 0; kk < 4; ++kk) {
+                            if (kk >= kv) break;
+                            Wgmma<2 * NT>::mma(s, m, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
+                            acc = 1;
+                        }
+                    }
+                    #pragma unroll 1
+                    for (int tt = 0; tt < ntk; ++tt) {
+                        const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
+                        #pragma unroll
+                        for (int kk = 0; kk < 4; ++kk) {
+                            if (kk >= kv) break;
+                            Wgmma<NT>::mma(s, s + NT / 4, ad_lo + toff + 2 * kk, bd + hi16 + tt * tap16 + 2 * kk, 1u);
+                        }
+                    }
+                } else {
+                    #pragma unroll 1
+                    for (int tt = 0; tt < ntk; ++tt) {
+                        const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
+                        #pragma unroll
+                        for (int kk = 0; kk < 4; ++kk) {
+                            if (kk >= kv) break;
+                            Wgmma<NT>::mma(m, m + NT / 4, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
+                            acc = 1;
+                        }
+                    }
+                }
+                wg_commit();
+                const bool plane_end = tg == ngrp - 1;
+                bool close = false;
+                if constexpr (EX) {
+                    seg_cnt += ntk * kv;
+                    close = (c == nchunks - 1 && slot == npa - 1 && plane_end) || seg_cnt >= P.lseg;
+                }
+                if (close) {
+                    // close the K segment: the whole chain must have landed
+                    wg_wait_all();
+                    reg_fence<NV>(m);
+                    if constexpr (EX) {
+                        reg_fence<NV>(s);
+#pragma unroll
+                        for (int j = 0; j < NV; ++j) {
+                            sum[j] += m[j];
+                            sum[j] += s[j];
+                        }
+                    }
+                    acc = 0; seg_cnt = 0;
+                    release_pending();
+                    mbar_arrive_if(S.bar_b_empty + 8 * bs, leader);
+                    mbar_arrive_if(S.bar_a_empty + 8 * as_hi, leader && plane_end);
+                    if (EX) mbar_arrive_if(S.bar_a_empty + 8 * as_lo, leader && plane_end);
+                } else {
+                    // the block before this one is done: free its slots, keep this one's until the next wait
+                    wg_wait_1();
+                    release_pending();
+                    pend_b = bs;
+                    if (plane_end) { pend_ahi = as_hi; pend_alo = as_lo; }
+                }
+            }
+        }
+    }
+    // exact mode closed its last segment (drained) already; the wait tells ptxas that no MMA is in flight past here
+    wg_wait_all();
+    reg_fence<NV>(m);
+    if constexpr (EX) reg_fence<NV>(s);
+    release_pending();
+    // ReLU, split, store (fast mode adds bias + residual here, to the finished accumulator)
+    const int relu = P.relu;
+    float* __restrict__ y_f = P.y_f; __half* __restrict__ y_hi = P.y_hi; __half* __restrict__ y_lo = P.y_lo;
+#pragma unroll
+    for (int j = 0; j < nj; ++j) {
+        if (8 * j >= cw) continue;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (!ok[r]) continue;
+            float v0, v1;
+            if constexpr (EX) { v0 = sum[4 * j + 2 * r]; v1 = sum[4 * j + 2 * r + 1]; }
+            else {
+                const float2 t = init_term(j, r);
+                v0 = m[4 * j + 2 * r]; v1 = m[4 * j + 2 * r + 1];
+                v0 += t.x * wsc.x; v1 += t.y * wsc.x;
+            }
+            float x0 = v0 * wsc.y, x1 = v1 * wsc.y;
+            if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+            const uint32_t e = eoff[r] + 8 * j;
+            if (y_f) *reinterpret_cast<float2*>(y_f + e) = make_float2(x0, x1);
+            if (y_hi) {
+                const uint32_t hv = pack_h2_rn(x0, x1);
+                *reinterpret_cast<uint32_t*>(y_hi + e) = hv;
+                if (y_lo) {
+                    const float2 t = h2_to_f2(hv);
+                    *reinterpret_cast<uint32_t*>(y_lo + e) = pack_h2_rn(x0 - t.x, x1 - t.y);
+                }
+            }
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
 // EX: precision mode fixed at compile time (1: every problem of the launch is exact, 0: every problem is fast).
-// NV: fp32 accumulator registers per thread and array (a 64 x NT warpgroup tile holds NT / 2 per thread).
 template <int EX>
 __global__ void __launch_bounds__(kThreads, 1)
 k_conv_tc(const __grid_constant__ ArgsN a) {
     constexpr int NTMAX = EX ? kNtMaxExact : kNtMaxFast;
-    constexpr int NV = NTMAX / 2;
     extern __shared__ __align__(1024) uint8_t smem[];
     const uint32_t sbase = (smem_u32(smem) + 1023u) & ~1023u;          // swizzle atoms need 1024-byte alignment
     const uint32_t sA = sbase;
@@ -328,7 +547,9 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
     // global atomic counter, heaviest problems first) and read by the consumer warps
     const uint32_t bar_sched_full = sBar + 512, bar_sched_empty = sBar + 512 + 8 * kSchedDepth, sched_ring = sBar + 512 + 16 * kSchedDepth;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    // the warp index through a shuffle: ptxas then knows it is warp-uniform, and so is every branch on the warp role
+    // (a role branch it cannot prove uniform makes it serialise the wgmmas behind it)
+    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int i = 0; i < a.na_stages; ++i) { mbar_init(bar_a_full + 8 * i, 1); mbar_init(bar_a_empty + 8 * i, kConsumers); }
         for (int i = 0; i < a.nb_stages; ++i) { mbar_init(bar_b_full + 8 * i, 1); mbar_init(bar_b_empty + 8 * i, kConsumers); }
@@ -403,13 +624,11 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
         // ================= consumer warpgroups: wgmma main loop + epilogue =================
         const int wg = warp >> 2, w4 = warp & 3;
         const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
-        // accumulator fragment of m64nNk16: this thread owns tile rows prow0, prow0 + 1 at column pcol, and channels
-        // 8 j + cq, 8 j + cq + 1 of every 8-channel group j (registers 4 j + 2 r + {0, 1} for row prow0 + r)
-        const int prow0 = 8 * wg + 2 * w4, pcol = lane >> 2, cq = 2 * (lane & 3);
-        float m[NV];                      // main accumulator (fast mode: the only one)
-        float s[EX ? NV : 1];             // exact: small terms hi*lo + lo*hi
-        float sum[EX ? NV : 1];           // exact: bias + residual + every closed K segment, fp32 round-to-nearest
-        int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
+        const Smem S = {sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty};
+        Ring R = {0, 0, 0u, 0u};
+        constexpr int NVMAX = NTMAX / 2;
+        float accs[EX ? 2 * NVMAX : NVMAX];    // exact: small terms then main chain; fast: the main chain
+        float sum[EX ? NVMAX : 1];             // exact: bias + residual + every closed K segment, fp32 round-to-nearest
         pdl_wait();                                              // residual reads / output writes
         for (int seq = 0;; ++seq) {
             int tile = 0;
@@ -420,172 +639,23 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
             while (tile >= a.p[pi].tile_base + a.p[pi].tile_count) ++pi;
             const Prob& P = a.p[pi];
             const TileCoord tc = decode_tile(P, tile - P.tile_base);
-            const int NT = P.NT, Cout = P.Cout, Wo = P.Wo, Ho = P.Ho;
-            const int nj = NT >> 3;                               // 8-channel groups of the tile
-            const int cw = Cout - tc.nt * NT;                     // channels of this N tile that exist (multiple of 8)
-            // this thread's two output pixels: tile row prow of image tc.img, or (stacked small maps) row prow % hs of image
-            // tc.img * nstack + prow / hs -- rows hs-pad.. of a stacked image are the shared zero rows (no output)
-            uint32_t eoff[2]; int boff[2]; bool ok[2];
-            const int ow = tc.tw * kTileW + pcol;
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const int prow = prow0 + r;
-                int oh = tc.th * kTileH + prow, img = tc.img;
-                bool row_ok = oh < Ho;
-                if (P.nstack > 1) {
-                    const int n = prow / P.hs;
-                    oh = prow - n * P.hs; img = tc.img * P.nstack + n;
-                    row_ok = oh < Ho && n < P.nstack && img < P.N;
+            // one tile body per N tile width make_prob can produce; every body uses a prefix of the same accumulator
+            // arrays, so the widths share their registers
+#define DANET_NT_CASE(N) case N: consume_tile<EX, N>(a, P, tc, S, R, wg, w4, lane, leader, accs, sum); break;
+            if constexpr (EX) {
+                switch (P.NT) {
+                    DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64)
+                    default: __trap();
                 }
-                ok[r] = row_ok && ow < Wo;
-                eoff[r] = ((uint32_t)(img * Ho + oh) * Wo + ow) * Cout + tc.nt * NT + cq;
-                boff[r] = (img - mdiv(img, P.m_ws) * P.wsets) * Cout + tc.nt * NT + cq;
-            }
-            // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
-            // residual enter the sum times 2^s and the result leaves it times 2^-s -- exact in fp32
-            const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
-            // bias + residual of this thread's outputs, times 2^s, into v (the exact mode's running sum starts there;
-            // fast mode adds it to the accumulator after the main loop)
-            auto init = [&](float* v, bool add) {
-#pragma unroll
-                for (int j = 0; j < NV / 4; ++j) {
-                    if (j >= nj) break;
-#pragma unroll
-                    for (int r = 0; r < 2; ++r) {
-                        float2 t = make_float2(0.f, 0.f);
-                        if (8 * j < cw) {
-                            if (P.bias) t = __ldg(reinterpret_cast<const float2*>(P.bias + boff[r] + 8 * j));
-                            if (ok[r]) {
-                                if (P.res_f) {
-                                    const float2 q = __ldg(reinterpret_cast<const float2*>(P.res_f + eoff[r] + 8 * j));
-                                    t.x += q.x; t.y += q.y;
-                                } else if (P.res_hi) {
-                                    const float2 q = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_hi + eoff[r] + 8 * j)));
-                                    t.x += q.x; t.y += q.y;
-                                    if (P.res_lo) {
-                                        const float2 q2 = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_lo + eoff[r] + 8 * j)));
-                                        t.x += q2.x; t.y += q2.y;
-                                    }
-                                }
-                            }
-                        }
-                        if (add) { v[4 * j + 2 * r] += t.x * wsc.x; v[4 * j + 2 * r + 1] += t.y * wsc.x; }
-                        else { v[4 * j + 2 * r] = t.x * wsc.x; v[4 * j + 2 * r + 1] = t.y * wsc.x; }
-                    }
-                }
-            };
-            if constexpr (EX) init(sum, false);
-            const int nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
-            const int kmma = P.KCH / 16;                          // K = 16 halves (32 bytes) per MMA
-            const uint32_t tap16 = P.tap_bytes >> 4;
-            const uint64_t bd0 = make_desc(0, 8 * SWB, SWB);
-            uint32_t acc = 0;
-            int seg_cnt = 0;
-            for (int c = 0; c < nchunks; ++c) {
-                const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
-                const int kv = kreal < kmma ? kreal : kmma;       // K steps wholly beyond Cin are not issued
-                for (int slot = 0; slot < npa; ++slot) {
-                    const int as_hi = as;
-                    mbar_wait(bar_a_full + 8 * as, (aph >> as) & 1u);
-                    aph ^= 1u << as; if (++as == a.na_stages) as = 0;
-                    int as_lo = as_hi;
-                    if (EX) {
-                        as_lo = as;
-                        mbar_wait(bar_a_full + 8 * as, (aph >> as) & 1u);
-                        aph ^= 1u << as; if (++as == a.na_stages) as = 0;
-                    }
-                    // this warpgroup's 8 tile rows start 8 halo rows further down for the second warpgroup
-                    const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB) + ((uint32_t)(wg * 8 * P.sbo_a[slot]) >> 4);
-                    const uint64_t ad_hi = ad0 + ((sA + as_hi * a.a_slot_bytes) >> 4);
-                    const uint64_t ad_lo = ad0 + ((sA + as_lo * a.a_slot_bytes) >> 4);
-                    const int ngrp = P.ngrp[slot], ntap = P.ntap[slot];
-                    for (int tg = 0; tg < ngrp; ++tg) {
-                        const int k0 = tg * TG;
-                        const int ntk = min(TG, ntap - k0);
-                        mbar_wait(bar_b_full + 8 * bs, (bph >> bs) & 1u);
-                        const uint64_t bd = bd0 + ((sB + bs * a.b_slot_bytes) >> 4);
-                        wg_fence();
-                        if constexpr (EX) {
-                            // hi * [hi | lo]: main chain in m, small terms in s; then lo * hi into s
-                            #pragma unroll 1
-                            for (int tt = 0; tt < ntk; ++tt) {
-                                const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                                #pragma unroll 1
-                                for (int kk = 0; kk < kv; ++kk) {
-                                    mma_n<2 * NTMAX>(2 * NT, m, s, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
-                                    acc = 1;
-                                }
-                            }
-                            #pragma unroll 1
-                            for (int tt = 0; tt < ntk; ++tt) {
-                                const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                                #pragma unroll 1
-                                for (int kk = 0; kk < kv; ++kk)
-                                    mma_plain<NTMAX>(NT, s, ad_lo + toff + 2 * kk, bd + tt * tap16 + 2 * kk, 1u);
-                            }
-                        } else {
-                            #pragma unroll 1
-                            for (int tt = 0; tt < ntk; ++tt) {
-                                const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                                #pragma unroll 1
-                                for (int kk = 0; kk < kv; ++kk) {
-                                    mma_plain<NTMAX>(NT, m, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
-                                    acc = 1;
-                                }
-                            }
-                        }
-                        wg_commit();
-                        wg_wait_all();
-                        reg_fence<NV>(m);
-                        if (leader) mbar_arrive(bar_b_empty + 8 * bs);
-                        bph ^= 1u << bs; if (++bs == a.nb_stages) bs = 0;
-                        if constexpr (EX) {
-                            reg_fence<NV>(s);
-                            seg_cnt += ntk * kv;
-                            const bool last = c == nchunks - 1 && slot == npa - 1 && tg == ngrp - 1;
-                            if (last || seg_cnt >= P.lseg) {              // close the K segment
-#pragma unroll
-                                for (int j = 0; j < NV; ++j) {
-                                    if (j >= 4 * nj) break;
-                                    sum[j] += m[j];
-                                    sum[j] += s[j];
-                                }
-                                acc = 0; seg_cnt = 0;
-                            }
-                        }
-                    }
-                    if (leader) {
-                        mbar_arrive(bar_a_empty + 8 * as_hi);
-                        if (EX) mbar_arrive(bar_a_empty + 8 * as_lo);
-                    }
+            } else {
+                switch (P.NT) {
+                    DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64) DANET_NT_CASE(80) DANET_NT_CASE(96)
+                    DANET_NT_CASE(112) DANET_NT_CASE(128) DANET_NT_CASE(144) DANET_NT_CASE(160) DANET_NT_CASE(176) DANET_NT_CASE(192)
+                    DANET_NT_CASE(208) DANET_NT_CASE(224) DANET_NT_CASE(240) DANET_NT_CASE(256)
+                    default: __trap();
                 }
             }
-            if constexpr (!EX) init(m, true);
-            const float* v = EX ? sum : m;
-            // ReLU, split, store
-            const int relu = P.relu;
-            float* __restrict__ y_f = P.y_f; __half* __restrict__ y_hi = P.y_hi; __half* __restrict__ y_lo = P.y_lo;
-#pragma unroll
-            for (int j = 0; j < NV / 4; ++j) {
-                if (j >= nj) break;
-                if (8 * j >= cw) continue;
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    if (!ok[r]) continue;
-                    float x0 = v[4 * j + 2 * r] * wsc.y, x1 = v[4 * j + 2 * r + 1] * wsc.y;
-                    if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                    const uint32_t e = eoff[r] + 8 * j;
-                    if (y_f) *reinterpret_cast<float2*>(y_f + e) = make_float2(x0, x1);
-                    if (y_hi) {
-                        const uint32_t hv = pack_h2_rn(x0, x1);
-                        *reinterpret_cast<uint32_t*>(y_hi + e) = hv;
-                        if (y_lo) {
-                            const float2 t = h2_to_f2(hv);
-                            *reinterpret_cast<uint32_t*>(y_lo + e) = pack_h2_rn(x0 - t.x, x1 - t.y);
-                        }
-                    }
-                }
-            }
+#undef DANET_NT_CASE
         }
     }
     __syncthreads();
@@ -598,7 +668,7 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
 
 // weight packing: SIMT layout [wsets][ks*ks*Cin][Cout] fp32 -> swizzled smem-image blocks of split fp16.
 // block (ws, nt, chunk, parity plane, tap group[, plane]) = [TG taps][rows][SWB bytes]; rows = output channels
-// (exact mode: NT hi rows then NT lo rows)
+// (exact mode: NT lo rows then NT hi rows)
 __global__ void k_absmax(long long n, const float* __restrict__ w, unsigned* __restrict__ out) {
     unsigned m = 0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -628,7 +698,7 @@ __global__ void k_pack(const Prob g, const float* __restrict__ w, __half* __rest
     if (tt < g.TG) {
         const uint32_t r = loff - tt * g.tap_bytes;
         int n = r / g.SWB; const int kk = (r % g.SWB) / 2;
-        if (g.exact && n >= g.NT) { n -= g.NT; want_lo = 1; }
+        if (g.exact) { if (n < g.NT) want_lo = 1; else n -= g.NT; }
         int bi = (int)(blk % g.bpc); blk /= g.bpc;
         int slot = 0, base = 0;
         for (;;) { const int nb = g.ngrp[slot]; if (bi < base + nb || slot + 1 >= g.npa) break; base += nb; ++slot; }
