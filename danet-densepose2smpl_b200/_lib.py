@@ -48,6 +48,18 @@ class GcnParams(ctypes.Structure):
                 ("head_w", c_p), ("head_b", c_p), ("mean_pose", c_p)]
 
 
+class GcnTrainParams(ctypes.Structure):
+    """danet_gcn_train_params: raw head parameters and their gradient pointers."""
+    _fields_ = [("W", c_p * 5), ("b", c_p * 5), ("bn_weight", c_p * 5), ("bn_bias", c_p * 5),
+                ("running_mean", c_p * 5), ("running_var", c_p * 5),
+                ("r2p_A", c_p), ("p2r_A", c_p), ("I_n", c_p), ("A_mask", c_p), ("edge_importance", c_p),
+                ("pose_w", c_p * 2), ("pose_b", c_p * 2), ("coord_w", c_p * 2), ("coord_b", c_p * 2),
+                ("mean_pose", c_p),
+                ("gW", c_p * 5), ("gb", c_p * 5), ("g_bn_weight", c_p * 5), ("g_bn_bias", c_p * 5),
+                ("g_edge_importance", c_p),
+                ("g_pose_w", c_p * 2), ("g_pose_b", c_p * 2), ("g_coord_w", c_p * 2), ("g_coord_b", c_p * 2)]
+
+
 # name -> (restype, argtypes); every symbol include/danet_b200.h declares
 SIGNATURES = {
     "danet_last_error": (ctypes.c_char_p, []),
@@ -96,6 +108,10 @@ SIGNATURES = {
     "danet_stn_params": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_f, c_int, c_p, c_p, c_p]),
     "danet_stn_sample": (c_int, [c_int, c_int, c_int, ctypes.POINTER(Act), c_p, c_int, ctypes.POINTER(Act), c_p]),
     "danet_gcn_pose_head": (c_int, [c_int, ctypes.POINTER(GcnParams), c_p, c_p, c_p, c_p]),
+    "danet_gcn_head_train_workspace_bytes": (c_i64, [c_int]),
+    "danet_gcn_head_train_forward": (c_int, [c_int, ctypes.POINTER(GcnTrainParams), c_int] + [c_p] * 9),
+    "danet_gcn_head_train_backward": (c_int, [c_int, ctypes.POINTER(GcnTrainParams), c_int] + [c_p] * 9),
+    "danet_gcn_head_losses": (c_int, [c_int] + [c_p] * 6 + [c_f, c_f] + [c_p] * 5),
     "danet_net_load": (c_int, [c_p, ctypes.c_uint64, ctypes.POINTER(c_p)]),
     "danet_net_load_file": (c_int, [ctypes.c_char_p, ctypes.POINTER(c_p)]),
     "danet_net_destroy": (c_int, [c_p]),

@@ -314,6 +314,50 @@ int danet_gcn_pose_head(int32_t B, const danet_gcn_params* p, const float* rot_f
                         danet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Regressor head, training path (csrc/gcn_train.cu): the same head as danet_gcn_pose_head, with raw (unfolded)
+ * parameters, BatchNorm1d(24) on batch statistics (training = 1) or on the running statistics (training = 0), the
+ * intermediate supervision heads of training mode and the backward.  fp32 throughout; no float atomics, every
+ * reduction in a fixed order (bit-repeatable), no host synchronisation (capturable in a CUDA graph).
+ * Layer l = 0..4: r2p_gcn.gc.0 [128->128], refine_gcn.gc.0..2 [128->256->256->128], p2r_gcn.gc.0 [128->128];
+ * W[l] [in,out] and b[l] [out] of GraphConv, bn_weight / bn_bias / running_mean / running_var [24] of act.<i>.0.
+ * Graph buffers [24*24]: r2p_A, p2r_A, I_n, A_mask; edge_importance [24*24] (a parameter).
+ * pose_w[k] [24*6][128], pose_b[k] [144] = pose_regressors.<k>.1; coord_w[k] [24*3][128], coord_b[k] [72] =
+ * coord_regressors.<k>.1; mean_pose [144].  The g* pointers receive the gradients (written, not accumulated); the
+ * pose_regressors.0 / coord_regressors gradients only in training mode (they may be NULL otherwise).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+    const float* W[5]; const float* b[5]; const float* bn_weight[5]; const float* bn_bias[5];
+    const float* running_mean[5]; const float* running_var[5];
+    const float* r2p_A; const float* p2r_A; const float* I_n; const float* A_mask; const float* edge_importance;
+    const float* pose_w[2]; const float* pose_b[2]; const float* coord_w[2]; const float* coord_b[2];
+    const float* mean_pose;
+    float* gW[5]; float* gb[5]; float* g_bn_weight[5]; float* g_bn_bias[5];
+    float* g_edge_importance;
+    float* g_pose_w[2]; float* g_pose_b[2]; float* g_coord_w[2]; float* g_coord_b[2];
+} danet_gcn_train_params;
+/* Bytes of the workspace one forward + backward pair shares (saved activations and backward scratch). */
+int64_t danet_gcn_head_train_workspace_bytes(int32_t B);
+/* smpl_regressor.py:849-895 + GCN.py:29-92 + graph.py:232-261 (normalize_undigraph of I_n + A_mask * relu(E), on the
+ * device) + geometry.py rot6d_to_rotmat: rot_feats [B,24,128], global_para [B,13] -> para [B,229]; in training mode
+ * also pose0 [B,216] (:849-856), coord0 / coord1 [B,24,3] (:863-882) and, when new_stats is not NULL, the updated
+ * running statistics new_stats [2][5][24] (mean | unbiased variance, momentum 0.1) -- the caller copies them into
+ * its buffers.  The workspace (16-byte aligned) keeps what the backward needs; pass the same one to it. */
+int danet_gcn_head_train_forward(int32_t B, const danet_gcn_train_params* p, int32_t training, const float* rot_feats,
+                                 const float* global_para, float* para, float* pose0, float* coord0, float* coord1,
+                                 float* new_stats, void* workspace, danet_stream_t stream);
+/* Backward of the forward above (same B, p, training, rot_feats, workspace): g_para [B,229] and, in training mode,
+ * g_pose0 [B,216], g_coord0 / g_coord1 [B,24,3] -> g_rot_feats [B,24,128], g_global_para [B,13] and every g* of p. */
+int danet_gcn_head_train_backward(int32_t B, const danet_gcn_train_params* p, int32_t training, const float* rot_feats,
+                                  const float* g_para, const float* g_pose0, const float* g_coord0, const float* g_coord1,
+                                  float* g_rot_feats, float* g_global_para, void* workspace, danet_stream_t stream);
+/* smpl_regressor.py:147-166,233-238: losses [3] = joint_rotation0 = rot_w * MSE(pose0, target[:,13:]) over the
+ * selected images, joint_position0/1 = pos_w * sum |coord - gt_joints| / #selected; has [B] (1 = selected).  With no
+ * image selected the losses and gradients are 0.  g_pose0 / g_coord0 / g_coord1 receive d(loss k)/d(input k). */
+int danet_gcn_head_losses(int32_t B, const float* pose0, const float* coord0, const float* coord1, const float* target,
+                          const float* gt_joints, const uint8_t* has, float rot_w, float pos_w, float* losses,
+                          float* g_pose0, float* g_coord0, float* g_coord1, danet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Whole-network entry (csrc/net.cu).  Replaces the network half of DaNet.infer_net
  * (models/danet/danet.py:78-98: img2iuv -> iuvmap_clean -> iuv2smpl, up to `para`) for hosts without Python.
  * A "network program" is what danet_b200.plan.Plan.export() writes for ONE batch size: the launch steps (each one of
