@@ -42,6 +42,12 @@ class ConvProblem(ctypes.Structure):
     _fields_ = [("d", ConvDesc), ("x", Act), ("res", Act), ("y", Act), ("w_packed", c_p), ("bias", c_p)]
 
 
+class DgradPiece(ctypes.Structure):
+    """danet_dgrad_piece: one stride-1 engine problem of the input gradient (see include/danet_b200.h)."""
+    _fields_ = [("a", c_int), ("b", c_int), ("K", c_int), ("tr", c_int), ("tc", c_int), ("jr0", c_int), ("jr1", c_int),
+                ("jc0", c_int), ("jc1", c_int)]
+
+
 class GcnParams(ctypes.Structure):
     _fields_ = [("adj", c_p), ("W", c_p * 5), ("b", c_p * 5), ("bn_scale", c_p * 5),
                 ("bn_shift", c_p * 5), ("dim_in", c_int * 5), ("dim_out", c_int * 5),
@@ -94,6 +100,17 @@ SIGNATURES = {
     "danet_conv_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),
     "danet_conv_tc_group": (c_int, [c_int, ctypes.POINTER(ConvProblem), c_p]),
     "danet_conv_tc_config": (c_int, [c_int, ctypes.POINTER(ConvDesc), c_p, c_p]),
+    "danet_conv_tc_pack_async": (c_int, [ctypes.POINTER(ConvDesc), c_p, c_p, c_p]),
+    "danet_conv_weights_simt": (c_int, [c_int] * 6 + [c_p, c_p, c_p]),
+    "danet_conv_dgrad_pieces": (c_int, [c_int, c_int, c_p]),
+    "danet_conv_dgrad_weights": (c_int, [c_int] * 5 + [c_p, c_int, c_int, c_p, c_p, c_p]),
+    "danet_conv_dgrad_scatter": (c_int, [c_int] * 9 + [c_p, ctypes.POINTER(c_p), c_p, c_p, c_p]),
+    "danet_conv_grad_split": (c_int, [c_int] * 4 + [c_p] * 5),
+    "danet_conv_wgrad_workspace_bytes": (c_i64, [ctypes.POINTER(ConvDesc)]),
+    "danet_conv_wgrad": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_int, ctypes.POINTER(Act), ctypes.POINTER(Act), c_p, c_p,
+                                 c_p, c_p]),
+    "danet_conv_bias_grad_workspace_bytes": (c_i64, [c_int, c_int, c_int]),
+    "danet_conv_bias_grad": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
     "danet_act_split": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_act_merge": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_nchw_to_nhwc": (c_int, [c_int, c_int, c_int, c_int, c_p, ctypes.POINTER(Act), c_p]),

@@ -36,6 +36,7 @@
 //   Launch: programmatic dependent launch; every mbarrier wait is bounded (traps instead of hanging).
 #include "common.cuh"
 #include "wgmma_f16.cuh"
+#include "tc_ptx.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <mutex>
@@ -203,58 +204,6 @@ static bool plan_rings(ArgsN* a) {
 // ---------------------------------------------------------------------------------------------
 // PTX helpers
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// arrive only where pred holds, as one predicated instruction: an `if (leader)` branch between wgmmas looks divergent
-// to ptxas, which then serialises them
-__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar), "r"((uint32_t)pred) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// one out-of-line copy: the bounded polling loop is ~40 SASS instructions and there are many wait sites
-__device__ __noinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-#pragma unroll 1
-    for (uint32_t it = 0; it < (1u << 22); ++it) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (done) return;
-    }
-    __trap();                                        // bounded wait: never hang the device
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3, uint32_t bar) {
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-                 ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
-}
-// programmatic dependent launch: this grid may start while the previous kernel of the stream drains; nothing the
-// previous kernel wrote (activations, residual) or still reads (our output may be its input) is touched before pdl_wait()
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// keeps the compiler from moving accumulator reads across wgmma.wait_group
-template <int NV> __device__ __forceinline__ void reg_fence(float* d) {
-#pragma unroll
-    for (int i = 0; i < NV; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
 // K-major swizzled shared-memory matrix descriptor of wgmma: start address and SBO (the stride between 8-row groups)
 // in 16-byte units, LBO unused for swizzled K-major layouts, swizzle mode in bits 62-63 (128B = 1, 64B = 2, 32B = 3).
 // The swizzle phase follows the absolute shared-memory address (the TMA writes the same pattern), so a start
@@ -287,23 +236,6 @@ __device__ __forceinline__ TileCoord decode_tile(const Prob& g, int t) {
     c.img = mdiv(r2, g.m_th); c.th = r2 - c.img * g.tiles_h;
     return c;
 }
-
-// Consumer-side wait: inlined, so that no call sits between wgmmas in flight (a call makes ptxas serialise them).
-// Still bounded: traps instead of hanging.
-__device__ __forceinline__ void mbar_wait_inl(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-#pragma unroll 1
-    for (uint32_t it = 0; it < (1u << 22); ++it) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (done) return;
-    }
-    __trap();
-}
-__device__ __forceinline__ void wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // ring positions of one consumer warpgroup (every consumer walks the A and B rings in the producer's order)
 struct Ring { int as, bs; uint32_t aph, bph; };
@@ -682,7 +614,7 @@ __global__ void k_pack_header(float scale, float* __restrict__ hdr) {
     if (threadIdx.x < kPackHeader / 4) hdr[threadIdx.x] = threadIdx.x == 0 ? scale : (threadIdx.x == 1 ? 1.0f / scale : 0.0f);
 }
 
-__global__ void k_pack(const Prob g, const float* __restrict__ w, __half* __restrict__ out, float scale) {
+__device__ __forceinline__ void pack_one(const Prob& g, const float* __restrict__ w, __half* __restrict__ out, float scale) {
     const int blk_halves = g.b_block_bytes / 2;
     const long long total = (long long)g.wsets * g.blocks_per_set * blk_halves;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -718,6 +650,25 @@ __global__ void k_pack(const Prob g, const float* __restrict__ w, __half* __rest
     const __half h = __float2half_rn(v);
     out[i] = want_lo ? __float2half_rn(v - __half2float(h)) : h;
 }
+__global__ void k_pack(const Prob g, const float* __restrict__ w, __half* __restrict__ out, float scale) {
+    pack_one(g, w, out, scale);
+}
+// the asynchronous packing path: the largest |w| lands in header word 2 (k_absmax), k_pack_header_dev turns it into the
+// scale and writes the header exactly as the host path does, and k_pack_dev reads the scale back from the header
+__global__ void k_pack_header_dev(float* __restrict__ hdr) {
+    __shared__ float sc;
+    if (threadIdx.x == 0) {
+        const float wmax = __uint_as_float(reinterpret_cast<const unsigned*>(hdr)[2]);
+        float scale = 1.0f;
+        if (wmax > 0.0f) { int e = 0; frexpf(wmax, &e); scale = ldexpf(1.0f, 14 - e); }
+        sc = scale;
+    }
+    __syncthreads();
+    if (threadIdx.x < kPackHeader / 4) hdr[threadIdx.x] = threadIdx.x == 0 ? sc : (threadIdx.x == 1 ? 1.0f / sc : 0.0f);
+}
+__global__ void k_pack_dev(const Prob g, const float* __restrict__ w, __half* __restrict__ out, const float* __restrict__ hdr) {
+    pack_one(g, w, out, __ldg(hdr));
+}
 
 // fp32 NHWC -> split-fp16 planes (test / boundary helper) and back
 __global__ void k_act_split(long long n, const float* __restrict__ x, __half* __restrict__ hi, __half* __restrict__ lo) {
@@ -737,22 +688,6 @@ __global__ void k_act_merge(long long n, const __half* __restrict__ hi, const __
 // ---------------------------------------------------------------------------------------------
 // host: tensor maps + launch
 // ---------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static PFN_encodeTiled encode_fn() {
-    static PFN_encodeTiled fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (PFN_encodeTiled)p;
-    });
-    return fn;
-}
-
 // the input tensor [N][H][W][Cin] fp16 as a 4-D tensor map whose box is the largest parity-plane halo of the problem
 // (all parity planes of a stride-2 problem share one map only if their boxes agree; they are encoded per slot otherwise --
 //  here every slot uses the MAXIMAL box and stage_bytes is that of the maximal box, see make_prob)
@@ -918,6 +853,23 @@ extern "C" int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt,
     tc::k_pack_header<<<1, 256, 0, st>>>(scale, (float*)w_packed);
     const long long total = (long long)g.wsets * g.blocks_per_set * (g.b_block_bytes / 2);
     tc::k_pack<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(g, w_simt, (__half*)((uint8_t*)w_packed + tc::kPackHeader), scale);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int danet_conv_tc_pack_async(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream) {
+    tc::Prob g;
+    DANET_CHECK(d && tc::make_prob(d, &g), "danet_conv_tc_pack_async: shape not supported by the tensor-core path");
+    DANET_CHECK(w_simt && w_packed, "danet_conv_tc_pack_async: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned* d_max = (unsigned*)w_packed + 2;         // header word 2: scratch for the absolute maximum
+    DANET_CUDA(cudaMemsetAsync(d_max, 0, 4, st));
+    const long long nw = (long long)d->wsets * d->ksize * d->ksize * d->Cin * d->Cout;
+    tc::k_absmax<<<132, 256, 0, st>>>(nw, w_simt, d_max);
+    tc::k_pack_header_dev<<<1, 256, 0, st>>>((float*)w_packed);
+    const long long total = (long long)g.wsets * g.blocks_per_set * (g.b_block_bytes / 2);
+    tc::k_pack_dev<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(g, w_simt, (__half*)((uint8_t*)w_packed + tc::kPackHeader),
+                                                                     (const float*)w_packed);
     DANET_LAUNCH_CHECK();
     return 0;
 }

@@ -241,9 +241,60 @@ int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* subti
 int64_t danet_conv_tc_packed_bytes(const danet_conv_desc* d);
 int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
 int danet_conv_tc_supported(const danet_conv_desc* d);
+/* danet_conv_tc_pack without host synchronisation or allocation (capturable in a CUDA graph), for weights that change
+ * every optimiser step: the same packed bytes.  Header word 2 of w_packed is its scratch while it runs. */
+int danet_conv_tc_pack_async(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
 /* fp32 -> split-fp16 planes (lo may be NULL) and back (lo may be NULL); n elements */
 int danet_act_split(int64_t n, const float* x, void* hi, void* lo, danet_stream_t stream);
 int danet_act_merge(int64_t n, const void* hi, const void* lo, float* y, danet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Convolution backward (csrc/conv_wgrad.cu), exact mode: the gradients of torch.nn.functional.conv2d for the shapes the
+ * tensor-core path accepts (k in {1,3,7}, pad k/2, stride 1|2, groups = wsets over the (batch, group)-flattened image
+ * axis).  Weights use the layout of nn.Conv2d.weight: w [wsets*cout][cin][k][k], where cout / cin are the real
+ * per-group channel counts and Cout / Cin >= them the multiples of 8 of the activation planes.  No float atomics: every
+ * result repeats bit for bit.  No host synchronisation: capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+/* forward weights in the SIMT layout [wsets][k*k*Cin][Cout] that danet_conv_tc_pack(_async) takes */
+int danet_conv_weights_simt(int32_t wsets, int32_t cout, int32_t cin, int32_t ksize, int32_t Cout, int32_t Cin,
+                            const float* w, float* w_simt, danet_stream_t stream);
+/* Input gradient.  Output-parity class (a, b) of dx (rows a mod stride, columns b mod stride) is a stride-1
+ * correlation of dy with the taps of w of that parity.  It is computed as one or more PIECES, each a 1x1 or 3x3
+ * stride-1 forward problem of the engine (input channels Cout, output channels Cin, padding K/2) whose output map at
+ * [u + tr][v + tc] adds to dx[stride*u + a][stride*v + b].  Taps jr0..jr1 / jc0..jc1 (tap r = r0 + stride*j of the
+ * class's parity) are the piece's.  Stride 1 has one piece: the filter rotated by 180 degrees.  7x7/s2: nine 3x3 pieces
+ * (81 taps executed for 49); 3x3/s2: four (28 for 9); 1x1/s2: one. */
+typedef struct { int32_t a, b, K, tr, tc, jr0, jr1, jc0, jc1; } danet_dgrad_piece;
+/* fills pieces[<= 9]; returns their number, or -1 for an unsupported ksize / stride (7x7 needs stride 2) */
+int32_t danet_conv_dgrad_pieces(int32_t ksize, int32_t stride, danet_dgrad_piece* pieces);
+/* the piece's kernel in the SIMT layout of its problem: w_out [wsets][K*K*Cout][Cin] */
+int danet_conv_dgrad_weights(int32_t wsets, int32_t cout, int32_t cin, int32_t ksize, int32_t stride,
+                             const danet_dgrad_piece* piece, int32_t Cout, int32_t Cin, const float* w, float* w_out,
+                             danet_stream_t stream);
+/* interleave / crop / sum: y NCHW [N,C,H,W] (fp32) with y[n][c][h][w] = sum in piece order over the pieces of class
+ * (h % stride, w % stride) of maps[i] at [n][h / stride + tr][w / stride + tc][c] (0 outside), times scale[1] when
+ * scale (device) is not NULL.  maps is a HOST array of npieces device pointers, each NHWC fp32 [N,Hc,Wc,Cp].  With
+ * stride 1 and the piece {0} it is the NHWC -> NCHW conversion. */
+int danet_conv_dgrad_scatter(int32_t N, int32_t C, int32_t H, int32_t W, int32_t Cp, int32_t stride, int32_t Hc, int32_t Wc,
+                             int32_t npieces, const danet_dgrad_piece* pieces, const float* const* maps,
+                             const float* scale, float* y, danet_stream_t stream);
+/* dy NCHW [N,C,HW] fp32 -> split-fp16 NHWC planes [N,HW,Cp] (Cp % 8 == 0, pad channels 0) of dy * 2^s, where the power
+ * of two 2^s brings max |dy| into [2^13, 2^14) (1 when dy is 0): gradients far below 1 keep their 22 bits.
+ * scale: device float[3]; receives scale[0] = 2^s, scale[1] = 2^-s (scale[2] is scratch).  No host synchronisation. */
+int danet_conv_grad_split(int32_t N, int32_t C, int32_t HW, int32_t Cp, const float* dy, void* hi, void* lo, float* scale,
+                          danet_stream_t stream);
+/* Weight gradient of the forward problem d (flags ignored; N % wsets == 0): x [N,H,W,Cin] and dy [N,Ho,Wo,Cout] as hi +
+ * lo split-fp16 planes; dy_scale = the scale danet_conv_grad_split wrote for dy (or NULL: unscaled).  dW
+ * [wsets*cout][cin][k][k] from a wgmma implicit GEMM over the pixels in split-fp16 exact arithmetic; split K over pixel
+ * chunks, partials in the workspace (16-byte aligned), chunks added in a fixed order in double, dy_scale removed
+ * exactly. */
+int64_t danet_conv_wgrad_workspace_bytes(const danet_conv_desc* d);
+int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout, int32_t cin, const danet_act* x, const danet_act* dy,
+                     const float* dy_scale, float* dW, void* workspace, danet_stream_t stream);
+/* Bias gradient: db[c] = sum over n and the HW pixels of the fp32 NCHW dy [N,C,HW]; image chunks summed in double with
+ * a fixed order, then added in chunk order.  Workspace 8-byte aligned. */
+int64_t danet_conv_bias_grad_workspace_bytes(int32_t N, int32_t C, int32_t HW);
+int danet_conv_bias_grad(int32_t N, int32_t C, int32_t HW, const float* dy, float* db, void* workspace, danet_stream_t stream);
 
 /* input boundary: x NCHW [N,C,HW] -> y NHWC [N,HW,Cp] with Cp >= C zero-padded channels
  * (images arrive NCHW: demo.py:106, eval.py:147) */
