@@ -138,6 +138,8 @@ SIGNATURES = {
     "danet_net_infer": (c_int, [c_p, c_p, c_int, c_p]),
     "danet_net_infer_host": (c_int, [c_p, c_p, c_int]),
     "danet_net_read_output": (c_int, [c_p, ctypes.c_char_p, c_p, ctypes.c_uint64]),
+    "danet_net_run_step": (c_int, [ctypes.c_uint32, c_int, ctypes.POINTER(c_int), c_int, ctypes.POINTER(c_f), c_int,
+                                   ctypes.POINTER(c_p), c_p]),
 }
 
 _lib = None

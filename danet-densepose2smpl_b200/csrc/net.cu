@@ -1,7 +1,8 @@
 // Whole-network entry of the C ABI: loads a "network program" (the launch steps, buffer table and packed / folded
 // weights that danet_b200.plan.Plan.export() writes for one batch size) and replays it -- the network half of
 // DaNet.infer_net (models/danet/danet.py:78-98: img2iuv -> iuvmap_clean -> iuv2smpl up to `para`) for hosts without
-// Python.  Every step calls the same C entry the Python plan calls, in the same order, so results are identical.
+// Python.  The Python plan runs each of its launches as one such step through danet_net_run_step, so both decode
+// every launch with the same prepare / run_step and results are identical.
 //
 // Program layout (little endian, sections 16-byte aligned):
 //   Header | u64 buf_bytes[n_buf] | {u64 off, u64 bytes} consts[n_const] | Out outs[n_out] | step stream | const payload
@@ -381,6 +382,18 @@ extern "C" int danet_net_infer_host(danet_net_t net, const float* images_host, i
     if (rc != 0) return rc;
     DANET_CUDA(cudaStreamSynchronize(net->own_stream));
     return 0;
+}
+
+extern "C" int danet_net_run_step(uint32_t op, int32_t n_i, const int32_t* i, int32_t n_f, const float* f, int32_t n_p,
+                                  void* const* p, danet_stream_t stream) {
+    DANET_CHECK(n_i >= 0 && n_f >= 0 && n_p >= 0 && (i || !n_i) && (f || !n_f) && (p || !n_p), "net_run_step: null argument");
+    Step s;
+    s.op = op;
+    s.i.assign(i, i + n_i);
+    s.f.assign(f, f + n_f);
+    s.p.assign(p, p + n_p);
+    int rc = prepare(s);
+    return rc != 0 ? rc : run_step(s, (cudaStream_t)stream);
 }
 
 extern "C" int danet_net_read_output(danet_net_t net, const char* name, void* host_dst, uint64_t bytes) {

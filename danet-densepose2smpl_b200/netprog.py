@@ -1,7 +1,8 @@
 """Python binding of the whole-network C entry (include/danet_b200.h danet_net_*, csrc/net.cu): loads a network
 program written by plan.Plan.export() / DaNet.export_program() and replays it without the Python plan.  This is what a
 non-Python host does through the same C calls (INTEGRATION.md, examples/net_host.c); here it mainly serves the tests
-that hold the C executor to the Python plan bit for bit."""
+that hold the C executor to the Python plan bit for bit (the plan launches through the same step decoder, one step at a
+time, with danet_net_run_step)."""
 import ctypes
 
 import torch

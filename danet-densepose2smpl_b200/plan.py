@@ -3,6 +3,7 @@ weights into the kernels' layouts, schedules the graph into launch steps (indepe
 HRNet's parallel branches, the body / limb regressors -- share one tensor-core launch), plans
 activation buffers (liveness-based reuse) and replays the steps through the C ABI (optionally as one
 CUDA graph)."""
+import collections
 import ctypes
 
 import numpy as np
@@ -23,13 +24,6 @@ class ActBuf(object):
     def __init__(self, f32=None, h=None):
         self.f32, self.h = f32, h
 
-    def c(self):
-        a = _lib.Act()
-        a.f32 = self.f32.data_ptr() if self.f32 is not None else None
-        a.hi = self.h[0].data_ptr() if self.h is not None else None
-        a.lo = self.h[1].data_ptr() if (self.h is not None and self.h.shape[0] > 1) else None
-        return a
-
     def value(self):
         """fp32 torch tensor of the activation (tests / debugging)."""
         if self.f32 is not None:
@@ -38,8 +32,108 @@ class ActBuf(object):
         return v + self.h[1].float() if self.h.shape[0] > 1 else v
 
 
-def _null_act():
-    return _lib.Act(None, None, None)
+# One launch of the plan: `name` is the CudaOps method that runs it, `args` its positional arguments.
+Step = collections.namedtuple("Step", "name args")
+
+# -- wire encoding ---------------------------------------------------------------------------------
+# A launch as one step record of the network program (csrc/net.cu): opcode, ints, floats and a flat pointer list in
+# the order net.cu's prepare / run_step decode it.  Plan.export writes these records and CudaOps runs them through
+# danet_net_run_step, so the Python plan and the C executor decode every launch with the same code.
+OPCODES = {"nchw_to_nhwc": 1, "conv_group": 2, "conv2d": 3, "fuse_sum": 4, "maxpool": 5, "avgpool": 6, "clean_global": 7,
+           "clean_parts": 8, "stn_params": 9, "stn_sample": 10, "linear": 11, "gcn_head": 12}
+_DESC_KEYS = ("N", "H", "W", "Cin", "Cout", "ksize", "stride", "pad", "wsets", "relu", "flags")
+
+
+def _desc_ints(d):
+    return [int(d.get(k, 0)) for k in _DESC_KEYS]
+
+
+def _act(a):
+    """danet_act pointers (f32, hi, lo) of an ActBuf; None is a null activation."""
+    if a is None:
+        return [None, None, None]
+    h = a.h
+    return [a.f32, h[0] if h is not None else None, h[1] if (h is not None and h.shape[0] > 1) else None]
+
+
+def _wire_conv_group(convs):
+    ints, ptrs = [len(convs)], []
+    for cv in convs:
+        ints += _desc_ints(cv["d"])
+        ptrs += _act(cv["x"]) + _act(cv["res"]) + _act(cv["y"]) + [cv["w"], cv["b"]]
+    return ints, [], ptrs
+
+
+def _wire_conv2d(d, x, w, bias, res, y):
+    return _desc_ints(d), [], [x.f32, w, bias, res.f32 if res is not None else None, y.f32]
+
+
+def _wire_nchw_to_nhwc(x, y):
+    N, C, H, W = x.shape
+    t = y.f32 if y.f32 is not None else y.h[0]
+    return [N, C, H * W, t.shape[-1]], [], [x] + _act(y)
+
+
+def _wire_fuse_sum(terms, factors, relu, y, shape):
+    N, H, W, C = shape
+    ptrs = []
+    for t in terms:
+        ptrs += _act(t)
+    return [N, H, W, C, len(terms), int(relu)] + [int(f) for f in factors], [], ptrs + _act(y)
+
+
+def _wire_maxpool(x, y, shape):
+    N, H, W, C = shape
+    return [N, H, W, C], [], _act(x) + _act(y)
+
+
+def _wire_avgpool(x, y, shape):
+    N, H, W, C = shape
+    return [N, H * W, C], [], _act(x) + [y]
+
+
+def _wire_linear(x, w, b, add, y):
+    return [x.shape[0], w.shape[1], w.shape[0]], [], [x, w, b, add, y]
+
+
+def _wire_clean_global(heads, body, amax, vis, shape):
+    B, H, W, Ch, Cb = shape
+    vis = list(vis) if vis is not None else [None] * 4
+    return [B, H * W, Ch, 0, 25, 50, 75, Cb], [], [heads.f32] + _act(body) + [amax] + vis
+
+
+def _wire_clean_parts(x, y, raw, shape):
+    N, H, W, Cx, Cy = shape
+    return [N, H * W, Cx, Cy], [], [x.f32] + _act(y) + [raw]
+
+
+def _wire_stn_params(hm, amax, ratio, offset, vis_thresh, align_corners, centers, theta):
+    B, S, _, Chm = hm.f32.shape
+    return [B, S, Chm, int(align_corners)], [float(vis_thresh)], [hm.f32, amax, ratio, offset, centers, theta]
+
+
+def _wire_stn_sample(xd, theta, align_corners, crops, shape):
+    B, S, C = shape
+    return [B, S, C, int(align_corners)], [], _act(xd) + [theta] + _act(crops)
+
+
+def _wire_gcn_head(gp, rot_feats, gpara, para):
+    ints = [para.shape[0]] + [int(w.shape[0]) for w in gp["W"]] + [int(w.shape[1]) for w in gp["W"]]
+    ptrs = [gp["adj"]] + gp["W"] + gp["b"] + gp["bn_scale"] + gp["bn_shift"] + \
+           [gp["head_w"], gp["head_b"], gp["mean_pose"], rot_feats, gpara, para]
+    return ints, [], ptrs
+
+
+_WIRE = {"nchw_to_nhwc": _wire_nchw_to_nhwc, "conv_group": _wire_conv_group, "conv2d": _wire_conv2d,
+         "fuse_sum": _wire_fuse_sum, "maxpool": _wire_maxpool, "avgpool": _wire_avgpool, "clean_global": _wire_clean_global,
+         "clean_parts": _wire_clean_parts, "stn_params": _wire_stn_params, "stn_sample": _wire_stn_sample,
+         "linear": _wire_linear, "gcn_head": _wire_gcn_head}
+
+
+def wire(name, args):
+    """(opcode, ints, floats, ptrs) of launch `name` with CudaOps arguments `args`; ptrs are tensors or None."""
+    ints, floats, ptrs = _WIRE[name](*args)
+    return OPCODES[name], ints, floats, ptrs
 
 
 class CudaOps(object):
@@ -91,85 +185,51 @@ class CudaOps(object):
         _lib.check(self.lib.danet_conv_tc_config(n, arr, ctypes.cast(S, ctypes.c_void_p), ctypes.cast(st, ctypes.c_void_p)), "conv_tc_config")
         return list(S), (st[0], st[1])
 
+    # -- launches: each is one step record (`wire`) run by danet_net_run_step --------------------------
+    def _run(self, name, *args):
+        op, ints, floats, ptrs = wire(name, args)
+        _lib.check(self.lib.danet_net_run_step(op, len(ints), (ctypes.c_int32 * len(ints))(*ints),
+                                               len(floats), (ctypes.c_float * len(floats))(*floats),
+                                               len(ptrs), (ctypes.c_void_p * len(ptrs))(*[_lib.ptr(p) for p in ptrs]),
+                                               self._sp()), name)
+
     def conv_group(self, convs):
         """convs: list of dict(d, x, res, y (ActBuf), w (packed), b)."""
-        arr = (_lib.ConvProblem * len(convs))()
-        for i, cv in enumerate(convs):
-            p = arr[i]
-            p.d = self._desc(cv["d"])
-            p.x = cv["x"].c()
-            p.res = cv["res"].c() if cv["res"] is not None else _null_act()
-            p.y = cv["y"].c()
-            p.w_packed = cv["w"].data_ptr()
-            p.bias = cv["b"].data_ptr() if cv["b"] is not None else None
-        _lib.check(self.lib.danet_conv_tc_group(len(convs), arr, self._sp()), "conv_tc_group")
+        self._run("conv_group", convs)
 
     def conv2d(self, d, x, w, bias, res, y):
         """fp32 FMA convolution on the fp32 views."""
-        _lib.check(self.lib.danet_conv2d(ctypes.byref(self._desc(d)), 0, _lib.ptr(x.f32), _lib.ptr(w), _lib.ptr(bias),
-                                         _lib.ptr(res.f32 if res is not None else None), _lib.ptr(y.f32), self._sp()), "conv2d")
+        self._run("conv2d", d, x, w, bias, res, y)
 
     def nchw_to_nhwc(self, x, y):
-        N, C, H, W = x.shape
-        t = y.f32 if y.f32 is not None else y.h[0]
-        _lib.check(self.lib.danet_nchw_to_nhwc(N, C, H * W, t.shape[-1], _lib.ptr(x), ctypes.byref(y.c()), self._sp()),
-                   "nchw_to_nhwc")
+        self._run("nchw_to_nhwc", x, y)
 
     def fuse_sum(self, terms, factors, relu, y, shape):
-        N, H, W, C = shape
-        n = len(terms)
-        arr = (_lib.Act * n)(*[t.c() for t in terms])
-        fac = (ctypes.c_int32 * n)(*factors)
-        _lib.check(self.lib.danet_fuse_sum(N, H, W, C, n, arr, ctypes.cast(fac, ctypes.c_void_p), int(relu),
-                                           ctypes.byref(y.c()), self._sp()), "fuse_sum")
+        self._run("fuse_sum", terms, factors, relu, y, shape)
 
     def maxpool(self, x, y, shape):
-        N, H, W, C = shape
-        _lib.check(self.lib.danet_maxpool3x3s2(N, H, W, C, ctypes.byref(x.c()), ctypes.byref(y.c()), self._sp()), "maxpool")
+        self._run("maxpool", x, y, shape)
 
     def avgpool(self, x, y, shape):
-        N, H, W, C = shape
-        _lib.check(self.lib.danet_global_avgpool(N, H * W, C, ctypes.byref(x.c()), _lib.ptr(y), self._sp()), "avgpool")
+        self._run("avgpool", x, y, shape)
 
     def linear(self, x, w, b, add, y):
-        N, In = x.shape[0], w.shape[1]
-        _lib.check(self.lib.danet_linear(N, In, w.shape[0], _lib.ptr(x), _lib.ptr(w), _lib.ptr(b), _lib.ptr(add),
-                                         _lib.ptr(y), self._sp()), "linear")
+        self._run("linear", x, w, b, add, y)
 
     def clean_global(self, heads, body, amax, vis, shape):
-        B, H, W, Ch, Cb = shape
-        u, v, i, a = vis if vis is not None else (None, None, None, None)
-        _lib.check(self.lib.danet_iuv_clean_global(B, H * W, Ch, 0, 25, 50, 75, Cb, _lib.ptr(heads.f32),
-                                                   ctypes.byref(body.c()), _lib.ptr(amax), _lib.ptr(u), _lib.ptr(v), _lib.ptr(i),
-                                                   _lib.ptr(a), self._sp()), "iuv_clean_global")
+        self._run("clean_global", heads, body, amax, vis, shape)
 
     def clean_parts(self, x, y, raw, shape):
-        N, H, W, Cx, Cy = shape
-        _lib.check(self.lib.danet_iuv_clean_parts(N, H * W, Cx, Cy, _lib.ptr(x.f32), ctypes.byref(y.c()), _lib.ptr(raw),
-                                                  self._sp()), "iuv_clean_parts")
+        self._run("clean_parts", x, y, raw, shape)
 
     def stn_params(self, hm, amax, ratio, offset, vis_thresh, align_corners, centers, theta):
-        B, S, _, Chm = hm.f32.shape
-        _lib.check(self.lib.danet_stn_params(B, S, Chm, _lib.ptr(hm.f32), _lib.ptr(amax), _lib.ptr(ratio), _lib.ptr(offset),
-                                             float(vis_thresh), int(align_corners), _lib.ptr(centers), _lib.ptr(theta),
-                                             self._sp()), "stn_params")
+        self._run("stn_params", hm, amax, ratio, offset, vis_thresh, align_corners, centers, theta)
 
     def stn_sample(self, xd, theta, align_corners, crops, shape):
-        B, S, C = shape
-        _lib.check(self.lib.danet_stn_sample(B, S, C, ctypes.byref(xd.c()), _lib.ptr(theta), int(align_corners),
-                                             ctypes.byref(crops.c()), self._sp()), "stn_sample")
+        self._run("stn_sample", xd, theta, align_corners, crops, shape)
 
     def gcn_head(self, gp, rot_feats, gpara, para):
-        B = para.shape[0]
-        p = _lib.GcnParams()
-        p.adj = gp["adj"].data_ptr()
-        for l in range(5):
-            p.W[l] = gp["W"][l].data_ptr(); p.b[l] = gp["b"][l].data_ptr()
-            p.bn_scale[l] = gp["bn_scale"][l].data_ptr(); p.bn_shift[l] = gp["bn_shift"][l].data_ptr()
-            p.dim_in[l], p.dim_out[l] = gp["W"][l].shape
-        p.head_w = gp["head_w"].data_ptr(); p.head_b = gp["head_b"].data_ptr(); p.mean_pose = gp["mean_pose"].data_ptr()
-        _lib.check(self.lib.danet_gcn_pose_head(B, ctypes.byref(p), _lib.ptr(rot_feats), _lib.ptr(gpara), _lib.ptr(para),
-                                                self._sp()), "gcn_pose_head")
+        self._run("gcn_head", gp, rot_feats, gpara, para)
 
 
 def fold_bn(sd, prefix, cout):
@@ -288,38 +348,38 @@ class Plan(object):
         self.group_convs = group_convs and self.tc
         self.keep_all = keep_all                      # debugging: no buffer reuse, every intermediate stays readable
         self.wcache = wcache if wcache is not None else {}
-        self.n_launch = 0
         self.n_tc = 0
+        self.consts = set()                           # data_ptr of every weight-like tensor a step reads (export: payload)
         sd = state_dict
         dev = self.device
         with self._guard():
             self._schedule()
             self._formats()
             self._plan_buffers()
-            self.steps = []
-            for level_ops in self.schedule:
-                group = []
-                for op in level_ops:
-                    kind = op["op"]
-                    if kind == "conv":
-                        cv = self._make_conv(op, sd)
-                        if self.tc:
-                            group.append(cv)
-                        else:
-                            self.steps.append(("conv_simt", cv))
-                    else:
-                        self._add_glue(op, sd)
-                # tensor-core convolutions of one level: independent by construction, <= MAX_GROUP per launch,
-                # most expensive tiles first (they start first inside the persistent grid)
-                group.sort(key=lambda c: -c["cost"])
-                for g in self._form_groups(group):
-                    self.steps.append(("conv_group", g))
             S = graph.outputs["heads"].H
             self.vis = None
             self.raw_parts = None
             if want_vis:
                 self.vis = [torch.empty(B, c, S, S, device=dev) for c in (25, 25, 25, 15)]
                 self.raw_parts = torch.empty(B * 24, 21, S, S, device=dev)
+            self.steps = []
+            for level_ops in self.schedule:
+                group = []
+                for op in level_ops:
+                    if op["op"] == "conv":
+                        cv = self._make_conv(op, sd)
+                        if self.tc:
+                            group.append(cv)
+                        else:
+                            self.steps.append(Step("conv2d", (cv["d"], cv["x"], cv["w"], cv["b"], cv["res"], cv["y"])))
+                    else:
+                        self.steps += self._lower_glue(op, sd)
+                # tensor-core convolutions of one level: independent by construction, <= MAX_GROUP per launch,
+                # most expensive tiles first (they start first inside the persistent grid)
+                group.sort(key=lambda c: -c["cost"])
+                for g in self._form_groups(group):
+                    self.steps.append(Step("conv_group", (g,)))
+        self.n_launch = len(self.steps)
         self.graph_exec = None
         self.use_cuda_graph = use_cuda_graph
         self.static_in = None
@@ -510,6 +570,7 @@ class Plan(object):
                 w = self.ops.conv_tc_pack(d, w)
             self.wcache[key] = (w, b)
         w, b = self.wcache[key]
+        self._const(w, b)
         if self.tc:
             self.n_tc += 1
         Ho, Wo = y.H, y.W
@@ -517,65 +578,57 @@ class Plan(object):
         return dict(d=d, w=w, b=b, x=self.T(x), y=self.T(y), res=self.T(op["res"]) if op["res"] is not None else None,
                     cost=cost, op=op)
 
-    def _add_glue(self, op, sd):
-        kind = op["op"]
-        dev, B = self.device, self.B
-        if kind in ("input", "fuse", "maxpool", "avgpool", "clean_global", "clean_parts", "stn_sample"):
-            self.steps.append((kind, op))
-        elif kind == "stn_params":
-            self.ratio = sd["img2iuv.learned_ratio"].float().contiguous().to(dev)
-            self.offset = sd["img2iuv.learned_offset"].float().contiguous().to(dev)
-            self.steps.append((kind, op))
-        elif kind == "body_fc":
-            self.fc_w = sd[self.RP + "body_net.3.final_layer.weight"].float().contiguous().to(dev)
-            self.fc_b = sd[self.RP + "body_net.3.final_layer.bias"].float().contiguous().to(dev)
-            self.fc_add = sd[self.RP + "mean_cam_shape"].float().reshape(13).contiguous().to(dev)
+    def _const(self, *ts):
+        """Marks weight-like tensors: an exported program carries them in its payload."""
+        self.consts.update(t.data_ptr() for t in ts)
+
+    def _lower_glue(self, op, sd):
+        """Step records of one op that is not a convolution."""
+        kind, T, dev, B = op["op"], self.T, self.device, self.B
+        x, y = op.get("x"), op.get("y")
+        if kind == "input":
+            # `run` puts the caller's image in place of this placeholder; export refers to the program's input
+            self.image = torch.empty(B, 3, y.H, y.W, device="meta")
+            return [Step("nchw_to_nhwc", (self.image, T(y)))]
+        if kind == "fuse":
+            terms = op["terms"]
+            return [Step("fuse_sum", ([T(t) for t, _ in terms], [f for _, f in terms], op["relu"], T(y), self.shape(y)))]
+        if kind == "maxpool":
+            return [Step("maxpool", (T(x), T(y), self.shape(x)))]
+        if kind == "avgpool":
+            return [Step("avgpool", (T(x), T(y).f32, self.shape(x)))]
+        if kind == "clean_global":
+            return [Step("clean_global", (T(x), T(y), T(op["amax"]), self.vis, (B, x.H, x.W, x.Cp, y.Cp)))]
+        if kind == "stn_params":
+            ratio = sd["img2iuv.learned_ratio"].float().contiguous().to(dev)
+            offset = sd["img2iuv.learned_offset"].float().contiguous().to(dev)
+            self._const(ratio, offset)
+            return [Step("stn_params", (T(op["hm"]), T(op["amax"]), ratio, offset, self.vis_thresh, self.align_corners,
+                                        T(op["centers"]).f32, T(op["theta"]).f32))]
+        if kind == "stn_sample":
+            return [Step("stn_sample", (T(x), T(op["theta"]).f32, self.align_corners, T(y), (B, x.H, x.Cp)))]
+        if kind == "clean_parts":
+            return [Step("clean_parts", (T(x), T(y), self.raw_parts, (B * x.nmult, x.H, x.W, x.Cp, y.Cp)))]
+        if kind == "body_fc":
+            fc_w = sd[self.RP + "body_net.3.final_layer.weight"].float().contiguous().to(dev)
+            fc_b = sd[self.RP + "body_net.3.final_layer.bias"].float().contiguous().to(dev)
+            fc_add = sd[self.RP + "mean_cam_shape"].float().reshape(13).contiguous().to(dev)
+            self._const(fc_w, fc_b, fc_add)
             self.pooled = torch.empty(B, 512, device=dev)
-            self.steps.append((kind, op))
-        elif kind == "gcn_head":
-            self.gcn = pack_gcn(sd, self.RP, dev)
-            self.steps.append((kind, op))
-        else:
-            raise ValueError("unknown op %s" % kind)
+            return [Step("avgpool", (T(x), self.pooled, self.shape(x))),
+                    Step("linear", (self.pooled, fc_w, fc_b, fc_add, T(y).f32))]
+        if kind == "gcn_head":
+            gp = self.gcn = pack_gcn(sd, self.RP, dev)
+            self._const(gp["adj"], *gp["W"], *gp["b"], *gp["bn_scale"], *gp["bn_shift"], gp["head_w"], gp["head_b"],
+                        gp["mean_pose"])
+            return [Step("gcn_head", (gp, T(x).f32, T(op["gpara"]).f32, T(y).f32))]
+        raise ValueError("unknown op %s" % kind)
 
     # -- run ----------------------------------------------------------------------------------
     def _run_steps(self, image):
-        ops = self.ops
-        n = 0
-        for kind, op in self.steps:
-            if kind == "conv_group":
-                ops.conv_group(op)
-            elif kind == "conv_simt":
-                ops.conv2d(op["d"], op["x"], op["w"], op["b"], op["res"], op["y"])
-            elif kind == "input":
-                ops.nchw_to_nhwc(image, self.T(op["y"]))
-            elif kind == "fuse":
-                ops.fuse_sum([self.T(t) for t, _ in op["terms"]], [f for _, f in op["terms"]], op["relu"], self.T(op["y"]),
-                             self.shape(op["y"]))
-            elif kind == "maxpool":
-                ops.maxpool(self.T(op["x"]), self.T(op["y"]), self.shape(op["x"]))
-            elif kind == "avgpool":
-                ops.avgpool(self.T(op["x"]), self.T(op["y"]).f32, self.shape(op["x"]))
-            elif kind == "clean_global":
-                x, y = op["x"], op["y"]
-                ops.clean_global(self.T(x), self.T(y), self.T(op["amax"]), self.vis, (self.B, x.H, x.W, x.Cp, y.Cp))
-            elif kind == "stn_params":
-                ops.stn_params(self.T(op["hm"]), self.T(op["amax"]), self.ratio, self.offset, self.vis_thresh,
-                               self.align_corners, self.T(op["centers"]).f32, self.T(op["theta"]).f32)
-            elif kind == "stn_sample":
-                x = op["x"]
-                ops.stn_sample(self.T(x), self.T(op["theta"]).f32, self.align_corners, self.T(op["y"]), (self.B, x.H, x.Cp))
-            elif kind == "clean_parts":
-                x, y = op["x"], op["y"]
-                ops.clean_parts(self.T(x), self.T(y), self.raw_parts, (self.B * x.nmult, x.H, x.W, x.Cp, y.Cp))
-            elif kind == "body_fc":
-                ops.avgpool(self.T(op["x"]), self.pooled, self.shape(op["x"]))
-                ops.linear(self.pooled, self.fc_w, self.fc_b, self.fc_add, self.T(op["y"]).f32)
-                n += 1
-            elif kind == "gcn_head":
-                ops.gcn_head(self.gcn, self.T(op["x"]).f32, self.T(op["gpara"]).f32, self.T(op["y"]).f32)
-            n += 1
-        self.n_launch = n
+        for s in self.steps:
+            args = (image,) + s.args[1:] if s.args[0] is self.image else s.args
+            getattr(self.ops, s.name)(*args)
 
     def run(self, image):
         """image [B,3,H,W] fp32 NCHW on the plan's device.  Results stay in the plan's buffers."""
@@ -601,10 +654,6 @@ class Plan(object):
             self.graph_exec.replay()
 
     # -- export ---------------------------------------------------------------------------------
-    OPCODES = {"input": 1, "conv_group": 2, "conv_simt": 3, "fuse": 4, "maxpool": 5, "avgpool": 6, "clean_global": 7,
-               "clean_parts": 8, "stn_params": 9, "stn_sample": 10, "linear": 11, "gcn_head": 12}
-    _DESC_KEYS = ("N", "H", "W", "Cin", "Cout", "ksize", "stride", "pad", "wsets", "relu", "flags")
-
     def export(self, path=None):
         """Serialise this plan as a network program for danet_net_load (csrc/net.cu, include/danet_b200.h): the launch
         steps with their arguments, the activation buffer table and the folded / packed weights.  Returns the bytes
@@ -612,97 +661,32 @@ class Plan(object):
         import struct
         bufs, consts = {}, {}                          # storage ptr -> (id, nbytes) ; tensor ptr -> (id, tensor)
 
-        def bref(t):
+        def ref(t):
+            """(kind, id, offset) of one pointer: 0 null, 1 activation buffer, 2 constant, 3 the input image."""
             if t is None:
                 return (0, 0, 0)
+            if t is self.image:
+                return (3, 0, 0)
+            key = t.data_ptr()
+            if key in self.consts:
+                if not t.is_contiguous():
+                    raise RuntimeError("export: constant tensors must be contiguous")
+                if key not in consts:
+                    consts[key] = (len(consts), t)
+                return (2, consts[key][0], 0)
             st = t.untyped_storage()
             key = st.data_ptr()
             if key not in bufs:
                 bufs[key] = (len(bufs), st.nbytes())
             return (1, bufs[key][0], t.data_ptr() - key)
 
-        def cref(t):
-            if t is None:
-                return (0, 0, 0)
-            if not t.is_contiguous():
-                raise RuntimeError("export: constant tensors must be contiguous")
-            key = t.data_ptr()
-            if key not in consts:
-                consts[key] = (len(consts), t)
-            return (2, consts[key][0], 0)
-
-        def aref(a):
-            if a is None:
-                return [(0, 0, 0)] * 3
-            lo = a.h[1] if (a.h is not None and a.h.shape[0] > 1) else None
-            return [bref(a.f32), bref(a.h[0] if a.h is not None else None), bref(lo)]
-
-        def desc(d):
-            return [int(d.get(k, 0)) for k in self._DESC_KEYS]
-
-        steps = []                                      # (opcode, ints, floats, refs)
-        OP = self.OPCODES
-        for kind, op in self.steps:
-            if kind == "conv_group":
-                ints, refs = [len(op)], []
-                for cv in op:
-                    ints += desc(cv["d"])
-                    refs += aref(cv["x"]) + aref(cv["res"]) + aref(cv["y"]) + [cref(cv["w"]), cref(cv["b"])]
-                steps.append((OP[kind], ints, [], refs))
-            elif kind == "conv_simt":
-                res = op["res"].f32 if op["res"] is not None else None
-                steps.append((OP[kind], desc(op["d"]), [], [bref(op["x"].f32), cref(op["w"]), cref(op["b"]), bref(res), bref(op["y"].f32)]))
-            elif kind == "input":
-                y = self.T(op["y"])
-                t = y.f32 if y.f32 is not None else y.h[0]
-                Hin, Win = op["y"].H, op["y"].W
-                steps.append((OP[kind], [self.B, 3, Hin * Win, t.shape[-1]], [], [(3, 0, 0)] + aref(y)))
-            elif kind == "fuse":
-                N, H, W, C = self.shape(op["y"])
-                terms = op["terms"]
-                refs = []
-                for t, _f in terms:
-                    refs += aref(self.T(t))
-                steps.append((OP[kind], [N, H, W, C, len(terms), int(op["relu"])] + [int(f) for _, f in terms], [],
-                              refs + aref(self.T(op["y"]))))
-            elif kind == "maxpool":
-                steps.append((OP[kind], list(self.shape(op["x"])), [], aref(self.T(op["x"])) + aref(self.T(op["y"]))))
-            elif kind == "avgpool":
-                N, H, W, C = self.shape(op["x"])
-                steps.append((OP[kind], [N, H * W, C], [], aref(self.T(op["x"])) + [bref(self.T(op["y"]).f32)]))
-            elif kind == "clean_global":
-                x, y = op["x"], op["y"]
-                vis = self.vis if self.vis is not None else [None] * 4
-                steps.append((OP[kind], [self.B, x.H * x.W, x.Cp, 0, 25, 50, 75, y.Cp], [],
-                              [bref(self.T(x).f32)] + aref(self.T(y)) + [bref(self.T(op["amax"]))] + [bref(v) for v in vis]))
-            elif kind == "stn_params":
-                hm = self.T(op["hm"]).f32
-                steps.append((OP[kind], [hm.shape[0], hm.shape[1], hm.shape[3], int(self.align_corners)], [float(self.vis_thresh)],
-                              [bref(hm), bref(self.T(op["amax"])), cref(self.ratio), cref(self.offset),
-                               bref(self.T(op["centers"]).f32), bref(self.T(op["theta"]).f32)]))
-            elif kind == "stn_sample":
-                x = op["x"]
-                steps.append((OP[kind], [self.B, x.H, x.Cp, int(self.align_corners)], [],
-                              aref(self.T(x)) + [bref(self.T(op["theta"]).f32)] + aref(self.T(op["y"]))))
-            elif kind == "clean_parts":
-                x, y = op["x"], op["y"]
-                steps.append((OP[kind], [self.B * x.nmult, x.H * x.W, x.Cp, y.Cp], [],
-                              [bref(self.T(x).f32)] + aref(self.T(y)) + [bref(self.raw_parts)]))
-            elif kind == "body_fc":
-                N, H, W, C = self.shape(op["x"])
-                steps.append((OP["avgpool"], [N, H * W, C], [], aref(self.T(op["x"])) + [bref(self.pooled)]))
-                steps.append((OP["linear"], [N, self.fc_w.shape[1], self.fc_w.shape[0]], [],
-                              [bref(self.pooled), cref(self.fc_w), cref(self.fc_b), cref(self.fc_add), bref(self.T(op["y"]).f32)]))
-            elif kind == "gcn_head":
-                gp = self.gcn
-                ints = [self.B] + [int(w.shape[0]) for w in gp["W"]] + [int(w.shape[1]) for w in gp["W"]]
-                refs = [cref(gp["adj"])] + [cref(t) for t in gp["W"]] + [cref(t) for t in gp["b"]] + \
-                       [cref(t) for t in gp["bn_scale"]] + [cref(t) for t in gp["bn_shift"]] + \
-                       [cref(gp["head_w"]), cref(gp["head_b"]), cref(gp["mean_pose"]), bref(self.T(op["x"]).f32),
-                        bref(self.T(op["gpara"]).f32), bref(self.T(op["y"]).f32)]
-                steps.append((OP[kind], ints, [], refs))
-            else:
-                raise ValueError("export: unknown step %s" % kind)
+        step_bytes = b""
+        for s in self.steps:
+            code, ints, floats, ptrs = wire(s.name, s.args)
+            step_bytes += struct.pack("<4I", code, len(ints), len(floats), len(ptrs))
+            step_bytes += struct.pack("<%di" % len(ints), *ints) + struct.pack("<%df" % len(floats), *floats)
+            for p in ptrs:
+                step_bytes += struct.pack("<IIQ", *ref(p))
 
         outs = []                                       # (name, ref, elem_bytes, dims)
         for k in self.KEEP:
@@ -710,21 +694,15 @@ class Plan(object):
                 continue
             a = self.T(self.g.outputs[k])
             t = a if torch.is_tensor(a) else a.f32
-            outs.append((k, bref(t), t.element_size(), list(t.shape)))
+            outs.append((k, ref(t), t.element_size(), list(t.shape)))
         if self.vis is not None:
             for nm, t in zip(("vis_u", "vis_v", "vis_i", "vis_a"), self.vis):
-                outs.append((nm, bref(t), 4, list(t.shape)))
-            outs.append(("part_iuv_raw", bref(self.raw_parts), 4, list(self.raw_parts.shape)))
+                outs.append((nm, ref(t), 4, list(t.shape)))
+            outs.append(("part_iuv_raw", ref(self.raw_parts), 4, list(self.raw_parts.shape)))
 
         def pad16(b):
             return b + b"\0" * (-len(b) % 16)
 
-        step_bytes = b""
-        for (code, ints, floats, refs) in steps:
-            step_bytes += struct.pack("<4I", code, len(ints), len(floats), len(refs))
-            step_bytes += struct.pack("<%di" % len(ints), *ints) + struct.pack("<%df" % len(floats), *floats)
-            for r in refs:
-                step_bytes += struct.pack("<IIQ", *r)
         buf_list = sorted(bufs.values())
         const_list = sorted(consts.values(), key=lambda c: c[0])
         hdr_size = 8 + 12 * 4 + 4 * 8
@@ -737,21 +715,20 @@ class Plan(object):
             crecs.append((off, n))
             off += (n + 15) // 16 * 16
         payload_bytes = off - payload_off
-        img = [op["y"] for kind, op in self.steps if kind == "input"][0]
-        Hin, Win = img.H, img.W
         prec = 2 if not self.tc else (1 if self.precision == "exact" else 0)
         blob = bytearray()
-        blob += b"DANETPRG" + struct.pack("<12I", 1, self.B, 3, Hin, Win, len(buf_list), len(const_list), len(outs), len(steps), prec, 0, 0)
+        blob += b"DANETPRG" + struct.pack("<12I", 1, *self.image.shape, len(buf_list), len(const_list), len(outs), len(self.steps), prec,
+                                             0, 0)
         blob += struct.pack("<4Q", steps_off, len(step_bytes), payload_off, payload_bytes)
         for (_i, nbytes) in buf_list:
             blob += struct.pack("<Q", nbytes)
         for (o, n) in crecs:
             blob += struct.pack("<QQ", o, n)
-        for (name, ref, eb, dims) in outs:
+        for (name, r, eb, dims) in outs:
             d = (list(dims) + [1, 1, 1, 1])[:4]
             if len(dims) > 4:
                 raise RuntimeError("export: output %s has more than 4 dims" % name)
-            blob += name.encode()[:31].ljust(32, b"\0") + struct.pack("<IIQ", *ref) + struct.pack("<Ii4i", eb, len(dims), *d)
+            blob += name.encode()[:31].ljust(32, b"\0") + struct.pack("<IIQ", *r) + struct.pack("<Ii4i", eb, len(dims), *d)
         blob += b"\0" * (steps_off - len(blob))
         blob += step_bytes
         blob += b"\0" * (payload_off - len(blob))

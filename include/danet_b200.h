@@ -414,8 +414,10 @@ int danet_gcn_head_losses(int32_t B, const float* pose0, const float* coord0, co
  * A "network program" is what danet_b200.plan.Plan.export() writes for ONE batch size: the launch steps (each one of
  * the entries above, with its arguments), the activation buffer table and the BN-folded, packed weights.  Loading
  * allocates everything on the CURRENT device; infer replays the steps (optionally as one CUDA graph, captured on the
- * first call).  A danet_net_t owns its buffers: one infer at a time per handle (load one handle per host thread / stream
- * that runs concurrently).  Outputs stay in the program's buffers until the next infer:
+ * first call).  danet_net_run_step runs one step record directly; the Python plan launches every kernel through it, so
+ * it and a loaded program decode the same records with the same code.  A danet_net_t owns its buffers: one infer at a
+ * time per handle (load one handle per host thread / stream that runs concurrently).  Outputs stay in the program's
+ * buffers until the next infer:
  *   "para" [B,229] f32 (cam 3 | shape 10 | 24 rotation matrices, danet.py:118), "centers" [B,24,2] (stn_kps_pred),
  *   "theta", "global_para", "rot_feats", "heads", "hm", "body_iuv", "amax" (u8 [B,S,S]) and, when the plan kept the
  *   visualisation maps, "vis_u" / "vis_v" / "vis_i" [B,25,S,S], "vis_a" [B,15,S,S], "part_iuv_raw" [B*24,21,S,S].
@@ -437,6 +439,10 @@ int danet_net_infer(danet_net_t net, const float* images, int32_t flags, danet_s
 int danet_net_infer_host(danet_net_t net, const float* images_host, int32_t flags);
 /* synchronous device -> host copy of a named output; `bytes` must equal the output's size */
 int danet_net_read_output(danet_net_t net, const char* name, void* host_dst, uint64_t bytes);
+/* one step of the program format (opcode, ints, floats and n_p raw pointers where a program has references; a danet_act
+ * is three pointers f32, hi, lo), checked and run on the current device exactly as danet_net_infer runs it */
+int danet_net_run_step(uint32_t op, int32_t n_i, const int32_t* i, int32_t n_f, const float* f, int32_t n_p,
+                       void* const* p, danet_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -62,8 +62,8 @@ def _views(a):
 
 
 @pytest.mark.parametrize("algo", ["simt", "tc"])
-def test_buffer_plan_reuses_memory_without_aliasing_live_tensors(algo):
-    """Liveness-based reuse over the scheduled steps: a step never reads and writes the same storage, and the
+def test_step_records_reuse_memory_without_aliasing_live_tensors(algo):
+    """Liveness-based reuse over the plan's step records: a step never reads and writes the same storage, and the
     convolutions that share one launch (tensor-core path) never write storage another member reads."""
     net = build(32, conv_algo=algo)
     plan = net.plan_for(1, "cpu", ops=TorchEmulOps())
@@ -80,13 +80,10 @@ def test_buffer_plan_reuses_memory_without_aliasing_live_tensors(algo):
                 for a in _views(plan.buf[t.name]):
                     for b in _views(plan.buf[y.name]):
                         assert a.data_ptr() != b.data_ptr(), (op["op"], t, y)
-    n_groups = 0
-    for kind, payload in plan.steps:
-        if kind != "conv_group":
-            continue
-        n_groups += 1
+    groups = [s.args[0] for s in plan.steps if s.name == "conv_group"]
+    for convs in groups:
         reads, writes = set(), set()
-        for cv in payload:
+        for cv in convs:
             for a in [cv["x"]] + ([cv["res"]] if cv["res"] is not None else []):
                 reads.update(v.data_ptr() for v in _views(a))
             for v in _views(cv["y"]):
@@ -95,8 +92,8 @@ def test_buffer_plan_reuses_memory_without_aliasing_live_tensors(algo):
         assert not (reads & writes), "a member of a launch writes a buffer another member reads"
     if algo == "tc":
         n_convs = sum(1 for op in g.ops if op["op"] == "conv")
-        assert n_groups < 0.5 * n_convs, (n_groups, n_convs)       # HRNet's branches share launches
-        assert max(len(p) for k, p in plan.steps if k == "conv_group") >= 4
+        assert len(groups) < 0.5 * n_convs, (len(groups), n_convs)  # HRNet's branches share launches
+        assert max(len(convs) for convs in groups) >= 4
 
 
 def test_tensor_core_plan_wiring_matches_reference_golden():
@@ -164,9 +161,9 @@ def test_in_place_parameter_edit_invalidates_cached_plans():
     assert len(net._plans) <= net.MAX_PLANS
 
 
-def test_network_program_export_is_well_formed():
+def test_exported_step_records_are_well_formed():
     """Plan.export (the input of danet_net_load, csrc/net.cu): every reference stays inside its buffer / constant, the
-    step list mirrors the plan's launch steps, the constants carry the packed weights byte for byte."""
+    step list mirrors the plan's step records, the constants carry the packed weights byte for byte."""
     from netprog_common import parse_program
     net = build(32)
     image = make_image(1, 3)
@@ -175,8 +172,8 @@ def test_network_program_export_is_well_formed():
     blob = plan.export()
     prog = parse_program(blob)
     assert prog["version"] == 1 and prog["batch"] == 1 and prog["chw"] == (3, 224, 224) and prog["precision"] == 2
-    n_expected = sum(2 if kind == "body_fc" else 1 for kind, _ in plan.steps)
-    assert len(prog["steps"]) == n_expected
+    n_expected = sum(2 if op["op"] == "body_fc" else 1 for op in plan.g.ops)       # fp32 path: one launch per op
+    assert len(prog["steps"]) == len(plan.steps) == plan.n_launch == n_expected
     for s in prog["steps"]:
         assert 1 <= s["op"] <= 12
         for (kind, rid, roff) in s["refs"]:
@@ -193,6 +190,33 @@ def test_network_program_export_is_well_formed():
     conv = [s for s in prog["steps"] if s["op"] == 3][0]
     wref = conv["refs"][1]
     coff, cbytes = prog["consts"][wref[1]]
-    first = [op for kind, op in plan.steps if kind == "conv_simt"][0]
-    assert cbytes == first["w"].numel() * 4
-    assert np.array_equal(np.frombuffer(blob, dtype=np.float32, count=first["w"].numel(), offset=coff), first["w"].reshape(-1).numpy())
+    w = [s.args[2] for s in plan.steps if s.name == "conv2d"][0]
+    assert cbytes == w.numel() * 4
+    assert np.array_equal(np.frombuffer(blob, dtype=np.float32, count=w.numel(), offset=coff), w.reshape(-1).numpy())
+
+
+# (n_i, n_f, n_r) of each fixed-size step kind, as csrc/net.cu prepare() requires them
+_FIXED_ARITY = {1: (4, 0, 4), 3: (11, 0, 5), 5: (4, 0, 6), 6: (3, 0, 4), 7: (8, 0, 9), 8: (4, 0, 5), 9: (4, 1, 6),
+                10: (4, 0, 7), 11: (3, 0, 5), 12: (11, 0, 27)}
+
+
+@pytest.mark.parametrize("algo", ["simt", "tc"])
+def test_exported_steps_have_the_arity_the_loader_requires(algo):
+    """Every step of an exported program carries the number of ints / floats / references that danet_net_load
+    accepts for its opcode (and that danet_net_run_step accepts for each Python launch)."""
+    from netprog_common import parse_program
+    net = build(32, conv_algo=algo)
+    plan = net.plan_for(2, "cpu", ops=TorchEmulOps())
+    seen = set()
+    for s in parse_program(plan.export())["steps"]:
+        op, ints, nf, nr = s["op"], s["ints"], len(s["floats"]), len(s["refs"])
+        seen.add(op)
+        if op == 2:                       # conv group: n problems of 11 descriptor ints and 11 references
+            n = ints[0]
+            assert 1 <= n <= 6 and len(ints) == 1 + 11 * n and nf == 0 and nr == 11 * n, s
+        elif op == 4:                     # fuse: n terms with one upsampling factor each, 3 references per activation
+            n = ints[4]
+            assert 1 <= n <= 4 and len(ints) == 6 + n and nf == 0 and nr == 3 * n + 3, s
+        else:
+            assert (len(ints), nf, nr) == _FIXED_ARITY[op], s
+    assert seen == set(range(1, 13)) - {3 if algo == "tc" else 2}
