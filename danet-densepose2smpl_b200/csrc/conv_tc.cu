@@ -128,16 +128,20 @@ static bool make_prob(const danet_conv_desc* d, Prob* g) {
         }
     // every parity plane is loaded with the box of the largest one (one tensor map per input plane)
     const int Hb = kTileH + tr_max - 1, Wb = kTileW + tc_max - 1;
-    // Small maps (H + pad <= 8): several images share the 16 row groups of a tile.  Image n of the tile is loaded by its
-    // own TMA box [(H + 2 pad) rows] at row offset n * (H + pad): the bottom halo of one image and the top halo of the
-    // next are the same shared-memory rows, both filled with out-of-bounds zeros.  Row groups that fall on those rows
-    // produce garbage outputs the epilogue never stores.  Needs one weight set (consecutive images share weights).
+    // Small maps: several images share the 16 row groups of a tile, each loaded by its own TMA box at row offset n * hs.
+    //   stride 1 (H + pad <= 8): box = H + 2 pad rows, hs = H + pad -- the bottom halo of one image and the top halo of
+    //     the next are the same shared-memory rows, both filled with out-of-bounds zeros;
+    //   stride 2 (Ho + tr - 1 <= 8): one box of Ho + tr - 1 rows per image and parity plane, hs = the box height.
+    // Row groups that fall outside an image's Ho output rows produce garbage outputs the epilogue never stores.  With
+    // several weight sets a tile stacks images n, n + wsets, n + 2 wsets, ...: all of them use one weight set.
     g->nstack = 1; g->hs = kTileH; g->box_h = Hb;
-    if (d->stride == 1 && d->wsets == 1 && d->H + d->pad <= kTileH / 2) {
+    if (d->stride == 1 && d->H + d->pad <= kTileH / 2) {
         g->hs = d->H + d->pad;
-        g->nstack = kTileH / g->hs;
         g->box_h = d->H + 2 * d->pad;
+    } else if (d->stride == 2 && g->Ho + tr_max - 1 <= kTileH / 2) {
+        g->hs = g->box_h = g->Ho + tr_max - 1;
     }
+    if (g->hs < kTileH) g->nstack = kTileH / g->hs;
     // swizzle width: the widest row unless the channel count is tiny
     int swb = 128;
     const int c16 = (d->Cin + 15) / 16 * 16;
@@ -170,7 +174,10 @@ static bool make_prob(const danet_conv_desc* d, Prob* g) {
     g->lseg = g->exact ? 8 : (1 << 30);
     g->blocks_per_set = (long long)g->ntn * g->nblk;
     g->tiles_w = (g->Wo + kTileW - 1) / kTileW; g->tiles_h = (g->Ho + kTileH - 1) / kTileH;
-    const long long tiles = (long long)((d->N + g->nstack - 1) / g->nstack) * g->tiles_h * g->tiles_w * g->ntn;
+    // image groups: one image each, or (stacked) wsets x ceil(images per set / nstack)
+    const long long groups = g->nstack == 1 ? d->N
+                           : (long long)d->wsets * (((d->N + d->wsets - 1) / d->wsets + g->nstack - 1) / g->nstack);
+    const long long tiles = groups * g->tiles_h * g->tiles_w * g->ntn;
     if (tiles >= (1 << 24) || g->wsets >= (1 << 16)) return false;
     if ((long long)d->N * g->Ho * g->Wo * d->Cout >= (1LL << 31) || (long long)d->N * d->H * d->W * d->Cin >= (1LL << 31)) return false;   // 32-bit element offsets
     g->tile_count = (int)tiles; g->tile_base = 0;
@@ -228,12 +235,16 @@ __device__ __forceinline__ int sched_next(uint32_t bar_full, uint32_t bar_empty,
     return tile;
 }
 
-struct TileCoord { int nt, tw, th, img; };
+// img0: the tile's first image; stacked image n is img0 + n * wsets.  ws: the tile's weight set.
+struct TileCoord { int nt, tw, th, img0, ws; };
 __device__ __forceinline__ TileCoord decode_tile(const Prob& g, int t) {
     TileCoord c;
     int r = mdiv(t, g.m_ntn); c.nt = t - r * g.ntn;
     int r2 = mdiv(r, g.m_tw); c.tw = r - r2 * g.tiles_w;
-    c.img = mdiv(r2, g.m_th); c.th = r2 - c.img * g.tiles_h;
+    const int grp = mdiv(r2, g.m_th); c.th = r2 - grp * g.tiles_h;
+    const int bg = mdiv(grp, g.m_ws);
+    c.ws = grp - bg * g.wsets;
+    c.img0 = c.ws + g.wsets * bg * g.nstack;          // = grp without stacking
     return c;
 }
 
@@ -261,24 +272,24 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
     float* m = EX ? accs + NV : accs;     // main accumulator (fast mode: the only one)
     const int Cout = P.Cout, Wo = P.Wo, Ho = P.Ho;
     const int cw = Cout - tc.nt * NT;     // channels of this N tile that exist (multiple of 8)
-    // this thread's two output pixels: tile row prow of image tc.img, or (stacked small maps) row prow % hs of image
-    // tc.img * nstack + prow / hs -- rows hs-pad.. of a stacked image are the shared zero rows (no output)
-    uint32_t eoff[2]; int boff[2]; bool ok[2];
+    // this thread's two output pixels: tile row prow of image tc.img0, or (stacked small maps) row prow % hs of image
+    // tc.img0 + (prow / hs) * wsets -- rows Ho.. of a stacked image's hs rows produce no output
+    uint32_t eoff[2]; bool ok[2];
     const int ow = tc.tw * kTileW + pcol;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int prow = prow0 + r;
-        int oh = tc.th * kTileH + prow, img = tc.img;
+        int oh = tc.th * kTileH + prow, img = tc.img0;
         bool row_ok = oh < Ho;
         if (P.nstack > 1) {
             const int n = prow / P.hs;
-            oh = prow - n * P.hs; img = tc.img * P.nstack + n;
+            oh = prow - n * P.hs; img = tc.img0 + n * P.wsets;
             row_ok = oh < Ho && n < P.nstack && img < P.N;
         }
         ok[r] = row_ok && ow < Wo;
         eoff[r] = ((uint32_t)(img * Ho + oh) * Wo + ow) * Cout + tc.nt * NT + cq;
-        boff[r] = (img - mdiv(img, P.m_ws) * P.wsets) * Cout + tc.nt * NT + cq;
     }
+    const int boff = tc.ws * Cout + tc.nt * NT + cq;
     // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
     // residual enter the sum times 2^s and the result leaves it times 2^-s -- exact in fp32
     const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
@@ -286,7 +297,7 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
     auto init_term = [&](int j, int r) {
         float2 t = make_float2(0.f, 0.f);
         if (8 * j < cw) {
-            if (P.bias) t = __ldg(reinterpret_cast<const float2*>(P.bias + boff[r] + 8 * j));
+            if (P.bias) t = __ldg(reinterpret_cast<const float2*>(P.bias + boff + 8 * j));
             if (ok[r]) {
                 if (P.res_f) {
                     const float2 q = __ldg(reinterpret_cast<const float2*>(P.res_f + eoff[r] + 8 * j));
@@ -521,8 +532,7 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
                 const Prob& P = a.p[pi];
                 const TileCoord tc = decode_tile(P, tile - P.tile_base);
                 const int h0 = tc.th * kTileH * P.stride - P.pad, w0 = tc.tw * kTileW * P.stride - P.pad;
-                const int ws = tc.img - mdiv(tc.img, P.m_ws) * P.wsets;
-                const uint8_t* src = P.wpk + kPackHeader + ((long long)ws * P.blocks_per_set + (long long)tc.nt * P.nblk) * P.b_block_bytes;
+                const uint8_t* src = P.wpk + kPackHeader + ((long long)tc.ws * P.blocks_per_set + (long long)tc.nt * P.nblk) * P.b_block_bytes;
                 int b = 0;
                 for (int c = 0; c < P.nchunks; ++c)
                     for (int slot = 0; slot < P.npa; ++slot) {
@@ -532,12 +542,12 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
                                 const uint32_t box_bytes = (uint32_t)(P.box_h * P.sbo_a[slot]);
                                 mbar_expect_tx(bar_a_full + 8 * as, box_bytes * P.nstack);
                                 for (int n = 0; n < P.nstack; ++n)       // images beyond N are out of bounds: zero rows
-                                    tma_load_4d(sA + as * a.a_slot_bytes + n * P.hs * P.sbo_a[slot], &P.tm[pl], c * P.KCH, w0, -P.pad,
-                                                tc.img * P.nstack + n, bar_a_full + 8 * as);
+                                    tma_load_4d(sA + as * a.a_slot_bytes + n * P.hs * P.sbo_a[slot], &P.tm[pl], c * P.KCH,
+                                                w0 + P.par_px[slot], h0 + P.par_py[slot], tc.img0 + n * P.wsets, bar_a_full + 8 * as);
                             } else {
                                 mbar_expect_tx(bar_a_full + 8 * as, (uint32_t)P.stage_bytes[slot]);
                                 tma_load_4d(sA + as * a.a_slot_bytes, &P.tm[pl], c * P.KCH, w0 + P.par_px[slot], h0 + P.par_py[slot],
-                                            tc.img, bar_a_full + 8 * as);
+                                            tc.img0, bar_a_full + 8 * as);
                             }
                             aph ^= 1u << as;
                             if (++as == a.na_stages) as = 0;
@@ -825,6 +835,26 @@ extern "C" int64_t danet_conv_tc_packed_bytes(const danet_conv_desc* d) {
     tc::Prob g;
     if (!d || !tc::make_prob(d, &g)) return 0;
     return tc::kPackHeader + (int64_t)d->wsets * g.blocks_per_set * g.b_block_bytes;
+}
+
+extern "C" int danet_conv_tc_geometry(const danet_conv_desc* d, int64_t* out) {
+    tc::Prob g;
+    if (!d || !out || !tc::make_prob(d, &g)) return -1;
+    int64_t ksteps = 0, taps = 0, a_bytes = 0;
+    for (int c = 0; c < g.nchunks; ++c) {
+        const int kreal = (g.Cin - c * g.KCH + 15) / 16;
+        ksteps += kreal < g.KCH / 16 ? kreal : g.KCH / 16;
+    }
+    for (int s = 0; s < g.npa; ++s) {
+        taps += g.ntap[s];
+        a_bytes += g.nstack > 1 ? (int64_t)g.nstack * g.box_h * g.sbo_a[s] : g.stage_bytes[s];
+    }
+    out[0] = tc::kTileH; out[1] = tc::kTileW; out[2] = g.tile_count; out[3] = g.nstack;
+    out[4] = g.exact ? 3 : 1;                                              // products per MAC (exact: hi*hi + hi*lo + lo*hi)
+    out[5] = (int64_t)tc::kTileH * tc::kTileW * g.NT * 16 * ksteps * taps;  // issued MACs of one product
+    out[6] = a_bytes * g.nchunks * (g.exact ? 2 : 1);                      // activation halo bytes (TMA)
+    out[7] = (int64_t)g.nblk * g.b_block_bytes;                            // weight bytes (bulk copies)
+    return 0;
 }
 
 extern "C" int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream) {

@@ -241,6 +241,10 @@ int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* subti
 int64_t danet_conv_tc_packed_bytes(const danet_conv_desc* d);
 int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
 int danet_conv_tc_supported(const danet_conv_desc* d);
+/* Host-only geometry of one problem, as the engine tiles it: out[0..7] = tile rows, tile columns, tiles, images per tile
+ * (small maps stack several), products per MAC (exact 3, fast 1), issued MACs of one product per tile, activation
+ * bytes and weight bytes copied into shared memory per tile.  -1 if the shape is not supported. */
+int danet_conv_tc_geometry(const danet_conv_desc* d, int64_t* out);
 /* danet_conv_tc_pack without host synchronisation or allocation (capturable in a CUDA graph), for weights that change
  * every optimiser step: the same packed bytes.  Header word 2 of w_packed is its scratch while it runs. */
 int danet_conv_tc_pack_async(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
