@@ -99,6 +99,7 @@ SIGNATURES = {
     "danet_conv_tc_pack": (c_int, [ctypes.POINTER(ConvDesc), c_p, c_p, c_p]),
     "danet_conv_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),
     "danet_conv_tc_geometry": (c_int, [ctypes.POINTER(ConvDesc), c_p]),
+    "danet_conv_tc_cta_geometry": (c_int, [ctypes.POINTER(ConvDesc), c_p]),
     "danet_conv_tc_group": (c_int, [c_int, ctypes.POINTER(ConvProblem), c_p]),
     "danet_conv_tc_config": (c_int, [c_int, ctypes.POINTER(ConvDesc), c_p, c_p]),
     "danet_conv_tc_pack_async": (c_int, [ctypes.POINTER(ConvDesc), c_p, c_p, c_p]),

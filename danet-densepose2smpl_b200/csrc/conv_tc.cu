@@ -9,8 +9,8 @@
 // term is 2^-22 relative): fp32-grade results from the fp16 tensor pipe, which is what lets the default path meet
 // the reference's fp32 outputs to 1e-4.  "fast" mode issues hi*hi only.
 //
-// Structure (one persistent CTA per SM, warp-specialised, up to kMaxProb independent convolutions -- e.g. the
-// parallel branches of one HRNet stage -- in ONE launch over a concatenated tile space):
+// Structure (one persistent CTA per SM, up to kMaxProb independent convolutions -- e.g. the parallel branches of one
+// HRNet stage -- in ONE launch over a concatenated tile space; fast mode's work unit is a tile, exact mode's a tile pair):
 //   A (activations): fp16 NHWC planes in HBM.  One TMA tensor-map load (cp.async.bulk.tensor.4d, SWIZZLE_128B/64B/32B,
 //       out-of-bounds zero fill = the convolution's padding, elementStrides = 2 for the parity planes of a
 //       stride-2 convolution) brings the input HALO of a tile -- (16+k-1) x (8+k-1) pixels x <= 64 channels --
@@ -19,7 +19,7 @@
 //       tap is just a different descriptor start address: an input element crosses L2->SM ~1.3x, not 9x.
 //   B (weights): pre-packed once (danet_conv_tc_pack) into the swizzled shared-memory image of every
 //       (N tile, channel chunk, parity plane, tap group[, hi/lo]) block; streamed with 1-D cp.async.bulk.
-//   MMA: two consumer warpgroups, each owning 64 of the tile's 128 output pixels (8 image rows x 8 columns), issue
+//   MMA: two consumer warpgroups per tile, each owning 64 of the tile's 128 output pixels (8 image rows x 8 columns), issue
 //       wgmma.mma_async m64nNk16 (N = the tile's output channels) with fp32 accumulators in registers.
 //       exact mode: the lo and hi weight rows are concatenated along N, so hi*[lo|hi] is ONE MMA of width 2N whose
 //       first half lands in a separate small-term accumulator; lo*hi joins the small terms.  Per weight block all
@@ -31,8 +31,11 @@
 //       bias + residual.
 //   Epilogue: each consumer thread holds 2 pixels x 2 consecutive channels per 8-channel group; ReLU, output as
 //       split-fp16 planes and/or fp32.
-//   One producer warp: a single thread runs the tile scheduler and issues every TMA / bulk copy in the order the
-//       consumers use them.
+//   Copies: one thread runs the tile scheduler and issues every TMA / bulk copy in the order the consumers use them.
+//       Fast mode (288 threads): a producer warp after the two consumer warpgroups.  Exact mode (512 threads): four
+//       consumer warpgroups, two per tile of a pair (two tiles with the same weight set and N tile, pair_coord), so one
+//       weight stream feeds 256 pixels.  A producer warp would be the 17th and cut every thread to 96 registers, so
+//       warp 0 issues the copies (one elected lane) where its warpgroup frees ring slots (produce).
 //   Launch: programmatic dependent launch; every mbarrier wait is bounded (traps instead of hanging).
 #include "common.cuh"
 #include "wgmma_f16.cuh"
@@ -40,6 +43,7 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <mutex>
+#include <type_traits>
 #include <string.h>
 #include <math.h>
 
@@ -47,15 +51,18 @@ namespace danet {
 namespace tc {
 
 constexpr int kTileH = 16, kTileW = 8;
-constexpr int kConsumers = 2;                          // consumer warpgroups: 64 pixels (8 tile rows) each
-constexpr int kWarpProd = 4 * kConsumers;              // the producer warp follows the consumer warpgroups
-constexpr int kThreads = (kWarpProd + 1) * 32;
+// Fast mode: two consumer warpgroups (64 pixels = 8 tile rows each) and a producer warp.  Exact mode: four consumer
+// warpgroups, two per tile of a tile pair, and no producer warp (warp 0 issues the copies): 16 warps x 32 lanes x 128
+// registers fill the register file, which a 17th warp would cut to 96 registers per thread.
+__host__ __device__ constexpr int kConsumersOf(int ex) { return ex ? 4 : 2; }
+__host__ __device__ constexpr int kThreadsOf(int ex) { return ex ? 4 * 4 * 32 : (4 * 2 + 1) * 32; }
+constexpr int kWarpProd = 4 * kConsumersOf(0);         // fast mode: the producer warp follows the consumer warpgroups
 constexpr int kNtMaxExact = 64, kNtMaxFast = 256;      // output channels per N tile: bounded by the register accumulators
 constexpr int kMaxAStages = 8, kMaxBStages = 8;
 constexpr int kSmemMax = 227 * 1024;                   // opt-in dynamic shared memory per CTA on sm_90
 constexpr int kSmemFixed = 2048;                       // barriers + 1024-byte alignment slack
 constexpr int kSchedDepth = 4, kSchedAhead = 2, kSchedStatic = 3;
-constexpr int kSchedConsumers = 4 * kConsumers;        // lane 0 of every consumer warp
+__host__ __device__ constexpr int kSchedConsumersOf(int ex) { return 4 * kConsumersOf(ex); }   // lane 0 of every consumer warp
 constexpr int kPackHeader = 1024;                      // packed weights start with a header: float[0] = 2^s applied to the weights, float[1] = 2^-s
 
 struct alignas(64) Prob {
@@ -88,6 +95,8 @@ struct ArgsN {
     int nprob, total_tiles, na_stages, a_slot_bytes, nb_stages, b_slot_bytes;
     unsigned* sched;                     // [2]: dynamic tile counter, finished-CTA counter (self-resetting); NULL = static round-robin
     Prob p[kMaxProb];
+    // exact mode's work unit, the tile pair: problem i owns pair indices pair_base[i] .. + pair_count[i] (pair_coord)
+    int pair_base[kMaxProb], pair_count[kMaxProb], total_pairs;
 };
 
 static unsigned long long magic40(int d) { return (1ull << 40) / (unsigned long long)d + 1ull; }
@@ -186,22 +195,44 @@ static bool make_prob(const danet_conv_desc* d, Prob* g) {
 }
 static int max_stage_bytes(const Prob& g) { int m = 0; for (int a = 0; a < g.npa; ++a) m = g.stage_bytes[a] > m ? g.stage_bytes[a] : m; return m; }
 
+// Exact mode's tile pairs (pair_coord).  The two tiles of a pair have the same weight set and N tile, so one weight
+// stream feeds both:
+//   - maps of two or more tile rows: tile rows 2q and 2q + 1 of one image group, same tile column;
+//   - maps of one tile row (small and stacked maps, the 1x1-tile maps): image groups 2q wsets + ws and (2q + 1) wsets + ws
+//     of one weight set ws, same tile column.
+// A pair without a partner (an odd number of tile rows, or of image groups per weight set) gets a second tile past the
+// map: its rows are >= Ho or its images >= N, so TMA fills its halo with zeros and it stores nothing.
+static int pair_count(const Prob& g) {
+    const int U = g.tiles_h * g.tiles_w * g.ntn;
+    const int groups = g.tile_count / U;
+    if (g.tiles_h > 1) return groups * ((g.tiles_h + 1) / 2) * g.tiles_w * g.ntn;
+    const int per_set = (groups + g.wsets - 1) / g.wsets;
+    return (per_set + 1) / 2 * g.wsets * U;
+}
+
 // ring sizes of a launch over n problems; false if they cannot fit
 static bool plan_rings(ArgsN* a) {
-    int amax = 0, bmax = 0, need_a = 2;
+    int amax = 0, bmax = 0, need_a = 2, max_a = kMaxAStages;
+    bool exact = false;
     for (int i = 0; i < a->nprob; ++i) {
         const int sb = max_stage_bytes(a->p[i]);
         amax = sb > amax ? sb : amax;
         bmax = a->p[i].b_block_bytes > bmax ? a->p[i].b_block_bytes : bmax;
-        if (a->p[i].exact) need_a = 4;
+        if (a->p[i].exact) exact = true;
     }
     a->a_slot_bytes = (amax + 1023) / 1024 * 1024;
     a->b_slot_bytes = (bmax + 1023) / 1024 * 1024;
+    if (exact) {
+        // an A slot holds the halos of both tiles of a pair.  Three slots: the current parity plane's hi and lo and one
+        // prefetch; the rest goes to weight blocks
+        a->a_slot_bytes *= 2;
+        need_a = max_a = 3;
+    }
     int nb = 3;
     int na = (kSmemMax - kSmemFixed - nb * a->b_slot_bytes) / a->a_slot_bytes;
     if (na < need_a) { nb = 2; na = (kSmemMax - kSmemFixed - nb * a->b_slot_bytes) / a->a_slot_bytes; }
     if (na < need_a) return false;
-    if (na > kMaxAStages) na = kMaxAStages;
+    if (na > max_a) na = max_a;
     // spend what is left on deeper weight prefetch
     while (nb < kMaxBStages && kSmemFixed + na * a->a_slot_bytes + (nb + 1) * a->b_slot_bytes <= kSmemMax) ++nb;
     a->na_stages = na; a->nb_stages = nb;
@@ -248,10 +279,165 @@ __device__ __forceinline__ TileCoord decode_tile(const Prob& g, int t) {
     return c;
 }
 
+// exact mode: tile h (0, 1) of pair pp (problem-relative); pair_count describes the pairing.  Pair index =
+// (outer * tiles_w + tw) * ntn + nt, outer = group * ceil(tiles_h / 2) + q (tile rows 2q, 2q + 1) or, with one tile
+// row, q * wsets + ws (image groups 2q wsets + ws, (2q + 1) wsets + ws).
+__device__ __forceinline__ TileCoord pair_coord(const Prob& g, int pp, int h) {
+    TileCoord c;
+    const int r = mdiv(pp, g.m_ntn); c.nt = pp - r * g.ntn;
+    const int outer = mdiv(r, g.m_tw); c.tw = r - outer * g.tiles_w;
+    int grp;
+    if (g.tiles_h > 1) {
+        const int th2 = (g.tiles_h + 1) >> 1;
+        grp = outer / th2;
+        c.th = 2 * (outer - grp * th2) + h;
+    } else {
+        const int q = mdiv(outer, g.m_ws);
+        grp = (2 * q + h) * g.wsets + (outer - q * g.wsets);
+        c.th = 0;
+    }
+    const int bg = mdiv(grp, g.m_ws);
+    c.ws = grp - bg * g.wsets;
+    c.img0 = c.ws + g.wsets * bg * g.nstack;          // = grp without stacking
+    return c;
+}
+
 // ring positions of one consumer warpgroup (every consumer walks the A and B rings in the producer's order)
 struct Ring { int as, bs; uint32_t aph, bph; };
+
 // shared-memory addresses of the rings and their barriers
 struct Smem { uint32_t sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty; };
+
+// barrier region (at bar_a_full): A / B ring barriers, then the tile scheduler's ring and, in exact mode, the copy cursor
+constexpr uint32_t kOffSchedFull = 512, kOffSchedEmpty = kOffSchedFull + 8 * kSchedDepth;
+constexpr uint32_t kOffSchedRing = kOffSchedFull + 16 * kSchedDepth, kOffCursor = 640, kOffPark = 768;
+
+// Exact mode's copy cursor.  Warp 0 walks the copy sequence of its CTA's tile pairs (each pair: per channel chunk and
+// parity plane, the hi and lo halos of both tiles, then the plane's weight blocks) and runs it ahead of consumption by
+// the ring depths.  Its state is a row of ints in shared memory, so that it costs no registers where warp 0 runs it,
+// between wgmmas with every accumulator live.  Every lane of warp 0 reads and writes the same values.
+enum CursorField {
+    kCurSeq, kCurPub, kCurPubEnd,        // pair being loaded, next scheduler ring entry to publish, the last one is out
+    kCurPi,                              // problem of the pair being loaded (-1: take the next pair)
+    kCurC, kCurSlot, kCurStep,           // channel chunk, parity plane, step (0, 1: halo planes hi, lo; 2..: weight blocks)
+    kCurH0, kCurH1, kCurW0,              // halo origin: rows of the pair's two tiles, columns (shared)
+    kCurImg0, kCurImg1, kCurBlk,         // first image of each tile; the pair's next weight block
+    kCurFa, kCurFb,                      // A / B ring fills issued
+    kCurRa, kCurRb,                      // A / B ring uses warpgroup 0 has released
+    kCurAs, kCurBs, kCurAph, kCurBph,    // next A / B slot and the empty-barrier phases
+    kCurFields
+};
+static_assert(kOffCursor + 4 * kCurFields <= kOffPark && kOffPark + 4 * 32 <= 1024, "barrier region layout");
+__device__ __forceinline__ int cur_get(uint32_t cur, int f) {
+    int v;
+    asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(cur + 4 * f) : "memory");
+    return v;
+}
+__device__ __forceinline__ void cur_set(uint32_t cur, int f, int v) {
+    asm volatile("st.shared.s32 [%0], %1;" ::"r"(cur + 4 * f), "r"(v) : "memory");
+}
+
+// Exact mode, warp 0 only, every lane (uniform control flow; the elected lane issues): warpgroup 0 has just released dA A
+// and dB B ring uses.  Issue the copies whose slots warpgroup 0 no longer holds, in consumption order, waiting for the
+// other warpgroups to free each slot.  Those never wait on a copy at or after the one waited for: a warpgroup frees a
+// weight block once the next block's MMAs are issued, and a halo slot at the end of its parity plane (drained), so only
+// earlier copies are needed.  Stops at the first copy whose slot warpgroup 0 still holds.
+__device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, int dB) {
+    const uint32_t cur = S.bar_a_full + kOffCursor;
+    cur_set(cur, kCurRa, cur_get(cur, kCurRa) + dA);
+    cur_set(cur, kCurRb, cur_get(cur, kCurRb) + dB);
+#pragma unroll 1
+    for (;;) {
+        if (cur_get(cur, kCurPi) < 0) {
+            // publish scheduler entries up to kSchedAhead pairs past the one loaded next, then take that one
+#pragma unroll 1
+            while (cur_get(cur, kCurPub) <= cur_get(cur, kCurSeq) + kSchedAhead && !cur_get(cur, kCurPubEnd)) {
+                const int pub = cur_get(cur, kCurPub), rs = pub & (kSchedDepth - 1);
+                mbar_wait_inl(S.bar_a_full + kOffSchedEmpty + 8 * rs, ((pub / kSchedDepth) & 1) ^ 1);
+                int t;
+                if (pub < kSchedStatic || !a.sched) t = (int)blockIdx.x + pub * (int)gridDim.x;
+                else t = __shfl_sync(0xffffffffu, atom_inc_elect(a.sched), 0) + kSchedStatic * (int)gridDim.x;
+                if (t >= a.total_pairs) { t = a.total_pairs; cur_set(cur, kCurPubEnd, 1); }
+                st_arrive_elect(S.bar_a_full + kOffSchedRing + 4 * rs, t, S.bar_a_full + kOffSchedFull + 8 * rs);
+                cur_set(cur, kCurPub, pub + 1);
+            }
+            int pair;
+            asm volatile("ld.shared.s32 %0, [%1];" : "=r"(pair)
+                         : "r"(S.bar_a_full + kOffSchedRing + 4 * (cur_get(cur, kCurSeq) & (kSchedDepth - 1))) : "memory");
+            pair = __shfl_sync(0xffffffffu, pair, 0);            // the elected lane 0 wrote it
+            if (pair >= a.total_pairs) return;
+            int pi = 0;
+            while (pair >= a.pair_base[pi] + a.pair_count[pi]) ++pi;
+            const Prob& P = a.p[pi];
+            const int pp = pair - a.pair_base[pi];
+            {
+                const TileCoord tc = pair_coord(P, pp, 0);
+                cur_set(cur, kCurH0, tc.th * kTileH * P.stride - P.pad);
+                cur_set(cur, kCurW0, tc.tw * kTileW * P.stride - P.pad);
+                cur_set(cur, kCurImg0, tc.img0);
+                cur_set(cur, kCurBlk, tc.ws * (int)P.blocks_per_set + tc.nt * P.nblk);
+            }
+            {
+                const TileCoord tc = pair_coord(P, pp, 1);
+                cur_set(cur, kCurH1, tc.th * kTileH * P.stride - P.pad);
+                cur_set(cur, kCurImg1, tc.img0);
+            }
+            cur_set(cur, kCurC, 0); cur_set(cur, kCurSlot, 0); cur_set(cur, kCurStep, 0);
+            cur_set(cur, kCurPi, pi);
+        }
+        const Prob& P = a.p[cur_get(cur, kCurPi)];
+        const int step = cur_get(cur, kCurStep);
+        if (step < 2) {
+            // the hi (step 0) or lo (step 1) halo plane of both tiles, into one A slot
+            if (cur_get(cur, kCurFa) >= cur_get(cur, kCurRa) + a.na_stages) return;
+            {
+                const int as = cur_get(cur, kCurAs);
+                mbar_wait_inl(S.bar_a_empty + 8 * as, ((cur_get(cur, kCurAph) >> as) & 1) ^ 1);
+                mbar_expect_tx_elect(S.bar_a_full + 8 * as, 2u * P.nstack * P.box_h * P.sbo_a[cur_get(cur, kCurSlot)]);
+            }
+            // box k: the first tile's nstack images, then the second tile's (rows or images beyond the map are out of
+            // bounds: zero fill).  Operands are read from the cursor right at the copy.
+#pragma unroll 1
+            for (int k = 0; k < 2 * P.nstack; ++k) {
+                const int h = k >= P.nstack ? 1 : 0, n = k - h * P.nstack, slot = cur_get(cur, kCurSlot), as = cur_get(cur, kCurAs);
+                tma_load_4d_elect(S.sA + as * a.a_slot_bytes + h * (a.a_slot_bytes >> 1) + n * P.hs * P.sbo_a[slot],
+                                  &P.tm[step], cur_get(cur, kCurC) * P.KCH, cur_get(cur, kCurW0) + P.par_px[slot],
+                                  cur_get(cur, kCurH0 + h) + P.par_py[slot], cur_get(cur, kCurImg0 + h) + n * P.wsets,
+                                  S.bar_a_full + 8 * as);
+            }
+            const int as = cur_get(cur, kCurAs);
+            cur_set(cur, kCurAph, cur_get(cur, kCurAph) ^ (1 << as));
+            cur_set(cur, kCurAs, as + 1 == a.na_stages ? 0 : as + 1);
+            cur_set(cur, kCurFa, cur_get(cur, kCurFa) + 1);
+            cur_set(cur, kCurStep, step + 1);
+        } else {
+            if (cur_get(cur, kCurFb) >= cur_get(cur, kCurRb) + a.nb_stages) return;
+            {
+                const int bs = cur_get(cur, kCurBs);
+                mbar_wait_inl(S.bar_b_empty + 8 * bs, ((cur_get(cur, kCurBph) >> bs) & 1) ^ 1);
+                const uint32_t bar = S.bar_b_full + 8 * bs;
+                mbar_expect_tx_elect(bar, (uint32_t)P.b_block_bytes);
+                bulk_g2s_elect(S.sB + bs * a.b_slot_bytes, P.wpk + kPackHeader + (long long)cur_get(cur, kCurBlk) * P.b_block_bytes,
+                               (uint32_t)P.b_block_bytes, bar);
+                cur_set(cur, kCurBph, cur_get(cur, kCurBph) ^ (1 << bs));
+                cur_set(cur, kCurBs, bs + 1 == a.nb_stages ? 0 : bs + 1);
+            }
+            cur_set(cur, kCurFb, cur_get(cur, kCurFb) + 1);
+            cur_set(cur, kCurBlk, cur_get(cur, kCurBlk) + 1);
+            const int slot = cur_get(cur, kCurSlot);
+            if (step - 1 < P.ngrp[slot]) cur_set(cur, kCurStep, step + 1);
+            else {                                            // the parity plane is complete
+                cur_set(cur, kCurStep, 0);
+                if (slot + 1 < P.npa) cur_set(cur, kCurSlot, slot + 1);
+                else {
+                    cur_set(cur, kCurSlot, 0);
+                    if (cur_get(cur, kCurC) + 1 < P.nchunks) cur_set(cur, kCurC, cur_get(cur, kCurC) + 1);
+                    else { cur_set(cur, kCurPi, -1); cur_set(cur, kCurSeq, cur_get(cur, kCurSeq) + 1); }
+                }
+            }
+        }
+    }
+}
 
 // ---------------------------------------------------------------------------------------------
 // one consumer warpgroup's share of one tile, at a compile-time N tile width
@@ -262,7 +448,10 @@ struct Smem { uint32_t sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty;
 // freed once the next block's MMAs are issued.  An exact-mode K segment close drains the chain (wait_group 0).
 template <int EX, int NT>
 __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, const TileCoord tc, const Smem S, Ring& R,
-                                             int wg, int w4, int lane, bool leader, float* accs, float* sum) {
+                                             int wg, int w4, int lane, bool leader, float* accs, float* sum,
+                                             int half = 0, bool prod = false) {
+    // exact mode: wg is the warpgroup's half of its tile, half the tile of the pair (its halo is the A slot's second
+    // half), prod marks warp 0, which issues the copies
     constexpr int NV = NT / 2;            // fp32 accumulator registers per thread and set (64 x NT warpgroup tile)
     constexpr int nj = NT / 8;            // 8-channel groups of the tile
     // accumulator fragment of m64nNk16: this thread owns tile rows prow0, prow0 + 1 at column pcol, and channels
@@ -288,6 +477,9 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
         }
         ok[r] = row_ok && ow < Wo;
         eoff[r] = ((uint32_t)(img * Ho + oh) * Wo + ow) * Cout + tc.nt * NT + cq;
+    }
+    if constexpr (EX) {                   // the second tile of a pair without a partner: images >= N store nothing
+        if (tc.img0 >= P.N) ok[0] = ok[1] = false;
     }
     const int boff = tc.ws * Cout + tc.nt * NT + cq;
     // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
@@ -323,10 +515,11 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
                 sum[4 * j + 2 * r] = t.x * wsc.x; sum[4 * j + 2 * r + 1] = t.y * wsc.x;
             }
     }
-    const int nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
-    const int kmma = P.KCH / 16;                          // K = 16 halves (32 bytes) per MMA
-    const uint32_t tap16 = P.tap_bytes >> 4;
-    const uint32_t hi16 = EX ? (NT * SWB) >> 4 : 0;       // exact: the hi weight rows follow the NT lo rows
+    using Var = std::conditional_t<EX, int, const int>;  // exact mode: warp 0 parks these while it runs the copy cursor
+    Var nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
+    Var kmma = P.KCH / 16;                                // K = 16 halves (32 bytes) per MMA
+    std::conditional_t<EX, int, const uint32_t> tap16 = P.tap_bytes >> 4;
+    std::conditional_t<EX, int, const uint32_t> hi16 = EX ? (NT * SWB) >> 4 : 0;   // exact: the hi weight rows follow the NT lo rows
     const uint64_t bd0 = make_desc(0, 8 * SWB, SWB);
     uint32_t acc = 0;
     int seg_cnt = 0;
@@ -340,9 +533,9 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
     };
     for (int c = 0; c < nchunks; ++c) {
         const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
-        const int kv = kreal < kmma ? kreal : kmma;       // K steps wholly beyond Cin are not issued
+        Var kv = kreal < kmma ? kreal : kmma;             // K steps wholly beyond Cin are not issued
         for (int slot = 0; slot < npa; ++slot) {
-            const int as_hi = R.as;
+            Var as_hi = R.as;
             mbar_wait_inl(S.bar_a_full + 8 * R.as, (R.aph >> R.as) & 1u);
             R.aph ^= 1u << R.as; if (++R.as == a.na_stages) R.as = 0;
             int as_lo = as_hi;
@@ -355,16 +548,24 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
             const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB) + ((uint32_t)(wg * 8 * P.sbo_a[slot]) >> 4);
             const uint64_t ad_hi = ad0 + ((S.sA + as_hi * a.a_slot_bytes) >> 4);
             const uint64_t ad_lo = ad0 + ((S.sA + as_lo * a.a_slot_bytes) >> 4);
-            const int ngrp = P.ngrp[slot], ntap = P.ntap[slot];
+            Var ngrp = P.ngrp[slot], ntap = P.ntap[slot];
             for (int tg = 0; tg < ngrp; ++tg) {
                 const int k0 = tg * TG;
                 const int ntk = min(TG, ntap - k0);
                 const int bs = R.bs;
                 mbar_wait_inl(S.bar_b_full + 8 * bs, (R.bph >> bs) & 1u);
                 R.bph ^= 1u << bs; if (++R.bs == a.nb_stages) R.bs = 0;
-                const uint64_t bd = bd0 + ((S.sB + bs * a.b_slot_bytes) >> 4);
+                uint64_t bd;
+                if constexpr (EX) bd = make_desc(0, 8 * SWB, SWB) + ((S.sB + bs * a.b_slot_bytes) >> 4);
+                else bd = bd0 + ((S.sB + bs * a.b_slot_bytes) >> 4);
                 wg_fence();
                 if constexpr (EX) {
+                    // the A operands: the pair's second tile is the slot's second half.  Computed here, per block,
+                    // because warp 0 parks as_hi / as_lo while it runs the copy cursor (below).
+                    const uint32_t tile_a = S.sA + half * (a.a_slot_bytes >> 1) + wg * 8 * P.sbo_a[slot];
+                    const uint64_t ad1 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB);
+                    const uint64_t ad_hi = ad1 + ((tile_a + as_hi * a.a_slot_bytes) >> 4);
+                    const uint64_t ad_lo = ad1 + ((tile_a + as_lo * a.a_slot_bytes) >> 4);
                     // hi * [lo | hi]: small terms in s, main chain in m; then lo * hi into s.  The instruction's
                     // accumulator is (s, m) in that order: ptxas keeps the wgmmas in flight only if the lo * hi
                     // accumulator s is the start of the wide one, not its second half.
@@ -406,7 +607,54 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
                     seg_cnt += ntk * kv;
                     close = (c == nchunks - 1 && slot == npa - 1 && plane_end) || seg_cnt >= P.lseg;
                 }
-                if (close) {
+                if constexpr (EX) {
+                    // A parity plane's end drains too, so that its two A slots are free before the next plane's halos
+                    // are loaded: with three A slots, that is what lets the next plane's lo halo in.  The chain goes on
+                    // (acc stays 1) unless the K segment closes, so the MMA sequence is unchanged.
+                    const int db = pend_b >= 0 ? 1 : 0;
+                    int dA = 0, dB = db;
+                    if (close || plane_end) {
+                        wg_wait_all();
+                        reg_fence<NV>(m);
+                        reg_fence<NV>(s);
+                        if (close) {
+#pragma unroll
+                            for (int j = 0; j < NV; ++j) {
+                                sum[j] += m[j];
+                                sum[j] += s[j];
+                            }
+                            acc = 0; seg_cnt = 0;
+                        }
+                        release_pending();
+                        mbar_arrive_if(S.bar_b_empty + 8 * bs, leader);
+                        mbar_arrive_if(S.bar_a_empty + 8 * as_hi, leader && plane_end);
+                        mbar_arrive_if(S.bar_a_empty + 8 * as_lo, leader && plane_end);
+                        dA = plane_end ? 2 : 0; dB = db + 1;
+                    } else {
+                        wg_wait_1();
+                        release_pending();
+                        pend_b = bs;
+                    }
+                    if (prod) {
+                        // Warp 0 runs the copy cursor.  Its loop state waits in shared memory meanwhile: with every
+                        // accumulator live, the cursor has no registers to spare otherwise.  The reloads go through a
+                        // shuffle so that ptxas still sees warp-uniform values (a loop bound it cannot prove uniform
+                        // would serialise the wgmmas).
+                        const uint32_t pk = S.bar_a_full + kOffPark;
+                        int* const v[] = {&c, &slot, &tg, &kv, &ngrp, &ntap, &as_hi, &as_lo, &seg_cnt, &pend_b, &R.as, &R.bs,
+                                          &nchunks, &npa, &TG, &SWB, &kmma, &tap16, &hi16};
+                        constexpr int nv = sizeof(v) / sizeof(v[0]);
+#pragma unroll
+                        for (int i = 0; i < nv; ++i) cur_set(pk, i, *v[i]);
+                        cur_set(pk, nv, (int)acc); cur_set(pk, nv + 1, (int)R.aph); cur_set(pk, nv + 2, (int)R.bph);
+                        produce(a, S, dA, dB);
+#pragma unroll
+                        for (int i = 0; i < nv; ++i) *v[i] = __shfl_sync(0xffffffffu, cur_get(pk, i), 0);
+                        acc = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv), 0);
+                        R.aph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 1), 0);
+                        R.bph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 2), 0);
+                    }
+                } else if (close) {
                     // close the K segment: the whole chain must have landed
                     wg_wait_all();
                     reg_fence<NV>(m);
@@ -475,7 +723,7 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
 // ---------------------------------------------------------------------------------------------
 // EX: precision mode fixed at compile time (1: every problem of the launch is exact, 0: every problem is fast).
 template <int EX>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreadsOf(EX), 1)
 k_conv_tc(const __grid_constant__ ArgsN a) {
     constexpr int NTMAX = EX ? kNtMaxExact : kNtMaxFast;
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -488,22 +736,55 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
     const uint32_t bar_b_full = sBar + 16 * kMaxAStages, bar_b_empty = bar_b_full + 8 * kMaxBStages;
     // dynamic tile scheduler: a ring of kSchedDepth tile indices published by the producer (it takes them from a
     // global atomic counter, heaviest problems first) and read by the consumer warps
-    const uint32_t bar_sched_full = sBar + 512, bar_sched_empty = sBar + 512 + 8 * kSchedDepth, sched_ring = sBar + 512 + 16 * kSchedDepth;
+    const uint32_t bar_sched_full = sBar + kOffSchedFull, bar_sched_empty = sBar + kOffSchedEmpty, sched_ring = sBar + kOffSchedRing;
+    constexpr int kCons = kConsumersOf(EX);
 
     // the warp index through a shuffle: ptxas then knows it is warp-uniform, and so is every branch on the warp role
     // (a role branch it cannot prove uniform makes it serialise the wgmmas behind it)
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < a.na_stages; ++i) { mbar_init(bar_a_full + 8 * i, 1); mbar_init(bar_a_empty + 8 * i, kConsumers); }
-        for (int i = 0; i < a.nb_stages; ++i) { mbar_init(bar_b_full + 8 * i, 1); mbar_init(bar_b_empty + 8 * i, kConsumers); }
-        for (int i = 0; i < kSchedDepth; ++i) { mbar_init(bar_sched_full + 8 * i, 1); mbar_init(bar_sched_empty + 8 * i, kSchedConsumers); }
+        for (int i = 0; i < a.na_stages; ++i) { mbar_init(bar_a_full + 8 * i, 1); mbar_init(bar_a_empty + 8 * i, kCons); }
+        for (int i = 0; i < a.nb_stages; ++i) { mbar_init(bar_b_full + 8 * i, 1); mbar_init(bar_b_empty + 8 * i, kCons); }
+        for (int i = 0; i < kSchedDepth; ++i) { mbar_init(bar_sched_full + 8 * i, 1); mbar_init(bar_sched_empty + 8 * i, kSchedConsumersOf(EX)); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        if constexpr (EX)
+            for (int f = 0; f < kCurFields; ++f) cur_set(sBar + kOffCursor, f, f == kCurPi ? -1 : 0);
     }
-    if (warp == kWarpProd && lane < a.nprob) { tma_prefetch_desc(&a.p[lane].tm[0]); if (EX) tma_prefetch_desc(&a.p[lane].tm[1]); }
+    if (warp == (EX ? 0 : kWarpProd) && lane < a.nprob) { tma_prefetch_desc(&a.p[lane].tm[0]); if (EX) tma_prefetch_desc(&a.p[lane].tm[1]); }
     __syncthreads();
     pdl_launch_dependents();            // the next launch may fill SMs as our CTAs retire
 
-    if (warp == kWarpProd) {
+    if constexpr (EX) {
+        // ================= exact mode: four consumer warpgroups over tile pairs; warp 0 also issues every copy =================
+        const int wg = warp >> 2, w4 = warp & 3;
+        const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
+        const bool prod = warp == 0;
+        const Smem S = {sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty};
+        Ring R = {0, 0, 0u, 0u};
+        constexpr int NVMAX = NTMAX / 2;
+        float accs[2 * NVMAX];                 // small terms then main chain
+        float sum[NVMAX];                      // bias + residual + every closed K segment, fp32 round-to-nearest
+        pdl_wait();                            // activations come from the previous kernel; residual reads / output writes
+        if (prod) produce(a, S, 0, 0);         // the first copies and scheduler entries
+        for (int seq = 0;; ++seq) {
+            int pair = 0;
+            if (lane == 0) pair = sched_next(bar_sched_full, bar_sched_empty, sched_ring, seq);
+            pair = __shfl_sync(0xffffffffu, pair, 0);
+            if (pair >= a.total_pairs) break;
+            int pi = 0;
+            while (pair >= a.pair_base[pi] + a.pair_count[pi]) ++pi;
+            const Prob& P = a.p[pi];
+            // warpgroups 0, 1 take the pair's first tile, 2, 3 the second (the same tile of the next image group)
+            const int half = wg >> 1;
+            const TileCoord tc = pair_coord(P, pair - a.pair_base[pi], half);
+#define DANET_NT_CASE(N) case N: consume_tile<EX, N>(a, P, tc, S, R, wg & 1, w4, lane, leader, accs, sum, half, prod); break;
+            switch (P.NT) {
+                DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64)
+                default: __trap();
+            }
+#undef DANET_NT_CASE
+        }
+    } else if (warp == kWarpProd) {
         // ================= producer: tile scheduler + every TMA / bulk copy, in consumption order =================
         if (lane == 0) {
             int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
@@ -783,8 +1064,11 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         else P.tm[1] = P.tm[0];
         P.tile_base = base; base += P.tile_count;
         DANET_CHECK(base < (1 << 24), "danet_conv_tc_group: too many tiles");
+        a.pair_base[i] = a.total_pairs; a.total_pairs += pair_count(P);
+        a.pair_count[i] = a.total_pairs - a.pair_base[i];
     }
     a.total_tiles = base;
+    const int units = a.p[0].exact ? a.total_pairs : a.total_tiles;          // scheduled work units: tile pairs or tiles
     int dev = 0;
     DANET_CUDA(cudaGetDevice(&dev));
     DANET_CHECK(dev >= 0 && dev < 64, "conv_tc: device ordinal %d out of range", dev);
@@ -802,9 +1086,9 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
     }
     const int smem_bytes = kSmemFixed + a.na_stages * a.a_slot_bytes + a.nb_stages * a.b_slot_bytes;
     const int cap = g_sm_count[dev];
-    const int grid = a.total_tiles < cap ? a.total_tiles : cap;
+    const int grid = units < cap ? units : cap;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads);
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreadsOf(a.p[0].exact));
     cfg.dynamicSmemBytes = smem_bytes;
     cfg.stream = stream;
     cudaLaunchAttribute at[1];
@@ -854,6 +1138,19 @@ extern "C" int danet_conv_tc_geometry(const danet_conv_desc* d, int64_t* out) {
     out[5] = (int64_t)tc::kTileH * tc::kTileW * g.NT * 16 * ksteps * taps;  // issued MACs of one product
     out[6] = a_bytes * g.nchunks * (g.exact ? 2 : 1);                      // activation halo bytes (TMA)
     out[7] = (int64_t)g.nblk * g.b_block_bytes;                            // weight bytes (bulk copies)
+    return 0;
+}
+
+extern "C" int danet_conv_tc_cta_geometry(const danet_conv_desc* d, int64_t* out) {
+    int64_t t[8];
+    if (danet_conv_tc_geometry(d, t) != 0) return -1;
+    tc::Prob g;
+    tc::make_prob(d, &g);
+    const int tiles = g.exact ? 2 : 1;                  // exact mode: a tile pair shares one weight stream
+    out[0] = tiles;
+    out[1] = g.exact ? tc::pair_count(g) : g.tile_count;
+    out[2] = t[7];
+    out[3] = t[6] * tiles;
     return 0;
 }
 

@@ -46,6 +46,34 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm,
     asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
                  ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
 }
+// Elected forms: the whole (converged) warp executes them and one lane, the lowest, issues the operation.  The exact-mode
+// conv engine issues its copies from inside a consumer warp, where an `if (lane == 0)` branch would serialise its wgmmas.
+__device__ __forceinline__ void mbar_expect_tx_elect(uint32_t bar, uint32_t bytes) {
+    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\t@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}"
+                 ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_g2s_elect(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\t"
+                 "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d_elect(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3, uint32_t bar) {
+    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\t"
+                 "@p cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];\n\t}"
+                 ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
+}
+// st.shared of v at addr, then mbarrier.arrive on bar, both by the elected lane (the arrive releases the store)
+__device__ __forceinline__ void st_arrive_elect(uint32_t addr, int v, uint32_t bar) {
+    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\t@p st.shared.s32 [%0], %1;\n\t"
+                 "@p mbarrier.arrive.shared::cta.b64 _, [%2];\n\t}" ::"r"(addr), "r"(v), "r"(bar) : "memory");
+}
+// atomicAdd(ctr, 1) by the elected lane (lane 0 of a converged warp); the other lanes get 0
+__device__ __forceinline__ int atom_inc_elect(unsigned* ctr) {
+    int v = 0;
+    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\t@p atom.global.add.u32 %0, [%1], 1;\n\t}"
+                 : "+r"(v) : "l"(ctr) : "memory");
+    return v;
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }

@@ -245,6 +245,10 @@ int danet_conv_tc_supported(const danet_conv_desc* d);
  * (small maps stack several), products per MAC (exact 3, fast 1), issued MACs of one product per tile, activation
  * bytes and weight bytes copied into shared memory per tile.  -1 if the shape is not supported. */
 int danet_conv_tc_geometry(const danet_conv_desc* d, int64_t* out);
+/* Host-only geometry of the engine's CTA work unit (exact mode: a pair of tiles that share one weight stream; fast mode:
+ * one tile): out[0..3] = tiles per work unit, work units, weight bytes and activation bytes copied into shared memory
+ * per work unit.  -1 if the shape is not supported. */
+int danet_conv_tc_cta_geometry(const danet_conv_desc* d, int64_t* out);
 /* danet_conv_tc_pack without host synchronisation or allocation (capturable in a CUDA graph), for weights that change
  * every optimiser step: the same packed bytes.  Header word 2 of w_packed is its scratch while it runs. */
 int danet_conv_tc_pack_async(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
