@@ -113,6 +113,11 @@ SIGNATURES = {
                                  c_p, c_p]),
     "danet_conv_bias_grad_workspace_bytes": (c_i64, [c_int, c_int, c_int]),
     "danet_conv_bias_grad": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
+    "danet_bn2d_workspace_bytes": (c_i64, [c_int, c_int, c_int]),
+    "danet_bn2d_forward": (c_int, [c_int, c_int, c_int] + [c_p] * 5 + [c_int, c_f, c_f, c_p, c_int] + [c_p] * 5),
+    "danet_bn2d_backward": (c_int, [c_int, c_int, c_int] + [c_p] * 5 + [c_int, c_int] + [c_p] * 6),
+    "danet_maxpool3x3s2_nchw_forward": (c_int, [c_int] * 4 + [c_p] * 4),
+    "danet_maxpool3x3s2_nchw_backward": (c_int, [c_int] * 4 + [c_p] * 4),
     "danet_act_split": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_act_merge": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_nchw_to_nhwc": (c_int, [c_int, c_int, c_int, c_int, c_p, ctypes.POINTER(Act), c_p]),

@@ -1,0 +1,339 @@
+// BatchNorm2d in training and eval mode with its backward, and the 3x3 / stride 2 / padding 1 max pool with its
+// backward, on fp32 NCHW tensors: the layers of the regressor's ResNet blocks (res_module.py:27-61,393-448) that train
+// around the differentiable convolution (conv.py).  No float atomics and no host synchronisation: every result repeats
+// bit for bit and the calls can be captured in a CUDA graph.
+//
+// BatchNorm (x [N][C][HW], n = N * HW values per channel):
+//   Statistics.  Training mode sums x and x * x per channel in double (chan_sums_partial: (channel, image chunk)
+//       partials with a fixed thread assignment and tree); k_bn2d_stats_finish adds the chunks in order and writes
+//       mean, invstd = 1 / sqrt(biased var + eps) and the new running statistics (momentum, unbiased variance
+//       n / (n - 1)).  Eval mode uses the running statistics.  save [2][C] (double) keeps mean and invstd for the
+//       backward.
+//   Apply.  y = ((x - m_hi) - m_lo) * (w * invstd) + b (+ r), then ReLU: the mean as an fp32 pair (hi + lo) is
+//       subtracted before scaling, so |mean| >> std does not cancel away the deviation.
+//   Backward.  dz = dy masked by y > 0 with ReLU (threshold_backward on the output).  One reduction gives sum dz and
+//       sum dz * (x - mean) in double; dbias = sum dz, dweight = invstd * sum dz (x - mean).  One apply pass writes
+//       dx = w invstd (dz - sum dz / n - xhat * sum dz xhat / n) (training) or w invstd dz (eval), and dresidual = dz.
+//   The apply passes run over the flat tensor in float4 groups; a group that straddles two (n, c) planes (planes of
+//       49 or 2 elements) looks up each element's channel.
+//
+// Max pool: the forward stores per output the window slot (0..8, row-major) of its maximum: the first maximum wins,
+// and NaN wins over numbers (torch's rule, so the slots equal its indices).  The backward is a gather: an input pixel
+// adds, in row-major window order, the dy of the windows (at most four) whose slot points at it.
+#include "common.cuh"
+#include <math.h>
+
+namespace danet {
+namespace bn {
+
+constexpr int kThreads = 256;
+constexpr int kCoef = 8;                         // floats of per-channel apply coefficients
+
+// workspace: chunk partials [2][nchunk][C] (double), then coefficients [C][kCoef] (float)
+static int64_t part_bytes(int N, int C, int HW) { return align_up((int64_t)2 * chan_sums_chunks(N, HW) * C * 8, 256); }
+static int64_t ws_bytes(int N, int C, int HW) { return part_bytes(N, C, HW) + (int64_t)C * kCoef * 4; }
+
+// double -> fp32 pair hi + lo
+__device__ __forceinline__ void split_f(double v, float* hi, float* lo) {
+    *hi = (float)v;
+    *lo = (float)(v - (double)*hi);
+}
+
+// Training: chunks of sum x and sum x^2 in order -> save (mean, invstd), the forward coefficients
+// {m_hi, m_lo, w * invstd, b} and new_running [2][C] (mean, unbiased variance).  Eval: the running statistics.
+__global__ void k_bn2d_stats_finish(const double* __restrict__ part, int nchunk, int C, long long n, int training,
+                                    const float* __restrict__ w, const float* __restrict__ b, const float* __restrict__ rm,
+                                    const float* __restrict__ rv, float momentum, float eps, double* __restrict__ save,
+                                    float* __restrict__ coef, float* __restrict__ new_running) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double mean, invstd;
+    if (training) {
+        double s1 = 0.0, s2 = 0.0;
+        for (int j = 0; j < nchunk; ++j) s1 += part[(size_t)j * C + c];
+        for (int j = 0; j < nchunk; ++j) s2 += part[((size_t)nchunk + j) * C + c];
+        mean = s1 / (double)n;
+        const double var = fmax(s2 / (double)n - mean * mean, 0.0);
+        invstd = 1.0 / sqrt(var + (double)eps);
+        if (new_running) {
+            const double m = (double)momentum;
+            new_running[c] = (float)((1.0 - m) * (double)rm[c] + m * mean);
+            new_running[C + c] = (float)((1.0 - m) * (double)rv[c] + m * var * ((double)n / (double)(n - 1)));
+        }
+    } else {
+        mean = (double)rm[c];
+        invstd = 1.0 / sqrt((double)rv[c] + (double)eps);
+    }
+    save[c] = mean;
+    save[C + c] = invstd;
+    float* k = coef + (size_t)c * kCoef;
+    split_f(mean, &k[0], &k[1]);
+    k[2] = (float)((double)w[c] * invstd);
+    k[3] = b[c];
+}
+
+// Backward: chunks of sum dz and sum dz (x - mean) in order -> dbias, dweight and the dx coefficients
+// {m_hi, m_lo, c1 = sum dz / n, c2 = invstd^2 sum dz (x - mean) / n, w * invstd}
+__global__ void k_bn2d_grad_finish(const double* __restrict__ part, int nchunk, int C, long long n, int training,
+                                   const float* __restrict__ w, const double* __restrict__ save, float* __restrict__ dweight,
+                                   float* __restrict__ dbias, float* __restrict__ coef) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double s1 = 0.0, s2 = 0.0;
+    for (int j = 0; j < nchunk; ++j) s1 += part[(size_t)j * C + c];
+    for (int j = 0; j < nchunk; ++j) s2 += part[((size_t)nchunk + j) * C + c];
+    const double mean = save[c], invstd = save[C + c];
+    if (dbias) dbias[c] = (float)s1;
+    if (dweight) dweight[c] = (float)(s2 * invstd);
+    float* k = coef + (size_t)c * kCoef;
+    split_f(mean, &k[0], &k[1]);
+    k[2] = training ? (float)(s1 / (double)n) : 0.0f;
+    k[3] = training ? (float)(s2 * invstd * invstd / (double)n) : 0.0f;
+    k[4] = (float)((double)w[c] * invstd);
+}
+
+// Eval-mode backward without weight / bias gradients needs no sums: only w * invstd
+__global__ void k_bn2d_eval_coef(int C, const float* __restrict__ w, const double* __restrict__ save, float* __restrict__ coef) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    float* k = coef + (size_t)c * kCoef;
+    k[0] = k[1] = k[2] = k[3] = 0.0f;
+    k[4] = (float)((double)w[c] * save[C + c]);
+}
+
+// channel of flat element e of [N][C][HW]
+__device__ __forceinline__ int chan_of(long long e, int HW, int C) { return (int)((e / HW) % C); }
+
+struct FwdArgs { const float* x; const float* r; const float* coef; float* y; long long total; int HW, C, relu, vec; };
+
+__device__ __forceinline__ float bn_fwd1(const FwdArgs& a, float x, float r, int c) {
+    const float4 k = __ldg(reinterpret_cast<const float4*>(a.coef + (size_t)c * kCoef));
+    float v = ((x - k.x) - k.y) * k.z + k.w;
+    if (a.r) v += r;
+    if (a.relu) v = fmaxf(v, 0.0f);
+    return v;
+}
+
+__global__ void __launch_bounds__(kThreads) k_bn2d_apply(const FwdArgs a) {
+    const long long e = 4 * ((long long)blockIdx.x * kThreads + threadIdx.x);
+    if (e >= a.total) return;
+    if (a.vec && e + 3 < a.total) {
+        const float4 x = __ldg(reinterpret_cast<const float4*>(a.x + e));
+        const float4 r = a.r ? __ldg(reinterpret_cast<const float4*>(a.r + e)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const long long p = e / a.HW;
+        const int q = (int)(e - p * a.HW);
+        float4 y;
+        if (q + 3 < a.HW) {                          // one plane: one channel
+            const int c = (int)(p % a.C);
+            y.x = bn_fwd1(a, x.x, r.x, c); y.y = bn_fwd1(a, x.y, r.y, c);
+            y.z = bn_fwd1(a, x.z, r.z, c); y.w = bn_fwd1(a, x.w, r.w, c);
+        } else {
+            y.x = bn_fwd1(a, x.x, r.x, chan_of(e, a.HW, a.C)); y.y = bn_fwd1(a, x.y, r.y, chan_of(e + 1, a.HW, a.C));
+            y.z = bn_fwd1(a, x.z, r.z, chan_of(e + 2, a.HW, a.C)); y.w = bn_fwd1(a, x.w, r.w, chan_of(e + 3, a.HW, a.C));
+        }
+        *reinterpret_cast<float4*>(a.y + e) = y;
+        return;
+    }
+    for (long long i = e; i < e + 4 && i < a.total; ++i)
+        a.y[i] = bn_fwd1(a, __ldg(a.x + i), a.r ? __ldg(a.r + i) : 0.0f, chan_of(i, a.HW, a.C));
+}
+
+struct BwdArgs {
+    const float* dy; const float* y; const float* x; const float* coef; float* dx; float* dres;
+    long long total; int HW, C, training, vec;
+};
+
+// dz, and dx when a.dx is set
+__device__ __forceinline__ float bn_bwd1(const BwdArgs& a, float dy, float y, float x, int c, float* dx) {
+    const float dz = (a.y && !(y > 0.0f)) ? 0.0f : dy;
+    if (a.dx) {
+        const float* k = a.coef + (size_t)c * kCoef;
+        const float kk = __ldg(k + 4);
+        if (a.training) {
+            const float4 m = __ldg(reinterpret_cast<const float4*>(k));
+            *dx = (dz - m.z - ((x - m.x) - m.y) * m.w) * kk;
+        } else {
+            *dx = dz * kk;
+        }
+    }
+    return dz;
+}
+
+__global__ void __launch_bounds__(kThreads) k_bn2d_bwd_apply(const BwdArgs a) {
+    const long long e = 4 * ((long long)blockIdx.x * kThreads + threadIdx.x);
+    if (e >= a.total) return;
+    const bool need_x = a.dx && a.training;
+    if (a.vec && e + 3 < a.total) {
+        const float4 dy = __ldg(reinterpret_cast<const float4*>(a.dy + e));
+        const float4 y = a.y ? __ldg(reinterpret_cast<const float4*>(a.y + e)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float4 x = need_x ? __ldg(reinterpret_cast<const float4*>(a.x + e)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const long long p = e / a.HW;
+        const int q = (int)(e - p * a.HW);
+        int c0, c1, c2, c3;
+        if (q + 3 < a.HW) {
+            c0 = c1 = c2 = c3 = (int)(p % a.C);
+        } else {
+            c0 = chan_of(e, a.HW, a.C); c1 = chan_of(e + 1, a.HW, a.C);
+            c2 = chan_of(e + 2, a.HW, a.C); c3 = chan_of(e + 3, a.HW, a.C);
+        }
+        float4 dz, dx;
+        dz.x = bn_bwd1(a, dy.x, y.x, x.x, c0, &dx.x); dz.y = bn_bwd1(a, dy.y, y.y, x.y, c1, &dx.y);
+        dz.z = bn_bwd1(a, dy.z, y.z, x.z, c2, &dx.z); dz.w = bn_bwd1(a, dy.w, y.w, x.w, c3, &dx.w);
+        if (a.dx) *reinterpret_cast<float4*>(a.dx + e) = dx;
+        if (a.dres) *reinterpret_cast<float4*>(a.dres + e) = dz;
+        return;
+    }
+    for (long long i = e; i < e + 4 && i < a.total; ++i) {
+        float dx = 0.0f;
+        const float dz = bn_bwd1(a, __ldg(a.dy + i), a.y ? __ldg(a.y + i) : 0.0f, need_x ? __ldg(a.x + i) : 0.0f,
+                                 chan_of(i, a.HW, a.C), &dx);
+        if (a.dx) a.dx[i] = dx;
+        if (a.dres) a.dres[i] = dz;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// max pool 3x3 / stride 2 / padding 1, NCHW
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads)
+k_maxpool3x3s2_fwd(long long total, int H, int W, int Ho, int Wo, const float* __restrict__ x, float* __restrict__ y,
+                   uint8_t* __restrict__ slot) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= total) return;
+    const long long p = i / ((long long)Ho * Wo);
+    const int r = (int)(i - p * Ho * Wo), oh = r / Wo, ow = r - oh * Wo;
+    const float* xp = x + p * H * W;
+    const int h0 = 2 * oh - 1, w0 = 2 * ow - 1;
+    const int hs = max(h0, 0), he = min(h0 + 3, H), ws = max(w0, 0), we = min(w0 + 3, W);
+    float m = -INFINITY;
+    int best = (hs - h0) * 3 + (ws - w0);
+    for (int h = hs; h < he; ++h)
+        for (int w = ws; w < we; ++w) {
+            const float v = __ldg(xp + h * W + w);
+            if (v > m || isnan(v)) { m = v; best = (h - h0) * 3 + (w - w0); }
+        }
+    y[i] = m;
+    slot[i] = (uint8_t)best;
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_maxpool3x3s2_bwd(long long total, int H, int W, int Ho, int Wo, const float* __restrict__ dy,
+                   const uint8_t* __restrict__ slot, float* __restrict__ dx) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= total) return;
+    const long long p = i / ((long long)H * W);
+    const int r = (int)(i - p * H * W), h = r / W, w = r - h * W;
+    const size_t base = (size_t)p * Ho * Wo;
+    float acc = 0.0f;
+    // windows oh with 2 oh - 1 <= h <= 2 oh + 1, in row-major order
+    for (int oh = h >> 1; oh <= min((h + 1) >> 1, Ho - 1); ++oh)
+        for (int ow = w >> 1; ow <= min((w + 1) >> 1, Wo - 1); ++ow) {
+            const size_t o = base + (size_t)oh * Wo + ow;
+            const int s = __ldg(slot + o);
+            if (2 * oh - 1 + s / 3 == h && 2 * ow - 1 + s % 3 == w) acc += __ldg(dy + o);
+        }
+    dx[i] = acc;
+}
+
+static unsigned grid_of(long long work) { return (unsigned)((work + kThreads - 1) / kThreads); }
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+}  // namespace bn
+}  // namespace danet
+
+using namespace danet;
+
+static bool bn_shape_ok(int32_t N, int32_t C, int32_t HW) {
+    return N >= 1 && C >= 1 && HW >= 1 && (long long)N * C * HW < (1LL << 31) && chan_sums_chunks(N, HW) < 65536;
+}
+
+extern "C" int64_t danet_bn2d_workspace_bytes(int32_t N, int32_t C, int32_t HW) {
+    if (!bn_shape_ok(N, C, HW)) return 0;
+    return bn::ws_bytes(N, C, HW);
+}
+
+extern "C" int danet_bn2d_forward(int32_t N, int32_t C, int32_t HW, const float* x, const float* weight, const float* bias,
+                                  const float* running_mean, const float* running_var, int32_t training, float momentum,
+                                  float eps, const float* residual, int32_t relu, float* y, double* save, float* new_running,
+                                  void* workspace, danet_stream_t stream) {
+    DANET_CHECK(bn_shape_ok(N, C, HW), "danet_bn2d_forward: bad sizes N=%d C=%d HW=%d", N, C, HW);
+    DANET_CHECK(x && y && weight && bias && running_mean && running_var && save,
+                "danet_bn2d_forward: x, y, weight, bias, running statistics and save must be non-null");
+    DANET_CHECK(workspace && ((uintptr_t)workspace & 15) == 0, "danet_bn2d_forward: workspace must be non-null and 16-byte aligned");
+    DANET_CHECK(!training || (long long)N * HW > 1, "danet_bn2d_forward: training needs more than one value per channel");
+    cudaStream_t st = (cudaStream_t)stream;
+    double* part = (double*)workspace;
+    float* coef = (float*)((char*)workspace + bn::part_bytes(N, C, HW));
+    if (training) {
+        const ChanSums s = {x, nullptr, x, nullptr};
+        if (chan_sums_partial(s, true, N, C, HW, part, st) != 0) return -3;
+    }
+    bn::k_bn2d_stats_finish<<<cdiv(C, 128), 128, 0, st>>>(part, chan_sums_chunks(N, HW), C, (long long)N * HW, training,
+                                                          weight, bias, running_mean, running_var, momentum, eps, save, coef,
+                                                          training ? new_running : nullptr);
+    bn::FwdArgs a;
+    a.x = x; a.r = residual; a.coef = coef; a.y = y; a.total = (long long)N * C * HW; a.HW = HW; a.C = C; a.relu = relu != 0;
+    a.vec = bn::aligned16(x) && bn::aligned16(y) && (!residual || bn::aligned16(residual));
+    bn::k_bn2d_apply<<<bn::grid_of((a.total + 3) / 4), bn::kThreads, 0, st>>>(a);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int danet_bn2d_backward(int32_t N, int32_t C, int32_t HW, const float* x, const float* y, const float* dy,
+                                   const float* weight, const double* save, int32_t training, int32_t relu, float* dx,
+                                   float* dweight, float* dbias, float* dresidual, void* workspace, danet_stream_t stream) {
+    DANET_CHECK(bn_shape_ok(N, C, HW), "danet_bn2d_backward: bad sizes N=%d C=%d HW=%d", N, C, HW);
+    DANET_CHECK(x && dy && weight && save, "danet_bn2d_backward: x, dy, weight and save must be non-null");
+    DANET_CHECK(!relu || y, "danet_bn2d_backward: relu needs the forward's output y");
+    DANET_CHECK(workspace && ((uintptr_t)workspace & 15) == 0, "danet_bn2d_backward: workspace must be non-null and 16-byte aligned");
+    DANET_CHECK(!training || (long long)N * HW > 1, "danet_bn2d_backward: training needs more than one value per channel");
+    cudaStream_t st = (cudaStream_t)stream;
+    double* part = (double*)workspace;
+    float* coef = (float*)((char*)workspace + bn::part_bytes(N, C, HW));
+    const float* mask = relu ? y : nullptr;
+    const bool sums = dweight || dbias || (dx && training);
+    if (sums) {
+        const ChanSums s = {dy, mask, x, save};
+        if (chan_sums_partial(s, true, N, C, HW, part, st) != 0) return -3;
+        bn::k_bn2d_grad_finish<<<cdiv(C, 128), 128, 0, st>>>(part, chan_sums_chunks(N, HW), C, (long long)N * HW, training,
+                                                             weight, save, dweight, dbias, coef);
+    } else if (dx) {
+        bn::k_bn2d_eval_coef<<<cdiv(C, 128), 128, 0, st>>>(C, weight, save, coef);
+    }
+    if (dx || dresidual) {
+        bn::BwdArgs a;
+        a.dy = dy; a.y = mask; a.x = x; a.coef = coef; a.dx = dx; a.dres = dresidual;
+        a.total = (long long)N * C * HW; a.HW = HW; a.C = C; a.training = training != 0;
+        a.vec = bn::aligned16(dy) && bn::aligned16(x) && (!mask || bn::aligned16(mask)) && (!dx || bn::aligned16(dx)) &&
+                (!dresidual || bn::aligned16(dresidual));
+        bn::k_bn2d_bwd_apply<<<bn::grid_of((a.total + 3) / 4), bn::kThreads, 0, st>>>(a);
+    }
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+static bool pool_shape_ok(int32_t N, int32_t C, int32_t H, int32_t W) {
+    return N >= 1 && C >= 1 && H >= 1 && W >= 1 && (long long)N * C * H * W < (1LL << 31);
+}
+
+extern "C" int danet_maxpool3x3s2_nchw_forward(int32_t N, int32_t C, int32_t H, int32_t W, const float* x, float* y,
+                                               uint8_t* slot, danet_stream_t stream) {
+    DANET_CHECK(pool_shape_ok(N, C, H, W), "danet_maxpool3x3s2_nchw_forward: bad sizes N=%d C=%d H=%d W=%d", N, C, H, W);
+    DANET_CHECK(x && y && slot, "danet_maxpool3x3s2_nchw_forward: x, y and slot must be non-null");
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    const long long total = (long long)N * C * Ho * Wo;
+    bn::k_maxpool3x3s2_fwd<<<bn::grid_of(total), bn::kThreads, 0, (cudaStream_t)stream>>>(total, H, W, Ho, Wo, x, y, slot);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int danet_maxpool3x3s2_nchw_backward(int32_t N, int32_t C, int32_t H, int32_t W, const float* dy,
+                                                const uint8_t* slot, float* dx, danet_stream_t stream) {
+    DANET_CHECK(pool_shape_ok(N, C, H, W), "danet_maxpool3x3s2_nchw_backward: bad sizes N=%d C=%d H=%d W=%d", N, C, H, W);
+    DANET_CHECK(dy && slot && dx, "danet_maxpool3x3s2_nchw_backward: dy, slot and dx must be non-null");
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    const long long total = (long long)N * C * H * W;
+    bn::k_maxpool3x3s2_bwd<<<bn::grid_of(total), bn::kThreads, 0, (cudaStream_t)stream>>>(total, H, W, Ho, Wo, dy, slot, dx);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}

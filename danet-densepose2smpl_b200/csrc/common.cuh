@@ -155,4 +155,11 @@ __device__ __forceinline__ void act_st1(const ActV& a, size_t e, float v) {
 }
 static inline bool act_any(const danet_act* a) { return a && (a->f32 || a->hi); }
 
+// Fixed-order per-channel sums of an fp32 NCHW tensor [N][C][HW] in double (conv_wgrad.cu, k_db_partial): sum 0 =
+// sum of a (counted only where mask > 0 when mask is given); with `two`, sum 1 = sum of a * (b - b_shift[c]) (b_shift
+// may be NULL).  part receives [two ? 2 : 1][chan_sums_chunks(N, HW)][C] chunk partials, to be added in chunk order.
+struct ChanSums { const float* a; const float* mask; const float* b; const double* b_shift; };
+int chan_sums_chunks(int N, int HW);
+int chan_sums_partial(const ChanSums& s, bool two, int N, int C, int HW, double* part, cudaStream_t st);
+
 }  // namespace danet

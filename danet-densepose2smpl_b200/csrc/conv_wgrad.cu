@@ -229,28 +229,44 @@ __global__ void k_wgrad_finish(const float* __restrict__ part, int nchunk, int w
     dW[i] = (float)acc;
 }
 
-// db from the fp32 NCHW dy [N][C][HW]: block (channel c, image chunk j) sums its images' planes with a fixed thread
-// assignment and a fixed tree, in double; k_db_finish adds the chunks in order
+// Per-channel sums of an fp32 NCHW tensor [N][C][HW] (db here, BatchNorm's statistics and gradient sums in
+// bn_train.cu): block (channel c, image chunk j) sums its images' planes with a fixed thread assignment and a fixed
+// tree, in double; the finishing kernels add the chunks in order.  u = a (0 where mask <= 0 when a mask is given);
+// sum 0 = sum u, and with kTwo sum 1 = sum u * (b - b_shift[c]).  Sum k of chunk j lands at part[(k * nchunk + j) * C + c].
 constexpr int kDbThreads = 256;
 constexpr int kDbElems = 16384;                  // elements of one channel per db partial (at least one image)
 static int db_images_per_chunk(int HW) { return HW >= kDbElems ? 1 : kDbElems / HW; }
+template <bool kTwo>
 __global__ void __launch_bounds__(kDbThreads)
-k_db_partial(const float* __restrict__ dy, int N, int C, int HW, int ipc, double* __restrict__ part) {
-    __shared__ double red[kDbThreads];
+k_db_partial(ChanSums s, int N, int C, int HW, int ipc, double* __restrict__ part) {
+    __shared__ double red[kTwo ? 2 : 1][kDbThreads];
     const int c = blockIdx.x, j = blockIdx.y;
     const int n0 = j * ipc, n1 = min(N, n0 + ipc);
-    double acc = 0.0;
+    const double shift = kTwo && s.b_shift ? s.b_shift[c] : 0.0;
+    double acc = 0.0, acc2 = 0.0;
     for (int n = n0; n < n1; ++n) {
-        const float* p = dy + ((size_t)n * C + c) * HW;
-        for (int q = threadIdx.x; q < HW; q += kDbThreads) acc += (double)__ldg(p + q);
+        const size_t off = ((size_t)n * C + c) * HW;
+        for (int q = threadIdx.x; q < HW; q += kDbThreads) {
+            float v = __ldg(s.a + off + q);
+            if (s.mask && !(__ldg(s.mask + off + q) > 0.0f)) v = 0.0f;
+            acc += (double)v;
+            if (kTwo) acc2 += (double)v * ((double)__ldg(s.b + off + q) - shift);
+        }
     }
-    red[threadIdx.x] = acc;
+    red[0][threadIdx.x] = acc;
+    if (kTwo) red[kTwo ? 1 : 0][threadIdx.x] = acc2;
     __syncthreads();
     for (int o = kDbThreads / 2; o > 0; o >>= 1) {
-        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        if (threadIdx.x < o) {
+            red[0][threadIdx.x] += red[0][threadIdx.x + o];
+            if (kTwo) red[kTwo ? 1 : 0][threadIdx.x] += red[kTwo ? 1 : 0][threadIdx.x + o];
+        }
         __syncthreads();
     }
-    if (threadIdx.x == 0) part[(size_t)j * C + c] = red[0];
+    if (threadIdx.x == 0) {
+        part[(size_t)j * C + c] = red[0][0];
+        if (kTwo) part[((size_t)gridDim.y + j) * C + c] = red[kTwo ? 1 : 0][0];
+    }
 }
 __global__ void k_db_finish(const double* __restrict__ part, int nchunk, int C, float* __restrict__ db) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -420,6 +436,20 @@ static int encode_plane(const void* base, int C, int W, int H, int N, int stride
 
 static unsigned long long g_wgrad_devs = 0;
 
+int chan_sums_chunks(int N, int HW) {
+    const int ipc = wg::db_images_per_chunk(HW);
+    return (N + ipc - 1) / ipc;
+}
+
+int chan_sums_partial(const ChanSums& s, bool two, int N, int C, int HW, double* part, cudaStream_t st) {
+    const int ipc = wg::db_images_per_chunk(HW), nchunk = chan_sums_chunks(N, HW);
+    DANET_CHECK(nchunk < 65536, "per-channel sums: too many images");
+    if (two) wg::k_db_partial<true><<<dim3(C, nchunk), wg::kDbThreads, 0, st>>>(s, N, C, HW, ipc, part);
+    else wg::k_db_partial<false><<<dim3(C, nchunk), wg::kDbThreads, 0, st>>>(s, N, C, HW, ipc, part);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
 }  // namespace danet
 
 using namespace danet;
@@ -475,18 +505,18 @@ extern "C" int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout_r, int32_
 
 extern "C" int64_t danet_conv_bias_grad_workspace_bytes(int32_t N, int32_t C, int32_t HW) {
     if (N < 1 || C < 1 || HW < 1) return 0;
-    const int ipc = wg::db_images_per_chunk(HW);
-    return (int64_t)((N + ipc - 1) / ipc) * C * 8;
+    return (int64_t)chan_sums_chunks(N, HW) * C * 8;
 }
 
 extern "C" int danet_conv_bias_grad(int32_t N, int32_t C, int32_t HW, const float* dy, float* db, void* workspace,
                                     danet_stream_t stream) {
     DANET_CHECK(N >= 1 && C >= 1 && HW >= 1 && dy && db && workspace && ((uintptr_t)workspace & 7) == 0,
                 "danet_conv_bias_grad: bad arguments");
-    const int ipc = wg::db_images_per_chunk(HW), nchunk = (N + ipc - 1) / ipc;
+    const int nchunk = chan_sums_chunks(N, HW);
     DANET_CHECK(nchunk < 65536, "danet_conv_bias_grad: too many images");
     cudaStream_t st = (cudaStream_t)stream;
-    wg::k_db_partial<<<dim3(C, nchunk), wg::kDbThreads, 0, st>>>(dy, N, C, HW, ipc, (double*)workspace);
+    const ChanSums s = {dy, nullptr, nullptr, nullptr};
+    if (chan_sums_partial(s, false, N, C, HW, (double*)workspace, st) != 0) return -3;
     wg::k_db_finish<<<cdiv(C, 128), 128, 0, st>>>((const double*)workspace, nchunk, C, db);
     DANET_LAUNCH_CHECK();
     return 0;

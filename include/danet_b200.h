@@ -304,6 +304,42 @@ int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout, int32_t cin, const 
 int64_t danet_conv_bias_grad_workspace_bytes(int32_t N, int32_t C, int32_t HW);
 int danet_conv_bias_grad(int32_t N, int32_t C, int32_t HW, const float* dy, float* db, void* workspace, danet_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training layers of the regressor's ResNet blocks (csrc/bn_train.cu), fp32 NCHW: BatchNorm2d with batch or running
+ * statistics (res_module.py:33-36,406,433,520; smpl_regressor.py:434,496) fused with the residual add and ReLU of
+ * BasicBlock.forward (res_module.py:40-56) and the stems (smpl_regressor.py:432-436,494-499, res_module.py:445-447),
+ * and nn.MaxPool2d(3, 2, 1) (res_module.py:408,448), each with its backward.  No float atomics: every result repeats bit
+ * for bit.  No host synchronisation: capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+/* Workspace of danet_bn2d_forward / danet_bn2d_backward (16-byte aligned; 0 for unsupported sizes): the per-channel
+ * partial sums [2][nchunk][C] (double, rounded up to 256 bytes) + [C][8] floats of coefficients, where nchunk =
+ * ceil(N / ipc) image chunks of ipc = max(1, 16384 / HW) images. */
+int64_t danet_bn2d_workspace_bytes(int32_t N, int32_t C, int32_t HW);
+/* y = relu?(bn(x) + residual?) over x [N,C,HW] with F.batch_norm's semantics.  training = 1: the biased batch variance
+ * normalises; new_running [2][C] (may be NULL) receives (1 - momentum) * running + momentum * (batch mean | unbiased
+ * batch variance); the caller copies it into its buffers.  training = 0: running_mean / running_var normalise.
+ * save [2][C] (double) receives the mean and invstd used, for the backward.  residual may be NULL.  Training needs
+ * N * HW > 1. */
+int danet_bn2d_forward(int32_t N, int32_t C, int32_t HW, const float* x, const float* weight, const float* bias,
+                       const float* running_mean, const float* running_var, int32_t training, float momentum, float eps,
+                       const float* residual, int32_t relu, float* y, double* save, float* new_running, void* workspace,
+                       danet_stream_t stream);
+/* Backward of the forward above (same sizes, x, save, training and relu; y = its output, needed when relu = 1):
+ * dz = dy (0 where y <= 0 with relu); dresidual = dz; dbias = sum dz; dweight = invstd * sum dz (x - mean); dx = w invstd
+ * (dz - sum dz / n - xhat sum dz xhat / n) in training mode, w invstd dz in eval mode.  Each output may be NULL, and
+ * only the non-NULL ones are computed. */
+int danet_bn2d_backward(int32_t N, int32_t C, int32_t HW, const float* x, const float* y, const float* dy,
+                        const float* weight, const double* save, int32_t training, int32_t relu, float* dx, float* dweight,
+                        float* dbias, float* dresidual, void* workspace, danet_stream_t stream);
+/* nn.MaxPool2d(3, 2, 1) (res_module.py:408,448) NCHW x [N,C,H,W] -> y [N,C,Ho,Wo], Ho = (H - 1) / 2 + 1, and per output
+ * the row-major slot (0..8) in its 3x3 window of the maximum taken: the first maximum, NaN over numbers (torch's
+ * choice); padding is never taken. */
+int danet_maxpool3x3s2_nchw_forward(int32_t N, int32_t C, int32_t H, int32_t W, const float* x, float* y, uint8_t* slot,
+                                    danet_stream_t stream);
+/* dx [N,C,H,W]: each input pixel sums, in row-major window order, dy of the windows whose slot chose it. */
+int danet_maxpool3x3s2_nchw_backward(int32_t N, int32_t C, int32_t H, int32_t W, const float* dy, const uint8_t* slot,
+                                     float* dx, danet_stream_t stream);
+
 /* input boundary: x NCHW [N,C,HW] -> y NHWC [N,HW,Cp] with Cp >= C zero-padded channels
  * (images arrive NCHW: demo.py:106, eval.py:147) */
 int danet_nchw_to_nhwc(int32_t N, int32_t C, int32_t HW, int32_t Cp, const float* x, const danet_act* y,
