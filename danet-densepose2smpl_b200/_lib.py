@@ -118,6 +118,8 @@ SIGNATURES = {
     "danet_bn2d_backward": (c_int, [c_int, c_int, c_int] + [c_p] * 5 + [c_int, c_int] + [c_p] * 6),
     "danet_maxpool3x3s2_nchw_forward": (c_int, [c_int] * 4 + [c_p] * 4),
     "danet_maxpool3x3s2_nchw_backward": (c_int, [c_int] * 4 + [c_p] * 4),
+    "danet_global_avgpool_backward": (c_int, [c_int, c_int, c_p, c_p, c_p]),
+    "danet_linear_backward": (c_int, [c_int] * 3 + [c_p] * 7),
     "danet_act_split": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_act_merge": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_nchw_to_nhwc": (c_int, [c_int, c_int, c_int, c_int, c_p, ctypes.POINTER(Act), c_p]),

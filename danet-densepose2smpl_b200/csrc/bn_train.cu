@@ -20,6 +20,10 @@
 // Max pool: the forward stores per output the window slot (0..8, row-major) of its maximum: the first maximum wins,
 // and NaN wins over numbers (torch's rule, so the slots equal its indices).  The backward is a gather: an input pixel
 // adds, in row-major window order, the dy of the windows (at most four) whose slot points at it.
+//
+// Branch tails (their forwards are danet_global_avgpool and danet_linear of glue.cu): the average pool's backward
+// spreads dy / HW over the plane; the linear layer's backward sums dx = dy W, dW = dy^T x and db = sum dy in double, in
+// index order.
 #include "common.cuh"
 #include <math.h>
 
@@ -235,6 +239,46 @@ k_maxpool3x3s2_bwd(long long total, int H, int W, int Ho, int Wo, const float* _
     dx[i] = acc;
 }
 
+// ------------------------------------------------------------------------------------------------
+// tails of the regressor branches: global average pool and linear layer, backward
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads)
+k_global_avgpool_bwd(long long total, int HW, const float* __restrict__ dy, float* __restrict__ dx) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= total) return;
+    dx[i] = __ldg(dy + i / HW) / (float)HW;
+}
+
+// One thread per output element over the flat index space [dx: N * In | dW: Out * In | db: Out] (a part is empty when
+// its output is NULL).  Every sum runs in double in index order: no atomics, bit-identical on every run.
+__global__ void __launch_bounds__(kThreads)
+k_linear_bwd(int N, int In, int Out, long long ndx, long long ndw, long long ndb, const float* __restrict__ x,
+             const float* __restrict__ w, const float* __restrict__ dy, float* __restrict__ dx, float* __restrict__ dw,
+             float* __restrict__ db) {
+    long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i < ndx) {                                  // dx[n,i] = sum_o dy[n,o] w[o,i]
+        const int n = (int)(i / In), k = (int)(i - (long long)n * In);
+        double s = 0.0;
+        for (int o = 0; o < Out; ++o) s += (double)__ldg(dy + (size_t)n * Out + o) * (double)__ldg(w + (size_t)o * In + k);
+        dx[i] = (float)s;
+        return;
+    }
+    i -= ndx;
+    if (i < ndw) {                                  // dW[o,i] = sum_n dy[n,o] x[n,i]
+        const int o = (int)(i / In), k = (int)(i - (long long)o * In);
+        double s = 0.0;
+        for (int n = 0; n < N; ++n) s += (double)__ldg(dy + (size_t)n * Out + o) * (double)__ldg(x + (size_t)n * In + k);
+        dw[i] = (float)s;
+        return;
+    }
+    i -= ndw;
+    if (i < ndb) {                                  // db[o] = sum_n dy[n,o]
+        double s = 0.0;
+        for (int n = 0; n < N; ++n) s += (double)__ldg(dy + (size_t)n * Out + i);
+        db[i] = (float)s;
+    }
+}
+
 static unsigned grid_of(long long work) { return (unsigned)((work + kThreads - 1) / kThreads); }
 static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
@@ -334,6 +378,32 @@ extern "C" int danet_maxpool3x3s2_nchw_backward(int32_t N, int32_t C, int32_t H,
     const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
     const long long total = (long long)N * C * H * W;
     bn::k_maxpool3x3s2_bwd<<<bn::grid_of(total), bn::kThreads, 0, (cudaStream_t)stream>>>(total, H, W, Ho, Wo, dy, slot, dx);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int danet_global_avgpool_backward(int32_t NC, int32_t HW, const float* dy, float* dx, danet_stream_t stream) {
+    DANET_CHECK(NC >= 1 && HW >= 1 && (long long)NC * HW < (1LL << 31), "danet_global_avgpool_backward: bad sizes NC=%d HW=%d",
+                NC, HW);
+    DANET_CHECK(dy && dx, "danet_global_avgpool_backward: dy and dx must be non-null");
+    const long long total = (long long)NC * HW;
+    bn::k_global_avgpool_bwd<<<bn::grid_of(total), bn::kThreads, 0, (cudaStream_t)stream>>>(total, HW, dy, dx);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int danet_linear_backward(int32_t N, int32_t In, int32_t Out, const float* x, const float* w, const float* dy,
+                                     float* dx, float* dw, float* db, danet_stream_t stream) {
+    DANET_CHECK(N >= 1 && In >= 1 && Out >= 1 && (long long)N * In < (1LL << 31) && (long long)Out * In < (1LL << 31) &&
+                (long long)N * Out < (1LL << 31), "danet_linear_backward: bad sizes N=%d In=%d Out=%d", N, In, Out);
+    DANET_CHECK(dy, "danet_linear_backward: dy must be non-null");
+    DANET_CHECK(!dx || w, "danet_linear_backward: dx needs the weight w");
+    DANET_CHECK(!dw || x, "danet_linear_backward: dw needs the input x");
+    const long long ndx = dx ? (long long)N * In : 0, ndw = dw ? (long long)Out * In : 0, ndb = db ? Out : 0;
+    const long long total = ndx + ndw + ndb;
+    if (total == 0) return 0;
+    bn::k_linear_bwd<<<bn::grid_of(total), bn::kThreads, 0, (cudaStream_t)stream>>>(N, In, Out, ndx, ndw, ndb, x, w, dy, dx,
+                                                                                   dw, db);
     DANET_LAUNCH_CHECK();
     return 0;
 }

@@ -5,6 +5,8 @@
     y = batch_norm(x, running_mean, running_var, weight, bias, training, momentum, eps,
                    residual=None, relu=False)      # relu(F.batch_norm(...) + residual)
     y = max_pool2d(x, 3, 2, 1)                     # F.max_pool2d(x, kernel_size=3, stride=2, padding=1)
+    y = adaptive_avg_pool2d(x, 1)                  # F.adaptive_avg_pool2d(x, 1)
+    y = linear(x, weight, bias, add=None)          # F.linear(x, weight, bias) + add (add: a constant [Out] term)
 
 `batch_norm` has the meaning and argument order of torch.nn.functional.batch_norm.  Training mode normalises with the
 biased batch variance over (N, H, W) and updates running_mean / running_var in place with `momentum` and the unbiased
@@ -21,6 +23,7 @@ fall-back to torch).  weight, bias and the running statistics must be given and 
 BatchNorm2d of the network is affine, tracks its statistics and uses momentum 0.1 (res_module.py:17).  The backward
 computes only the gradients in ctx.needs_input_grad.  Nothing synchronises with the host and no float atomics are used:
 results repeat bit for bit, and forward + backward can be captured in a CUDA graph."""
+import ctypes
 import numbers
 
 import torch
@@ -208,3 +211,102 @@ def max_pool2d(input, kernel_size, stride=None, padding=0, dilation=1, ceil_mode
         raise ValueError("danet_b200.layers.max_pool2d: empty input %s" % (tuple(input.shape),))
     _check_cuda("max_pool2d", [("input", input)], input.device)
     return _MaxPool.apply(input)
+
+
+class _AvgPool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        lib = _lib.load()
+        dev = x.device
+        N, C, H, W = x.shape
+        with torch.cuda.device(dev):
+            y = torch.empty(N, C, 1, 1, dtype=torch.float32, device=dev)
+            act = _lib.Act(x.data_ptr(), None, None)          # NCHW [N, C, HW] is NHWC [N * C, HW, 1]
+            _lib.check(lib.danet_global_avgpool(N * C, H * W, 1, ctypes.byref(act), _lib.ptr(y), _lib.stream_ptr(dev)),
+                       "global_avgpool")
+        ctx.shape = (N, C, H, W)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        N, C, H, W = ctx.shape
+        lib = _lib.load()
+        dev = gy.device
+        with torch.cuda.device(dev):
+            gy = gy.to(torch.float32).contiguous()
+            dx = torch.empty(N, C, H, W, dtype=torch.float32, device=dev)
+            _lib.check(lib.danet_global_avgpool_backward(N * C, H * W, _lib.ptr(gy), _lib.ptr(dx), _lib.stream_ptr(dev)),
+                       "global_avgpool_backward")
+        return dx
+
+
+def adaptive_avg_pool2d(input, output_size):
+    """F.adaptive_avg_pool2d for output size 1 (nn.AdaptiveAvgPool2d(1) of SmplResNet and LimbResLayers) on the GPU,
+    differentiable: [N, C, H, W] -> [N, C, 1, 1]."""
+    size = tuple(output_size) if isinstance(output_size, (tuple, list)) else (output_size, output_size)
+    if size != (1, 1):
+        raise ValueError("danet_b200.layers.adaptive_avg_pool2d: only output_size=1 is supported (got %r)" % (output_size,))
+    _check_tensor("adaptive_avg_pool2d", "input", input)
+    if input.dim() != 4:
+        raise ValueError("danet_b200.layers.adaptive_avg_pool2d: input must be 4-D NCHW (got %d-D)" % input.dim())
+    if min(input.shape) < 1:
+        raise ValueError("danet_b200.layers.adaptive_avg_pool2d: empty input %s" % (tuple(input.shape),))
+    _check_cuda("adaptive_avg_pool2d", [("input", input)], input.device)
+    return _AvgPool.apply(input)
+
+
+class _Linear(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, add):
+        lib = _lib.load()
+        dev = x.device
+        (N, In), Out = x.shape, weight.shape[0]
+        with torch.cuda.device(dev):
+            y = torch.empty(N, Out, dtype=torch.float32, device=dev)
+            _lib.check(lib.danet_linear(N, In, Out, _lib.ptr(x), _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(add), _lib.ptr(y),
+                                        _lib.stream_ptr(dev)), "linear")
+        need_x, need_w = ctx.needs_input_grad[:2]
+        ctx.save_for_backward(x if need_w else None, weight if need_x else None)
+        ctx.shape = (N, In, Out)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x, weight = ctx.saved_tensors
+        need_x, need_w, need_b = ctx.needs_input_grad[:3]
+        N, In, Out = ctx.shape
+        lib = _lib.load()
+        dev = gy.device
+        with torch.cuda.device(dev):
+            gy = gy.to(torch.float32).contiguous()
+            dx = torch.empty(N, In, dtype=torch.float32, device=dev) if need_x else None
+            dw = torch.empty(Out, In, dtype=torch.float32, device=dev) if need_w else None
+            db = torch.empty(Out, dtype=torch.float32, device=dev) if need_b else None
+            if need_x or need_w or need_b:
+                _lib.check(lib.danet_linear_backward(N, In, Out, _lib.ptr(x), _lib.ptr(weight), _lib.ptr(gy), _lib.ptr(dx),
+                                                     _lib.ptr(dw), _lib.ptr(db), _lib.stream_ptr(dev)), "linear_backward")
+        return dx, dw, db, None
+
+
+def linear(input, weight, bias=None, *, add=None):
+    """F.linear(input, weight, bias) + add on the GPU, differentiable w.r.t. input, weight and bias.  input [N, In],
+    weight [Out, In], bias and add [Out]; `add` is a constant term with no gradient (body_net's tail adds
+    mean_cam_shape there)."""
+    fn = "linear"
+    _check_tensor(fn, "input", input)
+    if input.dim() != 2:
+        raise ValueError("danet_b200.layers.linear: input must be 2-D [N, In] (got %d-D)" % input.dim())
+    _check_tensor(fn, "weight", weight)
+    if weight.dim() != 2 or weight.shape[1] != input.shape[1]:
+        raise ValueError("danet_b200.layers.linear: weight must be [Out, %d] (got %s)" % (input.shape[1], tuple(weight.shape)))
+    if min(input.shape) < 1 or weight.shape[0] < 1:
+        raise ValueError("danet_b200.layers.linear: empty input or weight (%s, %s)" % (tuple(input.shape), tuple(weight.shape)))
+    tensors = [("input", input), ("weight", weight)]
+    for name, t in (("bias", bias), ("add", add)):
+        if t is not None:
+            _check_tensor(fn, name, t, (weight.shape[0],))
+            tensors.append((name, t))
+    _check_cuda(fn, tensors, input.device)
+    return _Linear.apply(input, weight, bias, add.detach() if add is not None else None)

@@ -19,8 +19,28 @@ One torch.autograd.Function takes the head's 29 parameters as inputs: after back
 global_para.  Nothing synchronises with the host, and forward + backward + losses can be captured in a CUDA graph.
 
 Deviation from the reference, stated: with no image selected by has_smpl the head losses are 0-dim zeros with a zero
-gradient; the reference raises NameError there (`pred` is undefined at smpl_regressor.py:153)."""
+gradient; the reference raises NameError there (`pred` is undefined at smpl_regressor.py:153).
+
+The three ResNet branches in front of the head (smpl_regressor.py:688-725) train through the same module:
+
+    from danet_b200.regressor import body_branch, limb_branch, predictor
+    global_para = body_branch(model, body_iuv)          # [B,13] = body_net(body_iuv) + mean_cam_shape
+    rot_feats   = limb_branch(model, part_iuv)          # [B,24,128]: limb_net -> limb_reslayer -> average pool
+    out         = predictor(model, body_iuv, part_iuv)  # gcn_head(model, rot_feats, global_para)
+
+body_iuv [B,75,S,S] is cat[U,V,I] of the cleaned maps, part_iuv [B,24,3,7,S,S] the cleaned per-part maps, both fp32 on
+the model's CUDA device, any S.  The branches are not restated here: `lower_branches` walks the regressor ops of the
+network graph (model.graph, the description parameter registration and the inference plan consume) from `body_iuv` to
+`global_para` and from `part_iuv_clean` to `rot_feats`, and lowers each op once per graph into differentiable ops:
+conv2d (danet_b200.conv), batch_norm fused with residual and ReLU, max_pool2d, adaptive_avg_pool2d and linear
+(danet_b200.layers).  A limb tensor is NCHW [24B, C, H, W], the same memory as [B, 24C, H, W]: the grouped convolutions
+of limb_reslayer and their BatchNorm2d(24 * 128) take the second view (statistics over the batch), limb_net's
+BatchNorm2d(64) the first (statistics pooled over the parts).  model.training selects BatchNorm's mode as in gcn_head;
+training mode also adds 1 to every num_batches_tracked.  Inputs that do not require grad get no input gradient (the
+first convolution then skips its input gradient)."""
 import ctypes
+import types
+import weakref
 
 import torch
 from torch.autograd.function import once_differentiable
@@ -217,3 +237,170 @@ def gcn_head_losses(out, target, gt_smpl_joints, has_smpl, rot_weight=SMPL_POSE_
     has = (has_smpl.to(dev) == 1).to(torch.uint8).contiguous()
     L = _HeadLosses.apply(pose0, coord0, coord1, target.to(dev), gt_smpl_joints.to(dev), has, rot_weight, pos_weight)
     return {"joint_rotation0": L[0], "joint_position0": L[1], "joint_position1": L[2]}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# body_net, limb_net and limb_reslayer: the graph's regressor ops lowered into differentiable ops
+# ---------------------------------------------------------------------------------------------------------------------
+RP = "iuv2smpl.smpl_para_Outs."
+BN_MOMENTUM, BN_EPS = 0.1, 1e-5                   # every BatchNorm2d of the branches (res_module.py:17, nn defaults)
+BRANCHES = {"body": ("body_iuv", "global_para"), "limb": ("part_iuv_clean", "rot_feats")}
+_BN_KEYS = ("weight", "bias", "running_mean", "running_var", "num_batches_tracked")
+_LOWERED = weakref.WeakKeyDictionary()
+
+
+def _lower_op(op):
+    """One graph op -> training ops: dicts with the op name, input / output tensor names, their arguments and `keys`,
+    the state_dict keys the op consumes."""
+    kind, x, y = op["op"], op["x"].name, op["y"].name
+    if kind == "conv":
+        (wkey, _, has_bias), = op["parts"]
+        g = op["groups"]
+        conv = dict(op="conv2d", x=x, y=y, weight=wkey + ".weight", bias=wkey + ".bias" if has_bias else None,
+                    stride=op["stride"], padding=op["pad"], groups=g)
+        conv["keys"] = tuple(k for k in (conv["weight"], conv["bias"]) if k)
+        if not op["bn"]:
+            if op["relu"] or op["res"] is not None:
+                raise ValueError("lower_branches: a residual or ReLU without BatchNorm (%s) has no training lowering" % wkey)
+            return [conv]
+        conv["y"] = y + ":conv"
+        bn = dict(op="batch_norm", x=conv["y"], y=y, bn=op["bn"], res=op["res"].name if op["res"] is not None else None,
+                  relu=op["relu"], groups=g, keys=tuple("%s.%s" % (op["bn"], k) for k in _BN_KEYS))
+        return [conv, bn]
+    if kind == "maxpool":
+        return [dict(op="max_pool2d", x=x, y=y, keys=())]
+    if kind == "avgpool":
+        return [dict(op="adaptive_avg_pool2d", x=x, y=y, keys=())]
+    if kind == "body_fc":                         # SmplResNet's avg_pooling + final_layer, + mean_cam_shape (:696)
+        w, b, add = RP + "body_net.3.final_layer.weight", RP + "body_net.3.final_layer.bias", RP + "mean_cam_shape"
+        return [dict(op="adaptive_avg_pool2d", x=x, y=y + ":pool", keys=()),
+                dict(op="linear", x=y + ":pool", y=y, weight=w, bias=b, add=add, keys=(w, b, add))]
+    raise ValueError("lower_branches: graph op %r has no training lowering" % kind)
+
+
+def _walk(graph, src, dst):
+    live, out = {src}, []
+    for op in graph.ops:
+        x = op.get("x")
+        if x is None or getattr(x, "name", None) not in live:
+            continue
+        if op.get("res") is not None and op["res"].name not in live:
+            raise ValueError("lower_branches: residual %s of %s is not on the branch" % (op["res"].name, op["y"].name))
+        out += _lower_op(op)
+        live.add(op["y"].name)
+        if op["y"].name == dst:
+            return out
+    raise ValueError("lower_branches: the graph has no path from %s to %s" % (src, dst))
+
+
+def lower_branches(graph):
+    """{'body': ops, 'limb': ops}: the ops of `graph` reachable from body_iuv up to global_para and from part_iuv_clean
+    up to rot_feats, lowered once per graph (see _lower_op)."""
+    low = _LOWERED.get(graph)
+    if low is None:
+        low = {name: dict(src=src, dst=dst, ops=_walk(graph, src, dst)) for name, (src, dst) in BRANCHES.items()}
+        _LOWERED[graph] = low
+    return low
+
+
+def _grouped(t, g):
+    """[N, C, H, W] -> [N / g, g C, H, W] (the same memory)"""
+    return t if g == 1 else t.reshape(t.shape[0] // g, g * t.shape[1], t.shape[2], t.shape[3])
+
+
+def _ungrouped(t, g):
+    return t if g == 1 else t.reshape(t.shape[0] * g, t.shape[1] // g, t.shape[2], t.shape[3])
+
+
+def run_branch(branch, state, x, training, ops):
+    """Runs one lowered branch (lower_branches(graph)[name]) on x ([B,75,S,S] for 'body', [24B,21,S,S] for 'limb').
+    `state` maps state_dict keys to tensors; `ops` provides conv2d, batch_norm, max_pool2d, adaptive_avg_pool2d and
+    linear with the signatures of danet_b200.conv / danet_b200.layers.  Training mode adds 1 to num_batches_tracked.
+    Returns the branch output: [B,13] or [24B,128,1,1]."""
+    env = {branch["src"]: x}
+    for op in branch["ops"]:
+        kind, g, t = op["op"], op.get("groups", 1), env[op["x"]]
+        if kind == "conv2d":
+            bias = state[op["bias"]] if op["bias"] else None
+            y = _ungrouped(ops.conv2d(_grouped(t, g), state[op["weight"]], bias, op["stride"], op["padding"], 1, g), g)
+        elif kind == "batch_norm":
+            p = lambda k: state["%s.%s" % (op["bn"], k)]
+            res = _grouped(env[op["res"]], g) if op["res"] else None
+            y = _ungrouped(ops.batch_norm(_grouped(t, g), p("running_mean"), p("running_var"), p("weight"), p("bias"),
+                                          training, BN_MOMENTUM, BN_EPS, residual=res, relu=op["relu"]), g)
+        elif kind == "max_pool2d":
+            y = ops.max_pool2d(t, 3, 2, 1)
+        elif kind == "adaptive_avg_pool2d":
+            y = ops.adaptive_avg_pool2d(t, 1)
+        else:
+            y = ops.linear(t.reshape(t.shape[0], -1), state[op["weight"]], state[op["bias"]],
+                           add=state[op["add"]].reshape(-1))
+        env[op["y"]] = y
+    if training:
+        with torch.no_grad():
+            for op in branch["ops"]:
+                if op["op"] == "batch_norm":
+                    state[op["bn"] + ".num_batches_tracked"].add_(1)
+    return env[branch["dst"]]
+
+
+def _cuda_ops():
+    from . import conv, layers
+    return types.SimpleNamespace(conv2d=conv.conv2d, batch_norm=layers.batch_norm, max_pool2d=layers.max_pool2d,
+                                 adaptive_avg_pool2d=layers.adaptive_avg_pool2d, linear=layers.linear)
+
+
+def _model_state(model, branch):
+    graph = getattr(model, "graph", None)
+    if graph is None:
+        raise ValueError("danet_b200.regressor: model must be a danet_b200.DaNet (it has no network graph)")
+    low = lower_branches(graph)[branch]
+    state = {k: _attr(model, k) for op in low["ops"] for k in op["keys"]}
+    dev = state[low["ops"][0]["weight"]].device
+    if dev.type != "cuda":
+        raise ValueError("danet_b200.regressor: move the model to a CUDA device (there is no CPU path)")
+    return low, state, dev
+
+
+def _check_input(fn, name, t, dev, shape_tail, desc):
+    if not isinstance(t, torch.Tensor):
+        raise ValueError("danet_b200.regressor.%s: %s must be a tensor (got %s)" % (fn, name, type(t).__name__))
+    if t.dtype != torch.float32:
+        raise ValueError("danet_b200.regressor.%s: %s must be float32 (got %s)" % (fn, name, t.dtype))
+    if t.device != dev:
+        raise ValueError("danet_b200.regressor.%s: %s is on %s, the model on %s" % (fn, name, t.device, dev))
+    n = len(shape_tail)
+    if t.dim() != n + 3 or tuple(t.shape[1:n + 1]) != shape_tail or t.shape[0] < 1 or t.shape[-1] < 1 or \
+            t.shape[-1] != t.shape[-2]:
+        raise ValueError("danet_b200.regressor.%s: %s must be %s with B >= 1 (got %s)" % (fn, name, desc, tuple(t.shape)))
+
+
+def body_branch(model, body_iuv):
+    """global_para [B,13] = body_net(body_iuv) + mean_cam_shape (smpl_regressor.py:688,696) in model.training's
+    BatchNorm mode, differentiable w.r.t. body_iuv and body_net's parameters."""
+    low, state, dev = _model_state(model, "body")
+    _check_input("body_branch", "body_iuv", body_iuv, dev, (75,), "[B,75,S,S]")
+    return run_branch(low, state, body_iuv.contiguous(), bool(model.training), _cuda_ops())
+
+
+def limb_branch(model, part_iuv):
+    """rot_feats [B,24,128]: limb_net over the (batch, part) images, limb_reslayer over [B, 24 C, H, W] and the average
+    pool (smpl_regressor.py:713-725) in model.training's BatchNorm mode, differentiable w.r.t. part_iuv and the
+    parameters of limb_net and limb_reslayer."""
+    low, state, dev = _model_state(model, "limb")
+    _check_input("limb_branch", "part_iuv", part_iuv, dev, (24, 3, 7), "[B,24,3,7,S,S]")
+    B, S = part_iuv.shape[0], part_iuv.shape[-1]
+    y = run_branch(low, state, part_iuv.reshape(B * 24, 21, S, S).contiguous(), bool(model.training), _cuda_ops())
+    return y.reshape(B, 24, -1)
+
+
+def predictor(model, body_iuv, part_iuv):
+    """DecomposedPredictor.forward for the 'iuv' input and the 'gcn' strategy (smpl_regressor.py:676-928):
+    gcn_head(model, limb_branch(model, part_iuv), body_branch(model, body_iuv)), i.e. {'para' [B,229],
+    'joint_rotation', 'joint_position'}, which feed gcn_head_losses and smpl_losses unchanged."""
+    if body_iuv.shape[0] != part_iuv.shape[0]:
+        raise ValueError("danet_b200.regressor.predictor: body_iuv and part_iuv hold %d and %d images"
+                         % (body_iuv.shape[0], part_iuv.shape[0]))
+    global_para = body_branch(model, body_iuv)
+    rot_feats = limb_branch(model, part_iuv)
+    return gcn_head(model, rot_feats, global_para)

@@ -339,6 +339,14 @@ int danet_maxpool3x3s2_nchw_forward(int32_t N, int32_t C, int32_t H, int32_t W, 
 /* dx [N,C,H,W]: each input pixel sums, in row-major window order, dy of the windows whose slot chose it. */
 int danet_maxpool3x3s2_nchw_backward(int32_t N, int32_t C, int32_t H, int32_t W, const float* dy, const uint8_t* slot,
                                      float* dx, danet_stream_t stream);
+/* Backward of nn.AdaptiveAvgPool2d(1) over NC planes of HW pixels (the forward is danet_global_avgpool on the fp32 view
+ * [NC, HW, 1]): dx [NC][HW] = dy [NC] / HW. */
+int danet_global_avgpool_backward(int32_t NC, int32_t HW, const float* dy, float* dx, danet_stream_t stream);
+/* Backward of danet_linear (y = x W^T + b + add; add is not differentiated): x [N][In], w [Out][In], dy [N][Out] ->
+ * dx = dy W [N][In], dw = dy^T x [Out][In], db = sum_n dy [Out], each summed in double in index order.  Each output
+ * may be NULL, and only the non-NULL ones are computed (dx needs w, dw needs x). */
+int danet_linear_backward(int32_t N, int32_t In, int32_t Out, const float* x, const float* w, const float* dy, float* dx,
+                          float* dw, float* db, danet_stream_t stream);
 
 /* input boundary: x NCHW [N,C,HW] -> y NHWC [N,HW,Cp] with Cp >= C zero-padded channels
  * (images arrive NCHW: demo.py:106, eval.py:147) */
