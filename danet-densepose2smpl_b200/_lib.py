@@ -101,8 +101,7 @@ SIGNATURES = {
     "danet_conv_tc_geometry": (c_int, [ctypes.POINTER(ConvDesc), c_p]),
     "danet_conv_tc_cta_geometry": (c_int, [ctypes.POINTER(ConvDesc), c_p]),
     "danet_conv_tc_group": (c_int, [c_int, ctypes.POINTER(ConvProblem), c_p]),
-    "danet_conv_tc_config": (c_int, [c_int, ctypes.POINTER(ConvDesc), c_p, c_p]),
-    "danet_conv_tc_pack_async": (c_int, [ctypes.POINTER(ConvDesc), c_p, c_p, c_p]),
+    "danet_conv_tc_config": (c_int, [c_int, ctypes.POINTER(ConvDesc), c_p]),
     "danet_conv_weights_simt": (c_int, [c_int] * 6 + [c_p, c_p, c_p]),
     "danet_conv_dgrad_pieces": (c_int, [c_int, c_int, c_p]),
     "danet_conv_dgrad_weights": (c_int, [c_int] * 5 + [c_p, c_int, c_int, c_p, c_p, c_p]),

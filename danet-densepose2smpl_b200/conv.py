@@ -9,7 +9,7 @@ cover every convolution of the network.  Anything else raises ValueError; there 
 need not be multiples of 8: the op pads them internally.
 
 - Forward: x becomes split-fp16 NHWC planes (danet_nchw_to_nhwc), the current weights are packed on every call
-  (danet_conv_tc_pack_async: they change every optimiser step), danet_conv_tc_group runs the convolution, and
+  (danet_conv_tc_pack: they change every optimiser step), danet_conv_tc_group runs the convolution, and
   danet_conv_dgrad_scatter writes the fp32 NCHW result.
 - Input gradient: forward problems of the same engine.  Stride 1 is conv(dy, W') with W' the rotated filter.  Stride 2
   splits each output-parity class of dx into 1x1 / 3x3 stride-1 pieces (a 4-tap 7x7/s2 parity becomes a centred 3-tap
@@ -72,8 +72,7 @@ def _pack(lib, d, w_simt, dev):
     if nbytes <= 0:
         raise ValueError("danet_b200.conv.conv2d: shape not supported by the tensor-core path")
     pk = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    _lib.check(lib.danet_conv_tc_pack_async(ctypes.byref(d), _lib.ptr(w_simt), _lib.ptr(pk), _lib.stream_ptr(dev)),
-               "conv_tc_pack_async")
+    _lib.check(lib.danet_conv_tc_pack(ctypes.byref(d), _lib.ptr(w_simt), _lib.ptr(pk), _lib.stream_ptr(dev)), "conv_tc_pack")
     return pk
 
 

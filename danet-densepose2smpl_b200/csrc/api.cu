@@ -12,7 +12,9 @@ void set_error(const char* fmt, ...) {
 }  // namespace danet
 
 extern "C" const char* danet_last_error(void) { return danet::g_err; }
-extern "C" int danet_version(void) { return 3; }   // 3: danet_act views, danet_conv_tc_group (split-fp16 tensor-core engine)
+// 3: danet_act views, danet_conv_tc_group (split-fp16 tensor-core engine); 4: one weight packer
+// (danet_conv_tc_pack is stream-ordered, danet_conv_tc_pack_async is gone), danet_conv_tc_config without sub-tiles
+extern "C" int danet_version(void) { return 4; }
 extern "C" int danet_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     int dev = 0;
     DANET_CUDA(cudaGetDevice(&dev));

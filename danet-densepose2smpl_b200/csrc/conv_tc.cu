@@ -27,7 +27,7 @@
 //       Every MMA has a compile-time width (one tile body per N tile width); a warpgroup commits one group per
 //       weight block and waits only for the block before it, so the MMAs of consecutive blocks stay in flight.
 //   K segments (exact mode): the tensor core's fp32 accumulation truncates, which biases long chains; after every
-//       lseg main-chain MMAs the accumulators are added in fp32 round-to-nearest to a running sum that starts at
+//       kSegMmas main-chain MMAs the accumulators are added in fp32 round-to-nearest to a running sum that starts at
 //       bias + residual.
 //   Epilogue: each consumer thread holds 2 pixels x 2 consecutive channels per 8-channel group; ReLU, output as
 //       split-fp16 planes and/or fp32.
@@ -44,6 +44,7 @@
 #include <cuda_fp16.h>
 #include <mutex>
 #include <type_traits>
+#include <utility>
 #include <string.h>
 #include <math.h>
 
@@ -64,6 +65,7 @@ constexpr int kSmemFixed = 2048;                       // barriers + 1024-byte a
 constexpr int kSchedDepth = 4, kSchedAhead = 2, kSchedStatic = 3;
 __host__ __device__ constexpr int kSchedConsumersOf(int ex) { return 4 * kConsumersOf(ex); }   // lane 0 of every consumer warp
 constexpr int kPackHeader = 1024;                      // packed weights start with a header: float[0] = 2^s applied to the weights, float[1] = 2^-s
+constexpr int kSegMmas = 8;                            // exact mode: close a K segment after a weight block once it holds >= 8 main-chain MMAs
 
 struct alignas(64) Prob {
     CUtensorMap tm[2];                   // input planes: hi, lo
@@ -77,15 +79,13 @@ struct alignas(64) Prob {
     int NT, ntn;                         // output channels per N tile, N tiles
     int nstack, hs, box_h;               // small maps: nstack images share one tile; image n's rows start at group n*hs
                                          // (hs = H + pad: the zero rows between images are the TMA out-of-bounds fill)
-    int lseg;                            // K segmentation: close a segment after a weight block once it holds >= lseg
-                                         // main-chain MMAs (exact mode)
+    int bpc;                             // weight blocks per channel chunk
     int par_py[4], par_px[4], ntap[4], ngrp[4], stage_bytes[4], sbo_a[4];
     int tapoff16[4][16];                 // smem offset (16-byte units) of each tap's shifted view inside the plane
     int tapidx[4][16];                   // original filter tap index r*ks+s (weight packing)
     int tiles_w, tiles_h, tile_count, tile_base;
     int rows_blk;                        // rows of one weight block per tap
     int tap_bytes, b_block_bytes, nblk;  // nblk: weight blocks per (weight set, N tile)
-    int bpc;                             // weight blocks per channel chunk
     long long blocks_per_set;
     unsigned long long m_ntn, m_tw, m_th, m_ws;
 };
@@ -180,7 +180,6 @@ static bool make_prob(const danet_conv_desc* d, Prob* g) {
         }
     }
     g->nblk = g->nchunks * g->bpc;
-    g->lseg = g->exact ? 8 : (1 << 30);
     g->blocks_per_set = (long long)g->ntn * g->nblk;
     g->tiles_w = (g->Wo + kTileW - 1) / kTileW; g->tiles_h = (g->Ho + kTileH - 1) / kTileH;
     // image groups: one image each, or (stacked) wsets x ceil(images per set / nstack)
@@ -523,13 +522,13 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
     const uint64_t bd0 = make_desc(0, 8 * SWB, SWB);
     uint32_t acc = 0;
     int seg_cnt = 0;
-    // ring slots whose MMAs may still be in flight: freed once a later wait covers them (-1: none)
-    int pend_b = -1, pend_ahi = -1, pend_alo = -1;
+    // ring slots whose MMAs may still be in flight: freed once a later wait covers them (-1: none).  Only fast mode
+    // holds an A slot past its parity plane: exact mode drains at every plane end and frees its A slots there.
+    int pend_b = -1, pend_a = -1;
     auto release_pending = [&]() {
         mbar_arrive_if(S.bar_b_empty + 8 * pend_b, leader && pend_b >= 0);
-        mbar_arrive_if(S.bar_a_empty + 8 * pend_ahi, leader && pend_ahi >= 0);
-        if (EX) mbar_arrive_if(S.bar_a_empty + 8 * pend_alo, leader && pend_alo >= 0);
-        pend_b = pend_ahi = pend_alo = -1;
+        mbar_arrive_if(S.bar_a_empty + 8 * pend_a, leader && pend_a >= 0);
+        pend_b = pend_a = -1;
     };
     for (int c = 0; c < nchunks; ++c) {
         const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
@@ -547,7 +546,6 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
             // this warpgroup's 8 tile rows start 8 halo rows further down for the second warpgroup
             const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB) + ((uint32_t)(wg * 8 * P.sbo_a[slot]) >> 4);
             const uint64_t ad_hi = ad0 + ((S.sA + as_hi * a.a_slot_bytes) >> 4);
-            const uint64_t ad_lo = ad0 + ((S.sA + as_lo * a.a_slot_bytes) >> 4);
             Var ngrp = P.ngrp[slot], ntap = P.ntap[slot];
             for (int tg = 0; tg < ngrp; ++tg) {
                 const int k0 = tg * TG;
@@ -602,12 +600,9 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
                 }
                 wg_commit();
                 const bool plane_end = tg == ngrp - 1;
-                bool close = false;
                 if constexpr (EX) {
                     seg_cnt += ntk * kv;
-                    close = (c == nchunks - 1 && slot == npa - 1 && plane_end) || seg_cnt >= P.lseg;
-                }
-                if constexpr (EX) {
+                    const bool close = (c == nchunks - 1 && slot == npa - 1 && plane_end) || seg_cnt >= kSegMmas;
                     // A parity plane's end drains too, so that its two A slots are free before the next plane's halos
                     // are loaded: with three A slots, that is what lets the next plane's lo halo in.  The chain goes on
                     // (acc stays 1) unless the K segment closes, so the MMA sequence is unchanged.
@@ -654,29 +649,12 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
                         R.aph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 1), 0);
                         R.bph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 2), 0);
                     }
-                } else if (close) {
-                    // close the K segment: the whole chain must have landed
-                    wg_wait_all();
-                    reg_fence<NV>(m);
-                    if constexpr (EX) {
-                        reg_fence<NV>(s);
-#pragma unroll
-                        for (int j = 0; j < NV; ++j) {
-                            sum[j] += m[j];
-                            sum[j] += s[j];
-                        }
-                    }
-                    acc = 0; seg_cnt = 0;
-                    release_pending();
-                    mbar_arrive_if(S.bar_b_empty + 8 * bs, leader);
-                    mbar_arrive_if(S.bar_a_empty + 8 * as_hi, leader && plane_end);
-                    if (EX) mbar_arrive_if(S.bar_a_empty + 8 * as_lo, leader && plane_end);
                 } else {
                     // the block before this one is done: free its slots, keep this one's until the next wait
                     wg_wait_1();
                     release_pending();
                     pend_b = bs;
-                    if (plane_end) { pend_ahi = as_hi; pend_alo = as_lo; }
+                    if (plane_end) pend_a = as_hi;
                 }
             }
         }
@@ -725,7 +703,6 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
 template <int EX>
 __global__ void __launch_bounds__(kThreadsOf(EX), 1)
 k_conv_tc(const __grid_constant__ ArgsN a) {
-    constexpr int NTMAX = EX ? kNtMaxExact : kNtMaxFast;
     extern __shared__ __align__(1024) uint8_t smem[];
     const uint32_t sbase = (smem_u32(smem) + 1023u) & ~1023u;          // swizzle atoms need 1024-byte alignment
     const uint32_t sA = sbase;
@@ -761,7 +738,7 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
         const bool prod = warp == 0;
         const Smem S = {sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty};
         Ring R = {0, 0, 0u, 0u};
-        constexpr int NVMAX = NTMAX / 2;
+        constexpr int NVMAX = kNtMaxExact / 2;
         float accs[2 * NVMAX];                 // small terms then main chain
         float sum[NVMAX];                      // bias + residual + every closed K segment, fp32 round-to-nearest
         pdl_wait();                            // activations come from the previous kernel; residual reads / output writes
@@ -817,22 +794,20 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
                 int b = 0;
                 for (int c = 0; c < P.nchunks; ++c)
                     for (int slot = 0; slot < P.npa; ++slot) {
-                        for (int pl = 0; pl <= EX; ++pl) {
-                            mbar_wait(bar_a_empty + 8 * as, ((aph >> as) & 1u) ^ 1u);
-                            if (P.nstack > 1) {
-                                const uint32_t box_bytes = (uint32_t)(P.box_h * P.sbo_a[slot]);
-                                mbar_expect_tx(bar_a_full + 8 * as, box_bytes * P.nstack);
-                                for (int n = 0; n < P.nstack; ++n)       // images beyond N are out of bounds: zero rows
-                                    tma_load_4d(sA + as * a.a_slot_bytes + n * P.hs * P.sbo_a[slot], &P.tm[pl], c * P.KCH,
-                                                w0 + P.par_px[slot], h0 + P.par_py[slot], tc.img0 + n * P.wsets, bar_a_full + 8 * as);
-                            } else {
-                                mbar_expect_tx(bar_a_full + 8 * as, (uint32_t)P.stage_bytes[slot]);
-                                tma_load_4d(sA + as * a.a_slot_bytes, &P.tm[pl], c * P.KCH, w0 + P.par_px[slot], h0 + P.par_py[slot],
-                                            tc.img0, bar_a_full + 8 * as);
-                            }
-                            aph ^= 1u << as;
-                            if (++as == a.na_stages) as = 0;
+                        mbar_wait(bar_a_empty + 8 * as, ((aph >> as) & 1u) ^ 1u);
+                        if (P.nstack > 1) {
+                            const uint32_t box_bytes = (uint32_t)(P.box_h * P.sbo_a[slot]);
+                            mbar_expect_tx(bar_a_full + 8 * as, box_bytes * P.nstack);
+                            for (int n = 0; n < P.nstack; ++n)       // images beyond N are out of bounds: zero rows
+                                tma_load_4d(sA + as * a.a_slot_bytes + n * P.hs * P.sbo_a[slot], &P.tm[0], c * P.KCH,
+                                            w0 + P.par_px[slot], h0 + P.par_py[slot], tc.img0 + n * P.wsets, bar_a_full + 8 * as);
+                        } else {
+                            mbar_expect_tx(bar_a_full + 8 * as, (uint32_t)P.stage_bytes[slot]);
+                            tma_load_4d(sA + as * a.a_slot_bytes, &P.tm[0], c * P.KCH, w0 + P.par_px[slot], h0 + P.par_py[slot],
+                                        tc.img0, bar_a_full + 8 * as);
                         }
+                        aph ^= 1u << as;
+                        if (++as == a.na_stages) as = 0;
                         for (int t = 0; t < P.ngrp[slot]; ++t, ++b) {
                             mbar_wait(bar_b_empty + 8 * bs, ((bph >> bs) & 1u) ^ 1u);
                             mbar_expect_tx(bar_b_full + 8 * bs, (uint32_t)P.b_block_bytes);
@@ -849,9 +824,7 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
         const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
         const Smem S = {sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty};
         Ring R = {0, 0, 0u, 0u};
-        constexpr int NVMAX = NTMAX / 2;
-        float accs[EX ? 2 * NVMAX : NVMAX];    // exact: small terms then main chain; fast: the main chain
-        float sum[EX ? NVMAX : 1];             // exact: bias + residual + every closed K segment, fp32 round-to-nearest
+        float accs[kNtMaxFast / 2];                              // the main chain (the only accumulator set)
         pdl_wait();                                              // residual reads / output writes
         for (int seq = 0;; ++seq) {
             int tile = 0;
@@ -864,19 +837,12 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
             const TileCoord tc = decode_tile(P, tile - P.tile_base);
             // one tile body per N tile width make_prob can produce; every body uses a prefix of the same accumulator
             // arrays, so the widths share their registers
-#define DANET_NT_CASE(N) case N: consume_tile<EX, N>(a, P, tc, S, R, wg, w4, lane, leader, accs, sum); break;
-            if constexpr (EX) {
-                switch (P.NT) {
-                    DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64)
-                    default: __trap();
-                }
-            } else {
-                switch (P.NT) {
-                    DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64) DANET_NT_CASE(80) DANET_NT_CASE(96)
-                    DANET_NT_CASE(112) DANET_NT_CASE(128) DANET_NT_CASE(144) DANET_NT_CASE(160) DANET_NT_CASE(176) DANET_NT_CASE(192)
-                    DANET_NT_CASE(208) DANET_NT_CASE(224) DANET_NT_CASE(240) DANET_NT_CASE(256)
-                    default: __trap();
-                }
+#define DANET_NT_CASE(N) case N: consume_tile<EX, N>(a, P, tc, S, R, wg, w4, lane, leader, accs, nullptr); break;
+            switch (P.NT) {
+                DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64) DANET_NT_CASE(80) DANET_NT_CASE(96)
+                DANET_NT_CASE(112) DANET_NT_CASE(128) DANET_NT_CASE(144) DANET_NT_CASE(160) DANET_NT_CASE(176) DANET_NT_CASE(192)
+                DANET_NT_CASE(208) DANET_NT_CASE(224) DANET_NT_CASE(240) DANET_NT_CASE(256)
+                default: __trap();
             }
 #undef DANET_NT_CASE
         }
@@ -901,8 +867,19 @@ __global__ void k_absmax(long long n, const float* __restrict__ w, unsigned* __r
     for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
 }
-__global__ void k_pack_header(float scale, float* __restrict__ hdr) {
-    if (threadIdx.x < kPackHeader / 4) hdr[threadIdx.x] = threadIdx.x == 0 ? scale : (threadIdx.x == 1 ? 1.0f / scale : 0.0f);
+// k_absmax leaves the largest |w| in header word 2; k_pack_header turns it into the power-of-two scale 2^s that brings
+// it into [2^13, 2^14) -- the lo halves (2^-11 of the value) of all but the tiniest weights are then normal fp16 numbers
+// and the split keeps its 22 bits -- and writes the header; k_pack reads the scale back from the header
+__global__ void k_pack_header(float* __restrict__ hdr) {
+    __shared__ float sc;
+    if (threadIdx.x == 0) {
+        const float wmax = __uint_as_float(reinterpret_cast<const unsigned*>(hdr)[2]);
+        float scale = 1.0f;
+        if (wmax > 0.0f) { int e = 0; frexpf(wmax, &e); scale = ldexpf(1.0f, 14 - e); }
+        sc = scale;
+    }
+    __syncthreads();
+    if (threadIdx.x < kPackHeader / 4) hdr[threadIdx.x] = threadIdx.x == 0 ? sc : (threadIdx.x == 1 ? 1.0f / sc : 0.0f);
 }
 
 __device__ __forceinline__ void pack_one(const Prob& g, const float* __restrict__ w, __half* __restrict__ out, float scale) {
@@ -941,23 +918,7 @@ __device__ __forceinline__ void pack_one(const Prob& g, const float* __restrict_
     const __half h = __float2half_rn(v);
     out[i] = want_lo ? __float2half_rn(v - __half2float(h)) : h;
 }
-__global__ void k_pack(const Prob g, const float* __restrict__ w, __half* __restrict__ out, float scale) {
-    pack_one(g, w, out, scale);
-}
-// the asynchronous packing path: the largest |w| lands in header word 2 (k_absmax), k_pack_header_dev turns it into the
-// scale and writes the header exactly as the host path does, and k_pack_dev reads the scale back from the header
-__global__ void k_pack_header_dev(float* __restrict__ hdr) {
-    __shared__ float sc;
-    if (threadIdx.x == 0) {
-        const float wmax = __uint_as_float(reinterpret_cast<const unsigned*>(hdr)[2]);
-        float scale = 1.0f;
-        if (wmax > 0.0f) { int e = 0; frexpf(wmax, &e); scale = ldexpf(1.0f, 14 - e); }
-        sc = scale;
-    }
-    __syncthreads();
-    if (threadIdx.x < kPackHeader / 4) hdr[threadIdx.x] = threadIdx.x == 0 ? sc : (threadIdx.x == 1 ? 1.0f / sc : 0.0f);
-}
-__global__ void k_pack_dev(const Prob g, const float* __restrict__ w, __half* __restrict__ out, const float* __restrict__ hdr) {
+__global__ void k_pack(const Prob g, const float* __restrict__ w, __half* __restrict__ out, const float* __restrict__ hdr) {
     pack_one(g, w, out, __ldg(hdr));
 }
 
@@ -1008,10 +969,9 @@ constexpr int kSchedSlots = 1024;
 static std::mutex g_tc_mu;
 static unsigned long long g_tc_devs = 0;
 
-// geometry of every problem + the shared-memory rings of the launch
+// geometry of every problem + the shared-memory rings of the launch (1 <= n <= kMaxProb: the callers check n)
 static int configure_group(int n, const danet_conv_desc* const* descs, tc::ArgsN* a) {
     using namespace tc;
-    DANET_CHECK(n >= 1 && n <= kMaxProb, "danet_conv_tc_group: 1..%d problems per launch (got %d)", kMaxProb, n);
     memset(a, 0, sizeof(*a));
     a->nprob = n;
     for (int i = 0; i < n; ++i)
@@ -1033,6 +993,7 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
     }
     // tiles are dealt round-robin over the persistent CTAs in problem order: the problems with the most expensive
     // tiles go first, so that the long tiles start early and the cheap ones fill the tail
+    // (a stable insertion sort of a.p in place; order[i] is the caller's index of a.p[i])
     int order[kMaxProb];
     double tcost[kMaxProb];
     for (int i = 0; i < n; ++i) {
@@ -1043,12 +1004,9 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         order[i] = i;
     }
     for (int i = 1; i < n; ++i)
-        for (int j = i; j > 0 && tcost[order[j]] > tcost[order[j - 1]]; --j) { const int t = order[j]; order[j] = order[j - 1]; order[j - 1] = t; }
-    {
-        ArgsN* tmp = new ArgsN(a);
-        for (int i = 0; i < n; ++i) a.p[i] = tmp->p[order[i]];
-        delete tmp;
-    }
+        for (int j = i; j > 0 && tcost[j] > tcost[j - 1]; --j) {
+            std::swap(a.p[j], a.p[j - 1]); std::swap(tcost[j], tcost[j - 1]); std::swap(order[j], order[j - 1]);
+        }
     int base = 0;
     for (int i = 0; i < n; ++i) {
         Prob& P = a.p[i];
@@ -1158,60 +1116,27 @@ extern "C" int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt,
     tc::Prob g;
     DANET_CHECK(d && tc::make_prob(d, &g), "danet_conv_tc_pack: shape not supported by the tensor-core path");
     DANET_CHECK(w_simt && w_packed, "danet_conv_tc_pack: null pointer");
-    // power-of-two scale that brings the largest |w| into [2^13, 2^14): the lo halves (2^-11 of the value) of all but
-    // the tiniest weights are then normal fp16 numbers and the split keeps its 22 bits
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned* d_max = nullptr;
-    DANET_CUDA(cudaMalloc((void**)&d_max, 4));
-    DANET_CUDA(cudaMemsetAsync(d_max, 0, 4, st));
-    const long long nw = (long long)d->wsets * d->ksize * d->ksize * d->Cin * d->Cout;
-    tc::k_absmax<<<132, 256, 0, st>>>(nw, w_simt, d_max);
-    unsigned h_max = 0;
-    DANET_CUDA(cudaMemcpyAsync(&h_max, d_max, 4, cudaMemcpyDeviceToHost, st));
-    DANET_CUDA(cudaStreamSynchronize(st));
-    cudaFree(d_max);
-    float wmax, scale = 1.0f;
-    memcpy(&wmax, &h_max, 4);
-    if (wmax > 0.0f) {
-        int e = 0;
-        frexpf(wmax, &e);                             // wmax = m * 2^e, m in [0.5, 1)
-        scale = ldexpf(1.0f, 14 - e);                // wmax * scale in [2^13, 2^14)
-    }
-    tc::k_pack_header<<<1, 256, 0, st>>>(scale, (float*)w_packed);
-    const long long total = (long long)g.wsets * g.blocks_per_set * (g.b_block_bytes / 2);
-    tc::k_pack<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(g, w_simt, (__half*)((uint8_t*)w_packed + tc::kPackHeader), scale);
-    DANET_LAUNCH_CHECK();
-    return 0;
-}
-
-extern "C" int danet_conv_tc_pack_async(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream) {
-    tc::Prob g;
-    DANET_CHECK(d && tc::make_prob(d, &g), "danet_conv_tc_pack_async: shape not supported by the tensor-core path");
-    DANET_CHECK(w_simt && w_packed, "danet_conv_tc_pack_async: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
     unsigned* d_max = (unsigned*)w_packed + 2;         // header word 2: scratch for the absolute maximum
     DANET_CUDA(cudaMemsetAsync(d_max, 0, 4, st));
     const long long nw = (long long)d->wsets * d->ksize * d->ksize * d->Cin * d->Cout;
     tc::k_absmax<<<132, 256, 0, st>>>(nw, w_simt, d_max);
-    tc::k_pack_header_dev<<<1, 256, 0, st>>>((float*)w_packed);
+    tc::k_pack_header<<<1, 256, 0, st>>>((float*)w_packed);
     const long long total = (long long)g.wsets * g.blocks_per_set * (g.b_block_bytes / 2);
-    tc::k_pack_dev<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(g, w_simt, (__half*)((uint8_t*)w_packed + tc::kPackHeader),
-                                                                     (const float*)w_packed);
+    tc::k_pack<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(g, w_simt, (__half*)((uint8_t*)w_packed + tc::kPackHeader),
+                                                                 (const float*)w_packed);
     DANET_LAUNCH_CHECK();
     return 0;
 }
 
-extern "C" int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* subtiles, int32_t* stages) {
-    DANET_CHECK(descs && subtiles && stages, "danet_conv_tc_config: null pointer");
+extern "C" int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* stages) {
+    DANET_CHECK(descs && stages, "danet_conv_tc_config: null pointer");
     const danet_conv_desc* dp[tc::kMaxProb];
     DANET_CHECK(n >= 1 && n <= tc::kMaxProb, "danet_conv_tc_config: 1..%d problems (got %d)", tc::kMaxProb, n);
     for (int i = 0; i < n; ++i) dp[i] = &descs[i];
     tc::ArgsN* a = new tc::ArgsN();
     const int rc = configure_group(n, dp, a);
-    if (rc == 0) {
-        for (int i = 0; i < n; ++i) subtiles[i] = 1;
-        stages[0] = a->na_stages; stages[1] = a->nb_stages;
-    }
+    if (rc == 0) { stages[0] = a->na_stages; stages[1] = a->nb_stages; }
     delete a;
     return rc;
 }

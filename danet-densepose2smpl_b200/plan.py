@@ -176,15 +176,6 @@ class CudaOps(object):
         _lib.check(self.lib.danet_conv_tc_pack(ctypes.byref(c), _lib.ptr(w_simt), _lib.ptr(out), self._sp()), "conv_tc_pack")
         return out
 
-    def conv_config(self, descs):
-        """(sub-tiles per problem, (activation stages, weight stages)) of a would-be launch over `descs`."""
-        n = len(descs)
-        arr = (_lib.ConvDesc * n)(*[self._desc(d) for d in descs])
-        S = (ctypes.c_int32 * n)()
-        st = (ctypes.c_int32 * 2)()
-        _lib.check(self.lib.danet_conv_tc_config(n, arr, ctypes.cast(S, ctypes.c_void_p), ctypes.cast(st, ctypes.c_void_p)), "conv_tc_config")
-        return list(S), (st[0], st[1])
-
     # -- launches: each is one step record (`wire`) run by danet_net_run_step --------------------------
     def _run(self, name, *args):
         op, ints, floats, ptrs = wire(name, args)
@@ -385,30 +376,10 @@ class Plan(object):
         self.static_in = None
 
     def _form_groups(self, convs):
-        """Partition one level's convolutions (cost-descending) into launches of <= MAX_GROUP.  The shared-memory rings
-        of a launch are sized for its largest member, so a convolution joins a launch only if no member that carries
-        a noticeable share of the launch's work loses its sub-tile pair (S = 2 -> 1) by it."""
+        """Partition one level's convolutions (cost-descending) into consecutive launches of <= MAX_GROUP."""
         if not self.group_convs:
             return [[c] for c in convs]
-        if not hasattr(self.ops, "conv_config"):
-            return [convs[i:i + MAX_GROUP] for i in range(0, len(convs), MAX_GROUP)]
-        solo = {id(c): self.ops.conv_config([c["d"]])[0][0] for c in convs}
-        groups = []
-        for c in convs:
-            placed = False
-            for g in groups:
-                if len(g) >= MAX_GROUP:
-                    continue
-                S, _st = self.ops.conv_config([m["d"] for m in g] + [c["d"]])
-                tot = sum(m["cost"] for m in g) + c["cost"]
-                ok = all(s >= solo[id(m)] or m["cost"] < 0.05 * tot for m, s in zip(g + [c], S))
-                if ok:
-                    g.append(c)
-                    placed = True
-                    break
-            if not placed:
-                groups.append([c])
-        return groups
+        return [convs[i:i + MAX_GROUP] for i in range(0, len(convs), MAX_GROUP)]
 
     def _guard(self):
         """Kernels, buffers and the stream handle must belong to the plan's device, whatever the caller's

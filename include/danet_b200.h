@@ -232,12 +232,12 @@ typedef struct {
     const float* bias;                 /* [wsets][Cout] or NULL */
 } danet_conv_problem;
 int danet_conv_tc_group(int32_t n, const danet_conv_problem* problems, danet_stream_t stream);
-/* The launch configuration a group of n problems would get: sub-tiles per pipeline step (1 or 2) of every problem and
- * the depth of the shared activation / weight rings (stages[0], stages[1]).  The rings are sized for the largest
- * member, so a host may use this to keep a dominant problem from losing its sub-tile pair to a small companion. */
-int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* subtiles, int32_t* stages);
+/* The depth of the shared activation / weight rings (stages[0], stages[1]) a launch over a group of n problems would
+ * get; the rings are sized for the largest member.  Nonzero if the group cannot share one launch. */
+int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* stages);
 /* bytes / packing helper: converts the SIMT layout above into the swizzled shared-memory image blocks of
- * split-fp16 weights the wgmma kernel bulk-copies (device -> device, once at load). */
+ * split-fp16 weights the wgmma kernel bulk-copies (device -> device, stream-ordered, no host synchronisation or
+ * allocation: capturable in a CUDA graph).  Header word 2 of w_packed is its scratch while it runs. */
 int64_t danet_conv_tc_packed_bytes(const danet_conv_desc* d);
 int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
 int danet_conv_tc_supported(const danet_conv_desc* d);
@@ -249,9 +249,6 @@ int danet_conv_tc_geometry(const danet_conv_desc* d, int64_t* out);
  * one tile): out[0..3] = tiles per work unit, work units, weight bytes and activation bytes copied into shared memory
  * per work unit.  -1 if the shape is not supported. */
 int danet_conv_tc_cta_geometry(const danet_conv_desc* d, int64_t* out);
-/* danet_conv_tc_pack without host synchronisation or allocation (capturable in a CUDA graph), for weights that change
- * every optimiser step: the same packed bytes.  Header word 2 of w_packed is its scratch while it runs. */
-int danet_conv_tc_pack_async(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
 /* fp32 -> split-fp16 planes (lo may be NULL) and back (lo may be NULL); n elements */
 int danet_act_split(int64_t n, const float* x, void* hi, void* lo, danet_stream_t stream);
 int danet_act_merge(int64_t n, const void* hi, const void* lo, float* y, danet_stream_t stream);
@@ -263,7 +260,7 @@ int danet_act_merge(int64_t n, const void* hi, const void* lo, float* y, danet_s
  * per-group channel counts and Cout / Cin >= them the multiples of 8 of the activation planes.  No float atomics: every
  * result repeats bit for bit.  No host synchronisation: capturable in a CUDA graph.
  * ------------------------------------------------------------------------------------------ */
-/* forward weights in the SIMT layout [wsets][k*k*Cin][Cout] that danet_conv_tc_pack(_async) takes */
+/* forward weights in the SIMT layout [wsets][k*k*Cin][Cout] that danet_conv_tc_pack takes */
 int danet_conv_weights_simt(int32_t wsets, int32_t cout, int32_t cin, int32_t ksize, int32_t Cout, int32_t Cin,
                             const float* w, float* w_simt, danet_stream_t stream);
 /* Input gradient.  Output-parity class (a, b) of dx (rows a mod stride, columns b mod stride) is a stride-1

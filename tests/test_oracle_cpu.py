@@ -106,7 +106,7 @@ def test_raster_invariants(smpl_model, dp_mesh):
     assert np.abs(img1 - img).max() < 0.01
 
 
-def test_c_abi_exports_every_declared_symbol():
+def test_c_abi_v4_exports_every_declared_symbol():
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     so = os.path.join(root, "danet-densepose2smpl_b200", "libdanet_b200.so")
     if not os.path.exists(so):
@@ -122,7 +122,7 @@ def test_c_abi_exports_every_declared_symbol():
     from danet_b200 import _lib
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
     l = _lib.load()
-    assert l.danet_version() == 3
+    assert l.danet_version() == 4
 
 
 def test_product_does_not_import_oracle():
