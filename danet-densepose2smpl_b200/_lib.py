@@ -100,6 +100,7 @@ SIGNATURES = {
     "danet_conv_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),
     "danet_conv_tc_geometry": (c_int, [ctypes.POINTER(ConvDesc), c_p]),
     "danet_conv_tc_cta_geometry": (c_int, [ctypes.POINTER(ConvDesc), c_p]),
+    "danet_conv_tc_dispatch": (c_int, [ctypes.POINTER(ConvDesc), c_p]),
     "danet_conv_tc_group": (c_int, [c_int, ctypes.POINTER(ConvProblem), c_p]),
     "danet_conv_tc_config": (c_int, [c_int, ctypes.POINTER(ConvDesc), c_p]),
     "danet_conv_weights_simt": (c_int, [c_int] * 6 + [c_p, c_p, c_p]),

@@ -66,6 +66,9 @@ constexpr int kSchedDepth = 4, kSchedAhead = 2, kSchedStatic = 3;
 __host__ __device__ constexpr int kSchedConsumersOf(int ex) { return 4 * kConsumersOf(ex); }   // lane 0 of every consumer warp
 constexpr int kPackHeader = 1024;                      // packed weights start with a header: float[0] = 2^s applied to the weights, float[1] = 2^-s
 constexpr int kSegMmas = 8;                            // exact mode: close a K segment after a weight block once it holds >= 8 main-chain MMAs
+// The close rule, asked after every weight block: the tile's last block always closes; seg_mmas counts the main-chain
+// MMAs since the last close, this block included.  consume_tile and danet_conv_tc_dispatch both ask here.
+__host__ __device__ constexpr bool seg_close(bool last_block, int seg_mmas) { return last_block || seg_mmas >= kSegMmas; }
 
 struct alignas(64) Prob {
     CUtensorMap tm[2];                   // input planes: hi, lo
@@ -150,11 +153,15 @@ static bool make_prob(const danet_conv_desc* d, Prob* g) {
     } else if (d->stride == 2 && g->Ho + tr_max - 1 <= kTileH / 2) {
         g->hs = g->box_h = g->Ho + tr_max - 1;
     }
-    if (g->hs < kTileH) g->nstack = kTileH / g->hs;
     // swizzle width: the widest row unless the channel count is tiny
     int swb = 128;
     const int c16 = (d->Cin + 15) / 16 * 16;
     while (swb > 32 && swb / 2 >= 2 * c16) swb /= 2;
+    // Stacked image n's box lands at shared-memory offset n * hs * Wb * SWB, and a TMA destination must be 128-byte
+    // aligned.  With 32- and 64-byte rows some heights give an odd offset (2x2 maps of <= 16 channels under a 3x3
+    // filter: 3 rows x 10 pixels x 32 bytes); those maps get a tile per image.
+    if (g->hs < kTileH && (g->hs * Wb * swb) % 128 != 0) { g->hs = kTileH; g->box_h = Hb; }
+    if (g->hs < kTileH) g->nstack = kTileH / g->hs;
     g->SWB = swb; g->KCH = swb / 2;
     g->nchunks = (d->Cin + g->KCH - 1) / g->KCH;
     g->rows_blk = g->NT * (g->exact ? 2 : 1);
@@ -253,7 +260,7 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes
 }
 // physical offset of logical byte offset `off` inside a 1024-byte-aligned swizzled region
 __host__ __device__ __forceinline__ uint32_t swz(uint32_t off, uint32_t mask) { return off ^ (((off >> 7) & mask) << 4); }
-__device__ __forceinline__ int mdiv(int x, unsigned long long m) { return (int)(((unsigned long long)(unsigned)x * m) >> 40); }
+__host__ __device__ __forceinline__ int mdiv(int x, unsigned long long m) { return (int)(((unsigned long long)(unsigned)x * m) >> 40); }
 
 // consumer side of the tile ring: one lane waits for slot `seq`, reads the tile index and frees the slot
 __device__ __forceinline__ int sched_next(uint32_t bar_full, uint32_t bar_empty, uint32_t ring, int seq) {
@@ -281,7 +288,7 @@ __device__ __forceinline__ TileCoord decode_tile(const Prob& g, int t) {
 // exact mode: tile h (0, 1) of pair pp (problem-relative); pair_count describes the pairing.  Pair index =
 // (outer * tiles_w + tw) * ntn + nt, outer = group * ceil(tiles_h / 2) + q (tile rows 2q, 2q + 1) or, with one tile
 // row, q * wsets + ws (image groups 2q wsets + ws, (2q + 1) wsets + ws).
-__device__ __forceinline__ TileCoord pair_coord(const Prob& g, int pp, int h) {
+__host__ __device__ __forceinline__ TileCoord pair_coord(const Prob& g, int pp, int h) {
     TileCoord c;
     const int r = mdiv(pp, g.m_ntn); c.nt = pp - r * g.ntn;
     const int outer = mdiv(r, g.m_tw); c.tw = r - outer * g.tiles_w;
@@ -602,7 +609,7 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
                 const bool plane_end = tg == ngrp - 1;
                 if constexpr (EX) {
                     seg_cnt += ntk * kv;
-                    const bool close = (c == nchunks - 1 && slot == npa - 1 && plane_end) || seg_cnt >= kSegMmas;
+                    const bool close = seg_close(c == nchunks - 1 && slot == npa - 1 && plane_end, seg_cnt);
                     // A parity plane's end drains too, so that its two A slots are free before the next plane's halos
                     // are loaded: with three A slots, that is what lets the next plane's lo halo in.  The chain goes on
                     // (acc stays 1) unless the K segment closes, so the MMA sequence is unchanged.
@@ -1109,6 +1116,52 @@ extern "C" int danet_conv_tc_cta_geometry(const danet_conv_desc* d, int64_t* out
     out[1] = g.exact ? tc::pair_count(g) : g.tile_count;
     out[2] = t[7];
     out[3] = t[6] * tiles;
+    return 0;
+}
+
+extern "C" int danet_conv_tc_dispatch(const danet_conv_desc* d, int64_t* out) {
+    tc::Prob g;
+    if (!d || !out || !tc::make_prob(d, &g)) return -1;
+    const int kmma = g.KCH / 16;
+    int kv_last = 0, max_ntap = 0, max_ngrp = 0;
+    // the K segments of one tile: consume_tile's (chunk, parity plane, tap group) loop and its close rule
+    int64_t closes = 0, longest = 0, at_plane_end = 0, mid_plane = 0;
+    int seg = 0;
+    for (int c = 0; c < g.nchunks; ++c) {
+        const int kreal = (g.Cin - c * g.KCH + 15) >> 4;
+        const int kv = kreal < kmma ? kreal : kmma;
+        kv_last = kv;
+        for (int slot = 0; slot < g.npa; ++slot) {
+            max_ntap = g.ntap[slot] > max_ntap ? g.ntap[slot] : max_ntap;
+            max_ngrp = g.ngrp[slot] > max_ngrp ? g.ngrp[slot] : max_ngrp;
+            for (int tg = 0; tg < g.ngrp[slot]; ++tg) {
+                const int ntk = g.TG < g.ntap[slot] - tg * g.TG ? g.TG : g.ntap[slot] - tg * g.TG;
+                const bool plane_end = tg == g.ngrp[slot] - 1;
+                const bool last = c == g.nchunks - 1 && slot == g.npa - 1 && plane_end;
+                seg += ntk * kv;
+                if (!g.exact || !tc::seg_close(last, seg)) continue;
+                ++closes;
+                longest = seg > longest ? seg : longest;
+                if (!last) ++(plane_end ? at_plane_end : mid_plane);
+                seg = 0;
+            }
+        }
+    }
+    // the tile pairs of one (tile column, N tile): pair_coord says where each second tile lies
+    int64_t pairs = 0, past = 0;
+    if (g.exact) {
+        pairs = tc::pair_count(g);
+        const int inner = g.tiles_w * g.ntn;
+        for (int64_t o = 0; o < pairs / inner; ++o) {
+            const tc::TileCoord t = tc::pair_coord(g, (int)(o * inner), 1);
+            if (g.tiles_h > 1 ? t.th >= g.tiles_h : t.img0 >= g.N) past += inner;
+        }
+    }
+    const int64_t r[DANET_CONV_DISPATCH_FIELDS] = {
+        g.NT, g.ntn, g.Cout - (g.ntn - 1) * g.NT, g.SWB, g.KCH, g.nchunks, kv_last, g.npa, max_ntap, g.TG, max_ngrp,
+        g.nstack, g.hs, g.tiles_h, g.tiles_w, g.nblk, closes, longest, at_plane_end, mid_plane,
+        g.exact ? (g.tiles_h > 1 ? 1 : 2) : 0, pairs, past};
+    for (int i = 0; i < DANET_CONV_DISPATCH_FIELDS; ++i) out[i] = r[i];
     return 0;
 }
 

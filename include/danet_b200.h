@@ -249,6 +249,21 @@ int danet_conv_tc_geometry(const danet_conv_desc* d, int64_t* out);
  * one tile): out[0..3] = tiles per work unit, work units, weight bytes and activation bytes copied into shared memory
  * per work unit.  -1 if the shape is not supported. */
 int danet_conv_tc_cta_geometry(const danet_conv_desc* d, int64_t* out);
+/* Host-only report of what the kernel will do with one problem, from the engine's own make_prob, pairing and K segment
+ * close rule (for tests that must know which tile body, swizzle, tap grouping, stacking and pairing form a shape runs):
+ *   out[0..2]   N tile width NT (the compiled tile body), N tiles, output channels in the last N tile
+ *   out[3..6]   swizzle bytes per pixel row, channels per chunk, chunks, K steps (16 channels) of the last chunk
+ *   out[7..10]  parity planes, filter taps of the largest plane, taps per weight block TG, weight blocks of that plane
+ *   out[11..14] images stacked per tile, tile rows per stacked image hs (16 without stacking), tile rows and tile
+ *               columns of a map
+ *   out[15]     weight blocks per (weight set, N tile)
+ *   out[16..19] exact mode, per tile: K segment closes, main-chain MMAs of the longest segment, closes at the end of a
+ *               parity plane other than the tile's last block, closes inside a parity plane (fast mode: 0)
+ *   out[20..22] exact mode: pairing kind (1 = tile rows 2q, 2q + 1; 2 = image groups of one weight set; fast mode 0),
+ *               tile pairs, pairs whose second tile lies past the map (it computes zeros and stores nothing)
+ * -1 if the shape is not supported. */
+#define DANET_CONV_DISPATCH_FIELDS 23
+int danet_conv_tc_dispatch(const danet_conv_desc* d, int64_t* out);
 /* fp32 -> split-fp16 planes (lo may be NULL) and back (lo may be NULL); n elements */
 int danet_act_split(int64_t n, const float* x, void* hi, void* lo, danet_stream_t stream);
 int danet_act_merge(int64_t n, const void* hi, const void* lo, float* y, danet_stream_t stream);

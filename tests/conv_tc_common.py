@@ -119,3 +119,38 @@ def run_case(case, exact, res_as_planes=False, seed=None):
     launch([p])
     torch.cuda.synchronize()
     return y.cpu(), merge(yh, yl).cpu(), ref
+
+
+def prepare(case, exact, x, w, b, res, res_kind="f32", out_kind="both"):
+    """One problem of a launch from CPU tensors, with the residual as res_kind (none | f32 | planes; fast mode's planes
+    are the hi plane alone), the outputs of out_kind (f32 | planes | both), NaN-filled, and b = None for a NULL bias.
+    Returns (problem, (y_f32, y_hi, y_lo), tensors the launch needs alive)."""
+    N, H, W, Cin, Cout, k, s = case[:7]
+    Ho, Wo = (H + 2 * (k // 2) - k) // s + 1, (W + 2 * (k // 2) - k) // s + 1
+    d = desc(case, exact)
+    xp = split(x.to(DEV), want_lo=exact)
+    wpk = pack(d, w.to(DEV))
+    bc = b.to(DEV) if b is not None else None
+    rc = res.to(DEV) if (res is not None and res_kind != "none") else None
+    rp = split(rc, want_lo=exact) if (rc is not None and res_kind == "planes") else None
+    nan = lambda dt: torch.full((N, Ho, Wo, Cout), float("nan"), dtype=dt, device=DEV)
+    y = nan(torch.float32) if out_kind in ("f32", "both") else None
+    yh = nan(torch.float16) if out_kind in ("planes", "both") else None
+    yl = nan(torch.float16) if (yh is not None and exact) else None
+    p = problem(d, xp, wpk, bc, res=rc if rp is None else None, res_planes=rp, y_f32=y,
+                y_planes=(yh, yl) if yh is not None else None)
+    return p, (y, yh, yl), (xp, wpk, bc, rc, rp)
+
+
+def collect(outs):
+    """(y_f32, y_hi, y_lo) of prepare, after the launch -> {view name: CPU tensor}: f32, hi, lo, planes (merged)"""
+    y, yh, yl = outs
+    r = {}
+    if y is not None:
+        r["f32"] = y.cpu()
+    if yh is not None:
+        r["hi"] = yh.cpu()
+        if yl is not None:
+            r["lo"] = yl.cpu()
+        r["planes"] = merge(yh, yl).cpu()
+    return r
