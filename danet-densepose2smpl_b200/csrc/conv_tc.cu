@@ -512,14 +512,55 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
         }
         return t;
     };
-    if constexpr (EX) {                   // the exact mode's running sum starts at bias + residual
+    if constexpr (EX) {
+        // The exact mode's running sum starts at bias + residual, before the tile's first MMA.  The loads of two channel
+        // groups are issued together and the adds follow (init_term's adds, in its order), so that the loads' latencies
+        // overlap instead of adding up (with init_term per output, every bias and residual load was waited for before
+        // the next one was issued).  q holds the residual of output (j, r): an fp32 pair, or the hi and lo half2 words.
+        // Two groups at a time: the accumulators are live here, and a larger q spills.
+        const float* const bias = P.bias;
+        const float* const rf = P.res_f;
+        const __half* const rh = P.res_hi;
+        const __half* const rl = P.res_lo;
+        constexpr int kJ = 2;                         // nj = NT / 8 is even
 #pragma unroll
-        for (int j = 0; j < nj; ++j)
+        for (int j0 = 0; j0 < nj; j0 += kJ) {
+            uint32_t q[4 * kJ];
 #pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const float2 t = init_term(j, r);
-                sum[4 * j + 2 * r] = t.x * wsc.x; sum[4 * j + 2 * r + 1] = t.y * wsc.x;
-            }
+            for (int j = j0; j < j0 + kJ; ++j)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int i = 4 * j + 2 * r, k = i - 4 * j0;
+                    const bool in = 8 * j < cw && ok[r];
+                    float2 b = make_float2(0.f, 0.f);
+                    if (8 * j < cw && bias) b = __ldg(reinterpret_cast<const float2*>(bias + boff + 8 * j));
+                    sum[i] = b.x; sum[i + 1] = b.y;
+                    q[k] = q[k + 1] = 0u;
+                    if (in && rf) {
+                        const float2 v = __ldg(reinterpret_cast<const float2*>(rf + eoff[r] + 8 * j));
+                        q[k] = __float_as_uint(v.x); q[k + 1] = __float_as_uint(v.y);
+                    } else if (in && rh) {
+                        q[k] = __ldg(reinterpret_cast<const unsigned*>(rh + eoff[r] + 8 * j));
+                        if (rl) q[k + 1] = __ldg(reinterpret_cast<const unsigned*>(rl + eoff[r] + 8 * j));
+                    }
+                }
+#pragma unroll
+            for (int j = j0; j < j0 + kJ; ++j)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int i = 4 * j + 2 * r, k = i - 4 * j0;
+                    float tx = sum[i], ty = sum[i + 1];
+                    if (8 * j < cw && ok[r]) {
+                        if (rf) { tx += __uint_as_float(q[k]); ty += __uint_as_float(q[k + 1]); }
+                        else if (rh) {
+                            const float2 h = h2_to_f2(q[k]);
+                            tx += h.x; ty += h.y;
+                            if (rl) { const float2 l = h2_to_f2(q[k + 1]); tx += l.x; ty += l.y; }
+                        }
+                    }
+                    sum[i] = tx * wsc.x; sum[i + 1] = ty * wsc.x;
+                }
+        }
     }
     using Var = std::conditional_t<EX, int, const int>;  // exact mode: warp 0 parks these while it runs the copy cursor
     Var nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
