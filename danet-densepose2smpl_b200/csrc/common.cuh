@@ -155,6 +155,11 @@ __device__ __forceinline__ void act_st1(const ActV& a, size_t e, float v) {
 }
 static inline bool act_any(const danet_act* a) { return a && (a->f32 || a->hi); }
 
+// Power-of-two scale of n floats x (conv_tc.cu), on the device: hdr[0] = 2^s and hdr[1] = 2^-s, where 2^s brings the
+// largest finite |x| into [2^13, 2^14) (1 when there is none).  hdr[2] is scratch for that maximum; hdr[2 .. words) are
+// zeroed afterwards (words <= 256).  The packed conv weights' header and the dy scale of conv_wgrad.cu use it.
+int pow2_scale(const float* x, long long n, float* hdr, int words, cudaStream_t st);
+
 // Fixed-order per-channel sums of an fp32 NCHW tensor [N][C][HW] in double (conv_wgrad.cu, k_db_partial): sum 0 =
 // sum of a (counted only where mask > 0 when mask is given); with `two`, sum 1 = sum of a * (b - b_shift[c]) (b_shift
 // may be NULL).  part receives [two ? 2 : 1][chan_sums_chunks(N, HW)][C] chunk partials, to be added in chunk order.

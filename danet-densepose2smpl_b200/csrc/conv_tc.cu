@@ -10,7 +10,7 @@
 // the reference's fp32 outputs to 1e-4.  "fast" mode issues hi*hi only.
 //
 // Structure (one persistent CTA per SM, up to kMaxProb independent convolutions -- e.g. the parallel branches of one
-// HRNet stage -- in ONE launch over a concatenated tile space; fast mode's work unit is a tile, exact mode's a tile pair):
+// HRNet stage -- in ONE launch over a concatenated space of work units: tiles in fast mode, tile pairs in exact mode):
 //   A (activations): fp16 NHWC planes in HBM.  One TMA tensor-map load (cp.async.bulk.tensor.4d, SWIZZLE_128B/64B/32B,
 //       out-of-bounds zero fill = the convolution's padding, elementStrides = 2 for the parity planes of a
 //       stride-2 convolution) brings the input HALO of a tile -- (16+k-1) x (8+k-1) pixels x <= 64 channels --
@@ -31,10 +31,11 @@
 //       bias + residual.
 //   Epilogue: each consumer thread holds 2 pixels x 2 consecutive channels per 8-channel group; ReLU, output as
 //       split-fp16 planes and/or fp32.
-//   Copies: one thread runs the tile scheduler and issues every TMA / bulk copy in the order the consumers use them.
-//       Fast mode (288 threads): a producer warp after the two consumer warpgroups.  Exact mode (512 threads): four
-//       consumer warpgroups, two per tile of a pair (two tiles with the same weight set and N tile, pair_coord), so one
-//       weight stream feeds 256 pixels.  A producer warp would be the 17th and cut every thread to 96 registers, so
+//   Kernels: one per precision mode, each with its own tile body; they share the prologue, the scheduler, the output
+//       mapping and the epilogue.  One thread runs the scheduler and issues every TMA / bulk copy in consumption order.
+//       k_conv_tc_fast (288 threads, fast_tile): a producer warp after the two consumer warpgroups.  k_conv_tc_exact
+//       (512 threads, exact_tile): four consumer warpgroups, two per tile of a pair (same weight set and N tile,
+//       pair_coord), so one weight stream feeds 256 pixels.  A 17th warp would cut every thread to 96 registers, so
 //       warp 0 issues the copies (one elected lane) where its warpgroup frees ring slots (produce).
 //   Launch: programmatic dependent launch; every mbarrier wait is bounded (traps instead of hanging).
 #include "common.cuh"
@@ -43,7 +44,6 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <mutex>
-#include <type_traits>
 #include <utility>
 #include <string.h>
 #include <math.h>
@@ -55,19 +55,18 @@ constexpr int kTileH = 16, kTileW = 8;
 // Fast mode: two consumer warpgroups (64 pixels = 8 tile rows each) and a producer warp.  Exact mode: four consumer
 // warpgroups, two per tile of a tile pair, and no producer warp (warp 0 issues the copies): 16 warps x 32 lanes x 128
 // registers fill the register file, which a 17th warp would cut to 96 registers per thread.
-__host__ __device__ constexpr int kConsumersOf(int ex) { return ex ? 4 : 2; }
-__host__ __device__ constexpr int kThreadsOf(int ex) { return ex ? 4 * 4 * 32 : (4 * 2 + 1) * 32; }
-constexpr int kWarpProd = 4 * kConsumersOf(0);         // fast mode: the producer warp follows the consumer warpgroups
+constexpr int kConsFast = 2, kThreadsFast = (4 * kConsFast + 1) * 32;
+constexpr int kWarpProd = 4 * kConsFast;               // fast mode: the producer warp follows the consumer warpgroups
+constexpr int kConsExact = 4, kThreadsExact = 4 * kConsExact * 32;
 constexpr int kNtMaxExact = 64, kNtMaxFast = 256;      // output channels per N tile: bounded by the register accumulators
 constexpr int kMaxAStages = 8, kMaxBStages = 8;
 constexpr int kSmemMax = 227 * 1024;                   // opt-in dynamic shared memory per CTA on sm_90
 constexpr int kSmemFixed = 2048;                       // barriers + 1024-byte alignment slack
 constexpr int kSchedDepth = 4, kSchedAhead = 2, kSchedStatic = 3;
-__host__ __device__ constexpr int kSchedConsumersOf(int ex) { return 4 * kConsumersOf(ex); }   // lane 0 of every consumer warp
 constexpr int kPackHeader = 1024;                      // packed weights start with a header: float[0] = 2^s applied to the weights, float[1] = 2^-s
 constexpr int kSegMmas = 8;                            // exact mode: close a K segment after a weight block once it holds >= 8 main-chain MMAs
 // The close rule, asked after every weight block: the tile's last block always closes; seg_mmas counts the main-chain
-// MMAs since the last close, this block included.  consume_tile and danet_conv_tc_dispatch both ask here.
+// MMAs since the last close, this block included.  exact_tile and danet_conv_tc_dispatch both ask here.
 __host__ __device__ constexpr bool seg_close(bool last_block, int seg_mmas) { return last_block || seg_mmas >= kSegMmas; }
 
 struct alignas(64) Prob {
@@ -83,10 +82,10 @@ struct alignas(64) Prob {
     int nstack, hs, box_h;               // small maps: nstack images share one tile; image n's rows start at group n*hs
                                          // (hs = H + pad: the zero rows between images are the TMA out-of-bounds fill)
     int bpc;                             // weight blocks per channel chunk
-    int par_py[4], par_px[4], ntap[4], ngrp[4], stage_bytes[4], sbo_a[4];
+    int par_py[4], par_px[4], ntap[4], ngrp[4], stage_bytes, sbo_a;   // a plane's halo box (the largest): bytes, row pitch
     int tapoff16[4][16];                 // smem offset (16-byte units) of each tap's shifted view inside the plane
     int tapidx[4][16];                   // original filter tap index r*ks+s (weight packing)
-    int tiles_w, tiles_h, tile_count, tile_base;
+    int tiles_w, tiles_h, tile_count;
     int rows_blk;                        // rows of one weight block per tap
     int tap_bytes, b_block_bytes, nblk;  // nblk: weight blocks per (weight set, N tile)
     long long blocks_per_set;
@@ -95,11 +94,12 @@ struct alignas(64) Prob {
 
 constexpr int kMaxProb = 6;
 struct ArgsN {
-    int nprob, total_tiles, na_stages, a_slot_bytes, nb_stages, b_slot_bytes;
-    unsigned* sched;                     // [2]: dynamic tile counter, finished-CTA counter (self-resetting); NULL = static round-robin
+    int nprob, total_units, na_stages, a_slot_bytes, nb_stages, b_slot_bytes;
+    unsigned* sched;                     // [2]: dynamic unit counter, finished-CTA counter (self-resetting); NULL = static round-robin
     Prob p[kMaxProb];
-    // exact mode's work unit, the tile pair: problem i owns pair indices pair_base[i] .. + pair_count[i] (pair_coord)
-    int pair_base[kMaxProb], pair_count[kMaxProb], total_pairs;
+    // the scheduled work units, tiles in fast mode and tile pairs (pair_coord) in exact mode: problem i owns units
+    // unit_base[i] .. + unit_count[i]
+    int unit_base[kMaxProb], unit_count[kMaxProb];
 };
 
 static unsigned long long magic40(int d) { return (1ull << 40) / (unsigned long long)d + 1ull; }
@@ -171,12 +171,11 @@ static bool make_prob(const danet_conv_desc* d, Prob* g) {
     while (tg > 1 && tg * g->tap_bytes > (g->exact ? 24 : 48) * 1024) --tg;
     g->TG = tg;
     g->b_block_bytes = (tg * g->tap_bytes + 1023) / 1024 * 1024;
+    g->stage_bytes = Hb * Wb * swb; g->sbo_a = Wb * swb;
     g->bpc = 0;
     for (int a = 0; a < 4; ++a) {
-        if (a >= g->npa) { g->par_py[a] = g->par_px[a] = g->ntap[a] = g->ngrp[a] = g->stage_bytes[a] = g->sbo_a[a] = 0;
+        if (a >= g->npa) { g->par_py[a] = g->par_px[a] = g->ntap[a] = g->ngrp[a] = 0;
                            for (int k = 0; k < 16; ++k) g->tapoff16[a][k] = g->tapidx[a][k] = 0; continue; }
-        g->stage_bytes[a] = Hb * Wb * swb;
-        g->sbo_a[a] = Wb * swb;
         g->ngrp[a] = (g->ntap[a] + tg - 1) / tg;
         g->bpc += g->ngrp[a];
         for (int k = 0; k < 16; ++k) { g->tapoff16[a][k] = 0; g->tapidx[a][k] = 0; }
@@ -195,11 +194,10 @@ static bool make_prob(const danet_conv_desc* d, Prob* g) {
     const long long tiles = groups * g->tiles_h * g->tiles_w * g->ntn;
     if (tiles >= (1 << 24) || g->wsets >= (1 << 16)) return false;
     if ((long long)d->N * g->Ho * g->Wo * d->Cout >= (1LL << 31) || (long long)d->N * d->H * d->W * d->Cin >= (1LL << 31)) return false;   // 32-bit element offsets
-    g->tile_count = (int)tiles; g->tile_base = 0;
+    g->tile_count = (int)tiles;
     g->m_ntn = magic40(g->ntn); g->m_tw = magic40(g->tiles_w); g->m_th = magic40(g->tiles_h); g->m_ws = magic40(g->wsets);
     return true;
 }
-static int max_stage_bytes(const Prob& g) { int m = 0; for (int a = 0; a < g.npa; ++a) m = g.stage_bytes[a] > m ? g.stage_bytes[a] : m; return m; }
 
 // Exact mode's tile pairs (pair_coord).  The two tiles of a pair have the same weight set and N tile, so one weight
 // stream feeds both:
@@ -221,8 +219,7 @@ static bool plan_rings(ArgsN* a) {
     int amax = 0, bmax = 0, need_a = 2, max_a = kMaxAStages;
     bool exact = false;
     for (int i = 0; i < a->nprob; ++i) {
-        const int sb = max_stage_bytes(a->p[i]);
-        amax = sb > amax ? sb : amax;
+        amax = a->p[i].stage_bytes > amax ? a->p[i].stage_bytes : amax;
         bmax = a->p[i].b_block_bytes > bmax ? a->p[i].b_block_bytes : bmax;
         if (a->p[i].exact) exact = true;
     }
@@ -262,26 +259,20 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes
 __host__ __device__ __forceinline__ uint32_t swz(uint32_t off, uint32_t mask) { return off ^ (((off >> 7) & mask) << 4); }
 __host__ __device__ __forceinline__ int mdiv(int x, unsigned long long m) { return (int)(((unsigned long long)(unsigned)x * m) >> 40); }
 
-// consumer side of the tile ring: one lane waits for slot `seq`, reads the tile index and frees the slot
-__device__ __forceinline__ int sched_next(uint32_t bar_full, uint32_t bar_empty, uint32_t ring, int seq) {
-    const int slot = seq & (kSchedDepth - 1);
-    mbar_wait(bar_full + 8 * slot, (seq / kSchedDepth) & 1);
-    int tile;
-    asm volatile("ld.shared.s32 %0, [%1];" : "=r"(tile) : "r"(ring + 4 * slot) : "memory");
-    mbar_arrive(bar_empty + 8 * slot);
-    return tile;
-}
-
 // img0: the tile's first image; stacked image n is img0 + n * wsets.  ws: the tile's weight set.
 struct TileCoord { int nt, tw, th, img0, ws; };
+// image group grp: weight set grp % wsets; with stacking, the group holds images img0, img0 + wsets, ...
+__host__ __device__ __forceinline__ void group_coord(const Prob& g, int grp, TileCoord& c) {
+    const int bg = mdiv(grp, g.m_ws);
+    c.ws = grp - bg * g.wsets;
+    c.img0 = c.ws + g.wsets * bg * g.nstack;          // = grp without stacking
+}
 __device__ __forceinline__ TileCoord decode_tile(const Prob& g, int t) {
     TileCoord c;
     int r = mdiv(t, g.m_ntn); c.nt = t - r * g.ntn;
     int r2 = mdiv(r, g.m_tw); c.tw = r - r2 * g.tiles_w;
     const int grp = mdiv(r2, g.m_th); c.th = r2 - grp * g.tiles_h;
-    const int bg = mdiv(grp, g.m_ws);
-    c.ws = grp - bg * g.wsets;
-    c.img0 = c.ws + g.wsets * bg * g.nstack;          // = grp without stacking
+    group_coord(g, grp, c);
     return c;
 }
 
@@ -302,9 +293,7 @@ __host__ __device__ __forceinline__ TileCoord pair_coord(const Prob& g, int pp, 
         grp = (2 * q + h) * g.wsets + (outer - q * g.wsets);
         c.th = 0;
     }
-    const int bg = mdiv(grp, g.m_ws);
-    c.ws = grp - bg * g.wsets;
-    c.img0 = c.ws + g.wsets * bg * g.nstack;          // = grp without stacking
+    group_coord(g, grp, c);
     return c;
 }
 
@@ -334,6 +323,30 @@ enum CursorField {
     kCurFields
 };
 static_assert(kOffCursor + 4 * kCurFields <= kOffPark && kOffPark + 4 * 32 <= 1024, "barrier region layout");
+
+// consumer side of the scheduler ring: one lane waits for entry `seq`, reads the work unit and frees the entry
+__device__ __forceinline__ int sched_next(const Smem& S, int seq) {
+    const int slot = seq & (kSchedDepth - 1);
+    mbar_wait(S.bar_a_full + kOffSchedFull + 8 * slot, (seq / kSchedDepth) & 1);
+    int unit;
+    asm volatile("ld.shared.s32 %0, [%1];" : "=r"(unit) : "r"(S.bar_a_full + kOffSchedRing + 4 * slot) : "memory");
+    mbar_arrive(S.bar_a_full + kOffSchedEmpty + 8 * slot);
+    return unit;
+}
+
+// the problem that owns work unit u (u < total_units)
+__device__ __forceinline__ int unit_prob(const ArgsN& a, int u) {
+    for (int pi = 0;; ++pi) if (u < a.unit_base[pi] + a.unit_count[pi]) return pi;
+}
+
+// The work unit that scheduler entry pub of this CTA names, total_units once they are all taken.  A CTA's first
+// kSchedStatic entries are its round-robin share (no atomic latency at start-up); later ones come from the global
+// counter, which take() increments (heaviest problems first): greedy list scheduling over heterogeneous units.
+template <class Take>
+__device__ __forceinline__ int sched_unit(const ArgsN& a, int pub, Take take) {
+    const int t = pub < kSchedStatic || !a.sched ? (int)blockIdx.x + pub * (int)gridDim.x : take() + kSchedStatic * (int)gridDim.x;
+    return t < a.total_units ? t : a.total_units;
+}
 __device__ __forceinline__ int cur_get(uint32_t cur, int f) {
     int v;
     asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(cur + 4 * f) : "memory");
@@ -360,10 +373,8 @@ __device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, i
             while (cur_get(cur, kCurPub) <= cur_get(cur, kCurSeq) + kSchedAhead && !cur_get(cur, kCurPubEnd)) {
                 const int pub = cur_get(cur, kCurPub), rs = pub & (kSchedDepth - 1);
                 mbar_wait_inl(S.bar_a_full + kOffSchedEmpty + 8 * rs, ((pub / kSchedDepth) & 1) ^ 1);
-                int t;
-                if (pub < kSchedStatic || !a.sched) t = (int)blockIdx.x + pub * (int)gridDim.x;
-                else t = __shfl_sync(0xffffffffu, atom_inc_elect(a.sched), 0) + kSchedStatic * (int)gridDim.x;
-                if (t >= a.total_pairs) { t = a.total_pairs; cur_set(cur, kCurPubEnd, 1); }
+                const int t = sched_unit(a, pub, [&] { return __shfl_sync(0xffffffffu, atom_inc_elect(a.sched), 0); });
+                if (t == a.total_units) cur_set(cur, kCurPubEnd, 1);
                 st_arrive_elect(S.bar_a_full + kOffSchedRing + 4 * rs, t, S.bar_a_full + kOffSchedFull + 8 * rs);
                 cur_set(cur, kCurPub, pub + 1);
             }
@@ -371,11 +382,10 @@ __device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, i
             asm volatile("ld.shared.s32 %0, [%1];" : "=r"(pair)
                          : "r"(S.bar_a_full + kOffSchedRing + 4 * (cur_get(cur, kCurSeq) & (kSchedDepth - 1))) : "memory");
             pair = __shfl_sync(0xffffffffu, pair, 0);            // the elected lane 0 wrote it
-            if (pair >= a.total_pairs) return;
-            int pi = 0;
-            while (pair >= a.pair_base[pi] + a.pair_count[pi]) ++pi;
+            if (pair >= a.total_units) return;
+            const int pi = unit_prob(a, pair);
             const Prob& P = a.p[pi];
-            const int pp = pair - a.pair_base[pi];
+            const int pp = pair - a.unit_base[pi];
             {
                 const TileCoord tc = pair_coord(P, pp, 0);
                 cur_set(cur, kCurH0, tc.th * kTileH * P.stride - P.pad);
@@ -399,14 +409,14 @@ __device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, i
             {
                 const int as = cur_get(cur, kCurAs);
                 mbar_wait_inl(S.bar_a_empty + 8 * as, ((cur_get(cur, kCurAph) >> as) & 1) ^ 1);
-                mbar_expect_tx_elect(S.bar_a_full + 8 * as, 2u * P.nstack * P.box_h * P.sbo_a[cur_get(cur, kCurSlot)]);
+                mbar_expect_tx_elect(S.bar_a_full + 8 * as, 2u * P.nstack * P.box_h * P.sbo_a);
             }
             // box k: the first tile's nstack images, then the second tile's (rows or images beyond the map are out of
             // bounds: zero fill).  Operands are read from the cursor right at the copy.
 #pragma unroll 1
             for (int k = 0; k < 2 * P.nstack; ++k) {
                 const int h = k >= P.nstack ? 1 : 0, n = k - h * P.nstack, slot = cur_get(cur, kCurSlot), as = cur_get(cur, kCurAs);
-                tma_load_4d_elect(S.sA + as * a.a_slot_bytes + h * (a.a_slot_bytes >> 1) + n * P.hs * P.sbo_a[slot],
+                tma_load_4d_elect(S.sA + as * a.a_slot_bytes + h * (a.a_slot_bytes >> 1) + n * P.hs * P.sbo_a,
                                   &P.tm[step], cur_get(cur, kCurC) * P.KCH, cur_get(cur, kCurW0) + P.par_px[slot],
                                   cur_get(cur, kCurH0 + h) + P.par_py[slot], cur_get(cur, kCurImg0 + h) + n * P.wsets,
                                   S.bar_a_full + 8 * as);
@@ -446,30 +456,31 @@ __device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, i
 }
 
 // ---------------------------------------------------------------------------------------------
-// one consumer warpgroup's share of one tile, at a compile-time N tile width
+// the tile bodies: one consumer warpgroup's share of one tile, at a compile-time N tile width
 // ---------------------------------------------------------------------------------------------
-// EX: exact (1) or fast (0).  NT: the problem's N tile width (P.NT).  Every wgmma has a fixed width and a fixed
-// accumulator set, so ptxas keeps them in flight: one commit group per weight block, and the warpgroup waits only
-// for the block before it (wait_group 1) -- that block's B slot (and its A slots at the end of a parity plane) is
-// freed once the next block's MMAs are issued.  An exact-mode K segment close drains the chain (wait_group 0).
-template <int EX, int NT>
-__device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, const TileCoord tc, const Smem S, Ring& R,
-                                             int wg, int w4, int lane, bool leader, float* accs, float* sum,
-                                             int half = 0, bool prod = false) {
-    // exact mode: wg is the warpgroup's half of its tile, half the tile of the pair (its halo is the A slot's second
-    // half), prod marks warp 0, which issues the copies
-    constexpr int NV = NT / 2;            // fp32 accumulator registers per thread and set (64 x NT warpgroup tile)
-    constexpr int nj = NT / 8;            // 8-channel groups of the tile
-    // accumulator fragment of m64nNk16: this thread owns tile rows prow0, prow0 + 1 at column pcol, and channels
-    // 8 j + cq, 8 j + cq + 1 of every 8-channel group j (registers 4 j + 2 r + {0, 1} for row prow0 + r)
+// NT: the problem's N tile width (P.NT).  Every wgmma has a fixed width and a fixed accumulator set, so ptxas keeps
+// them in flight: one commit group per weight block, and the warpgroup waits only for the block before it (wait_group
+// 1) -- that block's B slot is freed once the next block's MMAs are issued.
+
+// the next slot of a ring: wait until it is full, flip its phase bit, advance
+__device__ __forceinline__ int ring_take(uint32_t bar_full, int& idx, uint32_t& ph, int n) {
+    const int s = idx;
+    mbar_wait_inl(bar_full + 8 * s, (ph >> s) & 1u);
+    ph ^= 1u << s; if (++idx == n) idx = 0;
+    return s;
+}
+
+// This thread's outputs in warpgroup wg's 64 pixels of a tile.  The accumulator fragment of m64nNk16 holds tile rows
+// prow0, prow0 + 1 at column pcol and channels 8 j + cq, 8 j + cq + 1 of every 8-channel group j: registers 4 j + 2 r
+// + {0, 1} for row prow0 + r.  Row prow is tile row prow of image tc.img0, or (stacked small maps) row prow % hs of image
+// tc.img0 + (prow / hs) * wsets -- rows Ho.. of a stacked image's hs rows produce no output.  eoff[r]: offset of the
+// pixel's channel tc.nt * NT + cq in the output; cw: channels of the N tile that exist (multiple of 8); boff: bias offset.
+struct TileOut { uint32_t eoff[2]; bool ok[2]; int cw, boff; };
+template <int NT>
+__device__ __forceinline__ TileOut tile_out(const Prob& P, const TileCoord& tc, int wg, int w4, int lane) {
+    TileOut o;
     const int prow0 = 8 * wg + 2 * w4, pcol = lane >> 2, cq = 2 * (lane & 3);
-    float* s = accs;                      // exact: small terms hi*lo + lo*hi
-    float* m = EX ? accs + NV : accs;     // main accumulator (fast mode: the only one)
     const int Cout = P.Cout, Wo = P.Wo, Ho = P.Ho;
-    const int cw = Cout - tc.nt * NT;     // channels of this N tile that exist (multiple of 8)
-    // this thread's two output pixels: tile row prow of image tc.img0, or (stacked small maps) row prow % hs of image
-    // tc.img0 + (prow / hs) * wsets -- rows Ho.. of a stacked image's hs rows produce no output
-    uint32_t eoff[2]; bool ok[2];
     const int ow = tc.tw * kTileW + pcol;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -481,256 +492,48 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
             oh = prow - n * P.hs; img = tc.img0 + n * P.wsets;
             row_ok = oh < Ho && n < P.nstack && img < P.N;
         }
-        ok[r] = row_ok && ow < Wo;
-        eoff[r] = ((uint32_t)(img * Ho + oh) * Wo + ow) * Cout + tc.nt * NT + cq;
+        o.ok[r] = row_ok && ow < Wo;
+        o.eoff[r] = ((uint32_t)(img * Ho + oh) * Wo + ow) * Cout + tc.nt * NT + cq;
     }
-    if constexpr (EX) {                   // the second tile of a pair without a partner: images >= N store nothing
-        if (tc.img0 >= P.N) ok[0] = ok[1] = false;
-    }
-    const int boff = tc.ws * Cout + tc.nt * NT + cq;
-    // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
-    // residual enter the sum times 2^s and the result leaves it times 2^-s -- exact in fp32
-    const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
-    // bias + residual of this thread's outputs (channel group j, row r); they enter the sum times 2^s
-    auto init_term = [&](int j, int r) {
-        float2 t = make_float2(0.f, 0.f);
-        if (8 * j < cw) {
-            if (P.bias) t = __ldg(reinterpret_cast<const float2*>(P.bias + boff + 8 * j));
-            if (ok[r]) {
-                if (P.res_f) {
-                    const float2 q = __ldg(reinterpret_cast<const float2*>(P.res_f + eoff[r] + 8 * j));
-                    t.x += q.x; t.y += q.y;
-                } else if (P.res_hi) {
-                    const float2 q = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_hi + eoff[r] + 8 * j)));
-                    t.x += q.x; t.y += q.y;
-                    if (P.res_lo) {
-                        const float2 q2 = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_lo + eoff[r] + 8 * j)));
-                        t.x += q2.x; t.y += q2.y;
-                    }
-                }
-            }
-        }
-        return t;
-    };
-    if constexpr (EX) {
-        // The exact mode's running sum starts at bias + residual, before the tile's first MMA.  The loads of two channel
-        // groups are issued together and the adds follow (init_term's adds, in its order), so that the loads' latencies
-        // overlap instead of adding up (with init_term per output, every bias and residual load was waited for before
-        // the next one was issued).  q holds the residual of output (j, r): an fp32 pair, or the hi and lo half2 words.
-        // Two groups at a time: the accumulators are live here, and a larger q spills.
-        const float* const bias = P.bias;
-        const float* const rf = P.res_f;
-        const __half* const rh = P.res_hi;
-        const __half* const rl = P.res_lo;
-        constexpr int kJ = 2;                         // nj = NT / 8 is even
+    o.cw = Cout - tc.nt * NT;
+    o.boff = tc.ws * Cout + tc.nt * NT + cq;
+    return o;
+}
+
+// The MMAs of taps k0 .. k0 + ntk - 1 of a weight block, kv K steps each (K steps wholly beyond Cin are not issued), of
+// width W into (d0, d1).  The first one overwrites the accumulators when acc is 0; returns the next acc (1).  Off: the
+// type of the caller's per-tap B stride tap16 (exact mode keeps it in an int that warp 0 can park).
+template <int W, class Off>
+__device__ __forceinline__ uint32_t mma_taps(float* d0, float* d1, uint64_t ad, uint64_t bd, const Prob& P, int slot, int k0,
+                                             int ntk, int kv, Off tap16, uint32_t acc) {
+#pragma unroll 1
+    for (int tt = 0; tt < ntk; ++tt) {
+        const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
 #pragma unroll
-        for (int j0 = 0; j0 < nj; j0 += kJ) {
-            uint32_t q[4 * kJ];
-#pragma unroll
-            for (int j = j0; j < j0 + kJ; ++j)
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const int i = 4 * j + 2 * r, k = i - 4 * j0;
-                    const bool in = 8 * j < cw && ok[r];
-                    float2 b = make_float2(0.f, 0.f);
-                    if (8 * j < cw && bias) b = __ldg(reinterpret_cast<const float2*>(bias + boff + 8 * j));
-                    sum[i] = b.x; sum[i + 1] = b.y;
-                    q[k] = q[k + 1] = 0u;
-                    if (in && rf) {
-                        const float2 v = __ldg(reinterpret_cast<const float2*>(rf + eoff[r] + 8 * j));
-                        q[k] = __float_as_uint(v.x); q[k + 1] = __float_as_uint(v.y);
-                    } else if (in && rh) {
-                        q[k] = __ldg(reinterpret_cast<const unsigned*>(rh + eoff[r] + 8 * j));
-                        if (rl) q[k + 1] = __ldg(reinterpret_cast<const unsigned*>(rl + eoff[r] + 8 * j));
-                    }
-                }
-#pragma unroll
-            for (int j = j0; j < j0 + kJ; ++j)
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const int i = 4 * j + 2 * r, k = i - 4 * j0;
-                    float tx = sum[i], ty = sum[i + 1];
-                    if (8 * j < cw && ok[r]) {
-                        if (rf) { tx += __uint_as_float(q[k]); ty += __uint_as_float(q[k + 1]); }
-                        else if (rh) {
-                            const float2 h = h2_to_f2(q[k]);
-                            tx += h.x; ty += h.y;
-                            if (rl) { const float2 l = h2_to_f2(q[k + 1]); tx += l.x; ty += l.y; }
-                        }
-                    }
-                    sum[i] = tx * wsc.x; sum[i + 1] = ty * wsc.x;
-                }
+        for (int kk = 0; kk < 4; ++kk) {
+            if (kk >= kv) break;
+            Wgmma<W>::mma(d0, d1, ad + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
+            acc = 1;
         }
     }
-    using Var = std::conditional_t<EX, int, const int>;  // exact mode: warp 0 parks these while it runs the copy cursor
-    Var nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB;
-    Var kmma = P.KCH / 16;                                // K = 16 halves (32 bytes) per MMA
-    std::conditional_t<EX, int, const uint32_t> tap16 = P.tap_bytes >> 4;
-    std::conditional_t<EX, int, const uint32_t> hi16 = EX ? (NT * SWB) >> 4 : 0;   // exact: the hi weight rows follow the NT lo rows
-    const uint64_t bd0 = make_desc(0, 8 * SWB, SWB);
-    uint32_t acc = 0;
-    int seg_cnt = 0;
-    // ring slots whose MMAs may still be in flight: freed once a later wait covers them (-1: none).  Only fast mode
-    // holds an A slot past its parity plane: exact mode drains at every plane end and frees its A slots there.
-    int pend_b = -1, pend_a = -1;
-    auto release_pending = [&]() {
-        mbar_arrive_if(S.bar_b_empty + 8 * pend_b, leader && pend_b >= 0);
-        mbar_arrive_if(S.bar_a_empty + 8 * pend_a, leader && pend_a >= 0);
-        pend_b = pend_a = -1;
-    };
-    for (int c = 0; c < nchunks; ++c) {
-        const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
-        Var kv = kreal < kmma ? kreal : kmma;             // K steps wholly beyond Cin are not issued
-        for (int slot = 0; slot < npa; ++slot) {
-            Var as_hi = R.as;
-            mbar_wait_inl(S.bar_a_full + 8 * R.as, (R.aph >> R.as) & 1u);
-            R.aph ^= 1u << R.as; if (++R.as == a.na_stages) R.as = 0;
-            int as_lo = as_hi;
-            if (EX) {
-                as_lo = R.as;
-                mbar_wait_inl(S.bar_a_full + 8 * R.as, (R.aph >> R.as) & 1u);
-                R.aph ^= 1u << R.as; if (++R.as == a.na_stages) R.as = 0;
-            }
-            // this warpgroup's 8 tile rows start 8 halo rows further down for the second warpgroup
-            const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB) + ((uint32_t)(wg * 8 * P.sbo_a[slot]) >> 4);
-            const uint64_t ad_hi = ad0 + ((S.sA + as_hi * a.a_slot_bytes) >> 4);
-            Var ngrp = P.ngrp[slot], ntap = P.ntap[slot];
-            for (int tg = 0; tg < ngrp; ++tg) {
-                const int k0 = tg * TG;
-                const int ntk = min(TG, ntap - k0);
-                const int bs = R.bs;
-                mbar_wait_inl(S.bar_b_full + 8 * bs, (R.bph >> bs) & 1u);
-                R.bph ^= 1u << bs; if (++R.bs == a.nb_stages) R.bs = 0;
-                uint64_t bd;
-                if constexpr (EX) bd = make_desc(0, 8 * SWB, SWB) + ((S.sB + bs * a.b_slot_bytes) >> 4);
-                else bd = bd0 + ((S.sB + bs * a.b_slot_bytes) >> 4);
-                wg_fence();
-                if constexpr (EX) {
-                    // the A operands: the pair's second tile is the slot's second half.  Computed here, per block,
-                    // because warp 0 parks as_hi / as_lo while it runs the copy cursor (below).
-                    const uint32_t tile_a = S.sA + half * (a.a_slot_bytes >> 1) + wg * 8 * P.sbo_a[slot];
-                    const uint64_t ad1 = make_desc(0, (uint32_t)P.sbo_a[slot], SWB);
-                    const uint64_t ad_hi = ad1 + ((tile_a + as_hi * a.a_slot_bytes) >> 4);
-                    const uint64_t ad_lo = ad1 + ((tile_a + as_lo * a.a_slot_bytes) >> 4);
-                    // hi * [lo | hi]: small terms in s, main chain in m; then lo * hi into s.  The instruction's
-                    // accumulator is (s, m) in that order: ptxas keeps the wgmmas in flight only if the lo * hi
-                    // accumulator s is the start of the wide one, not its second half.
-                    #pragma unroll 1
-                    for (int tt = 0; tt < ntk; ++tt) {
-                        const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                        #pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) {
-                            if (kk >= kv) break;
-                            Wgmma<2 * NT>::mma(s, m, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
-                            acc = 1;
-                        }
-                    }
-                    #pragma unroll 1
-                    for (int tt = 0; tt < ntk; ++tt) {
-                        const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                        #pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) {
-                            if (kk >= kv) break;
-                            Wgmma<NT>::mma(s, s + NT / 4, ad_lo + toff + 2 * kk, bd + hi16 + tt * tap16 + 2 * kk, 1u);
-                        }
-                    }
-                } else {
-                    #pragma unroll 1
-                    for (int tt = 0; tt < ntk; ++tt) {
-                        const uint32_t toff = (uint32_t)P.tapoff16[slot][k0 + tt];
-                        #pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) {
-                            if (kk >= kv) break;
-                            Wgmma<NT>::mma(m, m + NT / 4, ad_hi + toff + 2 * kk, bd + tt * tap16 + 2 * kk, acc);
-                            acc = 1;
-                        }
-                    }
-                }
-                wg_commit();
-                const bool plane_end = tg == ngrp - 1;
-                if constexpr (EX) {
-                    seg_cnt += ntk * kv;
-                    const bool close = seg_close(c == nchunks - 1 && slot == npa - 1 && plane_end, seg_cnt);
-                    // A parity plane's end drains too, so that its two A slots are free before the next plane's halos
-                    // are loaded: with three A slots, that is what lets the next plane's lo halo in.  The chain goes on
-                    // (acc stays 1) unless the K segment closes, so the MMA sequence is unchanged.
-                    const int db = pend_b >= 0 ? 1 : 0;
-                    int dA = 0, dB = db;
-                    if (close || plane_end) {
-                        wg_wait_all();
-                        reg_fence<NV>(m);
-                        reg_fence<NV>(s);
-                        if (close) {
-#pragma unroll
-                            for (int j = 0; j < NV; ++j) {
-                                sum[j] += m[j];
-                                sum[j] += s[j];
-                            }
-                            acc = 0; seg_cnt = 0;
-                        }
-                        release_pending();
-                        mbar_arrive_if(S.bar_b_empty + 8 * bs, leader);
-                        mbar_arrive_if(S.bar_a_empty + 8 * as_hi, leader && plane_end);
-                        mbar_arrive_if(S.bar_a_empty + 8 * as_lo, leader && plane_end);
-                        dA = plane_end ? 2 : 0; dB = db + 1;
-                    } else {
-                        wg_wait_1();
-                        release_pending();
-                        pend_b = bs;
-                    }
-                    if (prod) {
-                        // Warp 0 runs the copy cursor.  Its loop state waits in shared memory meanwhile: with every
-                        // accumulator live, the cursor has no registers to spare otherwise.  The reloads go through a
-                        // shuffle so that ptxas still sees warp-uniform values (a loop bound it cannot prove uniform
-                        // would serialise the wgmmas).
-                        const uint32_t pk = S.bar_a_full + kOffPark;
-                        int* const v[] = {&c, &slot, &tg, &kv, &ngrp, &ntap, &as_hi, &as_lo, &seg_cnt, &pend_b, &R.as, &R.bs,
-                                          &nchunks, &npa, &TG, &SWB, &kmma, &tap16, &hi16};
-                        constexpr int nv = sizeof(v) / sizeof(v[0]);
-#pragma unroll
-                        for (int i = 0; i < nv; ++i) cur_set(pk, i, *v[i]);
-                        cur_set(pk, nv, (int)acc); cur_set(pk, nv + 1, (int)R.aph); cur_set(pk, nv + 2, (int)R.bph);
-                        produce(a, S, dA, dB);
-#pragma unroll
-                        for (int i = 0; i < nv; ++i) *v[i] = __shfl_sync(0xffffffffu, cur_get(pk, i), 0);
-                        acc = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv), 0);
-                        R.aph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 1), 0);
-                        R.bph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 2), 0);
-                    }
-                } else {
-                    // the block before this one is done: free its slots, keep this one's until the next wait
-                    wg_wait_1();
-                    release_pending();
-                    pend_b = bs;
-                    if (plane_end) pend_a = as_hi;
-                }
-            }
-        }
-    }
-    // exact mode closed its last segment (drained) already; the wait tells ptxas that no MMA is in flight past here
-    wg_wait_all();
-    reg_fence<NV>(m);
-    if constexpr (EX) reg_fence<NV>(s);
-    release_pending();
-    // ReLU, split, store (fast mode adds bias + residual here, to the finished accumulator)
+    return acc;
+}
+
+// x 2^-s, ReLU, split, store.  value(j, r): the float2 of channel group j, row r, in the packed weights' 2^s scale.
+template <int NT, class Value>
+__device__ __forceinline__ void store_out(const Prob& P, const TileOut& o, float inv_scale, Value value) {
     const int relu = P.relu;
     float* __restrict__ y_f = P.y_f; __half* __restrict__ y_hi = P.y_hi; __half* __restrict__ y_lo = P.y_lo;
 #pragma unroll
-    for (int j = 0; j < nj; ++j) {
-        if (8 * j >= cw) continue;
+    for (int j = 0; j < NT / 8; ++j) {
+        if (8 * j >= o.cw) continue;
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-            if (!ok[r]) continue;
-            float v0, v1;
-            if constexpr (EX) { v0 = sum[4 * j + 2 * r]; v1 = sum[4 * j + 2 * r + 1]; }
-            else {
-                const float2 t = init_term(j, r);
-                v0 = m[4 * j + 2 * r]; v1 = m[4 * j + 2 * r + 1];
-                v0 += t.x * wsc.x; v1 += t.y * wsc.x;
-            }
-            float x0 = v0 * wsc.y, x1 = v1 * wsc.y;
+            if (!o.ok[r]) continue;
+            const float2 v = value(j, r);
+            float x0 = v.x * inv_scale, x1 = v.y * inv_scale;
             if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-            const uint32_t e = eoff[r] + 8 * j;
+            const uint32_t e = o.eoff[r] + 8 * j;
             if (y_f) *reinterpret_cast<float2*>(y_f + e) = make_float2(x0, x1);
             if (y_hi) {
                 const uint32_t hv = pack_h2_rn(x0, x1);
@@ -744,122 +547,366 @@ __device__ __forceinline__ void consume_tile(const ArgsN& a, const Prob& P, cons
     }
 }
 
-// ---------------------------------------------------------------------------------------------
-// the kernel
-// ---------------------------------------------------------------------------------------------
-// EX: precision mode fixed at compile time (1: every problem of the launch is exact, 0: every problem is fast).
-template <int EX>
-__global__ void __launch_bounds__(kThreadsOf(EX), 1)
-k_conv_tc(const __grid_constant__ ArgsN a) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    const uint32_t sbase = (smem_u32(smem) + 1023u) & ~1023u;          // swizzle atoms need 1024-byte alignment
-    const uint32_t sA = sbase;
-    const uint32_t sB = sbase + a.na_stages * a.a_slot_bytes;
-    const uint32_t sBar = sB + a.nb_stages * a.b_slot_bytes;
-    // barrier map (8 bytes each)
-    const uint32_t bar_a_full = sBar, bar_a_empty = sBar + 8 * kMaxAStages;
-    const uint32_t bar_b_full = sBar + 16 * kMaxAStages, bar_b_empty = bar_b_full + 8 * kMaxBStages;
-    // dynamic tile scheduler: a ring of kSchedDepth tile indices published by the producer (it takes them from a
-    // global atomic counter, heaviest problems first) and read by the consumer warps
-    const uint32_t bar_sched_full = sBar + kOffSchedFull, bar_sched_empty = sBar + kOffSchedEmpty, sched_ring = sBar + kOffSchedRing;
-    constexpr int kCons = kConsumersOf(EX);
-
-    // the warp index through a shuffle: ptxas then knows it is warp-uniform, and so is every branch on the warp role
-    // (a role branch it cannot prove uniform makes it serialise the wgmmas behind it)
-    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < a.na_stages; ++i) { mbar_init(bar_a_full + 8 * i, 1); mbar_init(bar_a_empty + 8 * i, kCons); }
-        for (int i = 0; i < a.nb_stages; ++i) { mbar_init(bar_b_full + 8 * i, 1); mbar_init(bar_b_empty + 8 * i, kCons); }
-        for (int i = 0; i < kSchedDepth; ++i) { mbar_init(bar_sched_full + 8 * i, 1); mbar_init(bar_sched_empty + 8 * i, kSchedConsumersOf(EX)); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        if constexpr (EX)
-            for (int f = 0; f < kCurFields; ++f) cur_set(sBar + kOffCursor, f, f == kCurPi ? -1 : 0);
+// Fast mode: warpgroup wg's 64 pixels (tile rows 8 wg ..) of a tile, hi * hi into the accumulator m.  Bias and residual
+// are added to the finished accumulator in the epilogue.  A parity plane's A slot is held, like a B slot, until the
+// wait after the next block.
+template <int NT>
+__device__ __forceinline__ void fast_tile(const ArgsN& a, const Prob& P, const TileCoord tc, const Smem S, Ring& R, int wg, int w4,
+                                          int lane, bool leader, float* m) {
+    constexpr int NV = NT / 2;            // fp32 accumulator registers per thread (64 x NT warpgroup tile)
+    const TileOut o = tile_out<NT>(P, tc, wg, w4, lane);
+    // the packed weights carry a power-of-two scale 2^s (so that their lo halves are normal fp16 numbers): bias and
+    // residual enter the sum times 2^s and the result leaves it times 2^-s -- exact in fp32
+    const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
+    // bias + residual of this thread's outputs (channel group j, row r)
+    auto init_term = [&](int j, int r) {
+        float2 t = make_float2(0.f, 0.f);
+        if (8 * j < o.cw) {
+            if (P.bias) t = __ldg(reinterpret_cast<const float2*>(P.bias + o.boff + 8 * j));
+            if (o.ok[r]) {
+                if (P.res_f) {
+                    const float2 q = __ldg(reinterpret_cast<const float2*>(P.res_f + o.eoff[r] + 8 * j));
+                    t.x += q.x; t.y += q.y;
+                } else if (P.res_hi) {
+                    const float2 q = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_hi + o.eoff[r] + 8 * j)));
+                    t.x += q.x; t.y += q.y;
+                    if (P.res_lo) {
+                        const float2 q2 = h2_to_f2(__ldg(reinterpret_cast<const unsigned*>(P.res_lo + o.eoff[r] + 8 * j)));
+                        t.x += q2.x; t.y += q2.y;
+                    }
+                }
+            }
+        }
+        return t;
+    };
+    const int nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB, kmma = P.KCH / 16;   // K = 16 halves per MMA
+    const uint32_t tap16 = P.tap_bytes >> 4;
+    const uint64_t bd0 = make_desc(0, 8 * SWB, SWB);
+    uint32_t acc = 0;
+    // ring slots whose MMAs may still be in flight: freed once a later wait covers them (-1: none)
+    int pend_b = -1, pend_a = -1;
+    auto release_pending = [&]() {
+        mbar_arrive_if(S.bar_b_empty + 8 * pend_b, leader && pend_b >= 0);
+        mbar_arrive_if(S.bar_a_empty + 8 * pend_a, leader && pend_a >= 0);
+        pend_b = pend_a = -1;
+    };
+    for (int c = 0; c < nchunks; ++c) {
+        const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
+        const int kv = kreal < kmma ? kreal : kmma;
+        for (int slot = 0; slot < npa; ++slot) {
+            const int as = ring_take(S.bar_a_full, R.as, R.aph, a.na_stages);
+            // this warpgroup's 8 tile rows start 8 halo rows further down for the second warpgroup
+            const uint64_t ad0 = make_desc(0, (uint32_t)P.sbo_a, SWB) + ((uint32_t)(wg * 8 * P.sbo_a) >> 4);
+            const uint64_t ad = ad0 + ((S.sA + as * a.a_slot_bytes) >> 4);
+            const int ngrp = P.ngrp[slot], ntap = P.ntap[slot];
+            for (int tg = 0; tg < ngrp; ++tg) {
+                const int k0 = tg * TG;
+                const int ntk = min(TG, ntap - k0);
+                const int bs = ring_take(S.bar_b_full, R.bs, R.bph, a.nb_stages);
+                const uint64_t bd = bd0 + ((S.sB + bs * a.b_slot_bytes) >> 4);
+                wg_fence();
+                acc = mma_taps<NT>(m, m + NT / 4, ad, bd, P, slot, k0, ntk, kv, tap16, acc);
+                wg_commit();
+                // the block before this one is done: free its slots, keep this one's until the next wait
+                wg_wait_1();
+                release_pending();
+                pend_b = bs;
+                if (tg == ngrp - 1) pend_a = as;
+            }
+        }
     }
-    if (warp == (EX ? 0 : kWarpProd) && lane < a.nprob) { tma_prefetch_desc(&a.p[lane].tm[0]); if (EX) tma_prefetch_desc(&a.p[lane].tm[1]); }
+    wg_wait_all();
+    reg_fence<NV>(m);
+    release_pending();
+    store_out<NT>(P, o, wsc.y, [&](int j, int r) {
+        const float2 t = init_term(j, r);
+        return make_float2(m[4 * j + 2 * r] + t.x * wsc.x, m[4 * j + 2 * r + 1] + t.y * wsc.x);
+    });
+}
+
+// Exact mode: warpgroup wg's 64 pixels of tile `half` of a pair (the second tile's halo is the second half of each A
+// slot); warp 0 (prod) also runs the copy cursor.  Per weight block, hi * [lo | hi] and then lo * hi: the main chain in
+// m, the small terms in s.  At every K segment close both are added to the running sum, which starts at bias + residual.
+// A parity plane's end drains too and frees its two A slots.
+template <int NT>
+__device__ __forceinline__ void exact_tile(const ArgsN& a, const Prob& P, const TileCoord tc, const Smem S, Ring& R, int wg, int w4,
+                                           int lane, bool leader, int half, bool prod, float* accs, float* sum) {
+    constexpr int NV = NT / 2, nj = NT / 8;   // accumulator registers per thread and set; 8-channel groups
+    float* s = accs;                      // small terms hi*lo + lo*hi
+    float* m = accs + NV;                 // main chain
+    TileOut o = tile_out<NT>(P, tc, wg, w4, lane);
+    if (tc.img0 >= P.N) o.ok[0] = o.ok[1] = false;       // the second tile of a pair without a partner stores nothing
+    // the packed weights' scale 2^s: bias and residual enter the sum times 2^s, the result leaves it times 2^-s
+    const float2 wsc = __ldg(reinterpret_cast<const float2*>(P.wpk));
+    {
+        // The running sum starts at bias + residual, before the tile's first MMA.  The loads of two channel groups are
+        // issued together and the adds follow, so that the loads' latencies overlap instead of adding up.  q holds the
+        // residual of output (j, r): an fp32 pair, or the hi and lo half2 words.  Two groups at a time: the accumulators
+        // are live here, and a larger q spills.
+        const float* const bias = P.bias, * const rf = P.res_f;
+        const __half* const rh = P.res_hi, * const rl = P.res_lo;
+        constexpr int kJ = 2;                         // nj = NT / 8 is even
+#pragma unroll
+        for (int j0 = 0; j0 < nj; j0 += kJ) {
+            uint32_t q[4 * kJ];
+#pragma unroll
+            for (int j = j0; j < j0 + kJ; ++j)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int i = 4 * j + 2 * r, k = i - 4 * j0;
+                    const bool in = 8 * j < o.cw && o.ok[r];
+                    float2 b = make_float2(0.f, 0.f);
+                    if (8 * j < o.cw && bias) b = __ldg(reinterpret_cast<const float2*>(bias + o.boff + 8 * j));
+                    sum[i] = b.x; sum[i + 1] = b.y;
+                    q[k] = q[k + 1] = 0u;
+                    if (in && rf) {
+                        const float2 v = __ldg(reinterpret_cast<const float2*>(rf + o.eoff[r] + 8 * j));
+                        q[k] = __float_as_uint(v.x); q[k + 1] = __float_as_uint(v.y);
+                    } else if (in && rh) {
+                        q[k] = __ldg(reinterpret_cast<const unsigned*>(rh + o.eoff[r] + 8 * j));
+                        if (rl) q[k + 1] = __ldg(reinterpret_cast<const unsigned*>(rl + o.eoff[r] + 8 * j));
+                    }
+                }
+#pragma unroll
+            for (int j = j0; j < j0 + kJ; ++j)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int i = 4 * j + 2 * r, k = i - 4 * j0;
+                    float tx = sum[i], ty = sum[i + 1];
+                    if (8 * j < o.cw && o.ok[r]) {
+                        if (rf) { tx += __uint_as_float(q[k]); ty += __uint_as_float(q[k + 1]); }
+                        else if (rh) {
+                            const float2 h = h2_to_f2(q[k]);
+                            tx += h.x; ty += h.y;
+                            if (rl) { const float2 l = h2_to_f2(q[k + 1]); tx += l.x; ty += l.y; }
+                        }
+                    }
+                    sum[i] = tx * wsc.x; sum[i + 1] = ty * wsc.x;
+                }
+        }
+    }
+    // ints, not consts: warp 0 parks these while it runs the copy cursor (below)
+    int nchunks = P.nchunks, npa = P.npa, TG = P.TG, SWB = P.SWB, kmma = P.KCH / 16;   // K = 16 halves per MMA
+    int tap16 = P.tap_bytes >> 4, hi16 = (NT * SWB) >> 4;                            // the hi weight rows follow the NT lo rows
+    uint32_t acc = 0;
+    int seg_cnt = 0;
+    int pend_b = -1;                                      // the previous block's B slot until a later wait covers it
+    for (int c = 0; c < nchunks; ++c) {
+        const int kreal = (P.Cin - c * P.KCH + 15) >> 4;
+        int kv = kreal < kmma ? kreal : kmma;
+        for (int slot = 0; slot < npa; ++slot) {
+            int as_hi = ring_take(S.bar_a_full, R.as, R.aph, a.na_stages);
+            int as_lo = ring_take(S.bar_a_full, R.as, R.aph, a.na_stages);
+            int ngrp = P.ngrp[slot], ntap = P.ntap[slot];
+            for (int tg = 0; tg < ngrp; ++tg) {
+                const int k0 = tg * TG;
+                const int ntk = min(TG, ntap - k0);
+                const int bs = ring_take(S.bar_b_full, R.bs, R.bph, a.nb_stages);
+                const uint64_t bd = make_desc(0, 8 * SWB, SWB) + ((S.sB + bs * a.b_slot_bytes) >> 4);
+                wg_fence();
+                // the A operands: the pair's second tile is the slot's second half.  Computed here, per block, because
+                // warp 0 parks as_hi / as_lo while it runs the copy cursor (below).
+                const uint32_t tile_a = S.sA + half * (a.a_slot_bytes >> 1) + wg * 8 * P.sbo_a;
+                const uint64_t ad1 = make_desc(0, (uint32_t)P.sbo_a, SWB);
+                const uint64_t ad_hi = ad1 + ((tile_a + as_hi * a.a_slot_bytes) >> 4);
+                const uint64_t ad_lo = ad1 + ((tile_a + as_lo * a.a_slot_bytes) >> 4);
+                // hi * [lo | hi]: small terms in s, main chain in m; then lo * hi into s.  The instruction's accumulator
+                // is (s, m) in that order: ptxas keeps the wgmmas in flight only if the lo * hi accumulator s is the
+                // start of the wide one, not its second half.
+                acc = mma_taps<2 * NT>(s, m, ad_hi, bd, P, slot, k0, ntk, kv, tap16, acc);
+                mma_taps<NT>(s, s + NT / 4, ad_lo, bd + hi16, P, slot, k0, ntk, kv, tap16, 1u);
+                wg_commit();
+                const bool plane_end = tg == ngrp - 1;
+                seg_cnt += ntk * kv;
+                const bool close = seg_close(c == nchunks - 1 && slot == npa - 1 && plane_end, seg_cnt);
+                // A parity plane's end drains too, so that its two A slots are free before the next plane's halos are
+                // loaded: with three A slots, that is what lets the next plane's lo halo in.  The chain goes on (acc
+                // stays 1) unless the K segment closes, so the MMA sequence is unchanged.
+                const int db = pend_b >= 0 ? 1 : 0;
+                int dA = 0, dB = db;
+                if (close || plane_end) {
+                    wg_wait_all();
+                    reg_fence<NV>(m);
+                    reg_fence<NV>(s);
+                    if (close) {
+#pragma unroll
+                        for (int j = 0; j < NV; ++j) {
+                            sum[j] += m[j];
+                            sum[j] += s[j];
+                        }
+                        acc = 0; seg_cnt = 0;
+                    }
+                    mbar_arrive_if(S.bar_b_empty + 8 * pend_b, leader && pend_b >= 0);
+                    pend_b = -1;
+                    mbar_arrive_if(S.bar_b_empty + 8 * bs, leader);
+                    mbar_arrive_if(S.bar_a_empty + 8 * as_hi, leader && plane_end);
+                    mbar_arrive_if(S.bar_a_empty + 8 * as_lo, leader && plane_end);
+                    dA = plane_end ? 2 : 0; dB = db + 1;
+                } else {
+                    wg_wait_1();
+                    mbar_arrive_if(S.bar_b_empty + 8 * pend_b, leader && pend_b >= 0);
+                    pend_b = bs;
+                }
+                if (prod) {
+                    // Warp 0 runs the copy cursor.  Its loop state waits in shared memory meanwhile: with every
+                    // accumulator live, the cursor has no registers to spare otherwise.  The reloads go through a
+                    // shuffle so that ptxas still sees warp-uniform values (a loop bound it cannot prove uniform
+                    // would serialise the wgmmas).
+                    const uint32_t pk = S.bar_a_full + kOffPark;
+                    int* const v[] = {&c, &slot, &tg, &kv, &ngrp, &ntap, &as_hi, &as_lo, &seg_cnt, &pend_b, &R.as, &R.bs,
+                                      &nchunks, &npa, &TG, &SWB, &kmma, &tap16, &hi16};
+                    constexpr int nv = sizeof(v) / sizeof(v[0]);
+#pragma unroll
+                    for (int i = 0; i < nv; ++i) cur_set(pk, i, *v[i]);
+                    cur_set(pk, nv, (int)acc); cur_set(pk, nv + 1, (int)R.aph); cur_set(pk, nv + 2, (int)R.bph);
+                    produce(a, S, dA, dB);
+#pragma unroll
+                    for (int i = 0; i < nv; ++i) *v[i] = __shfl_sync(0xffffffffu, cur_get(pk, i), 0);
+                    acc = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv), 0);
+                    R.aph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 1), 0);
+                    R.bph = (uint32_t)__shfl_sync(0xffffffffu, cur_get(pk, nv + 2), 0);
+                }
+            }
+        }
+    }
+    // the last segment closed (drained) already; the wait tells ptxas that no MMA is in flight past here
+    wg_wait_all();
+    reg_fence<NV>(m);
+    reg_fence<NV>(s);
+    store_out<NT>(P, o, wsc.y, [&](int j, int r) { return make_float2(sum[4 * j + 2 * r], sum[4 * j + 2 * r + 1]); });
+}
+
+// ---------------------------------------------------------------------------------------------
+// the kernels, one per precision mode
+// ---------------------------------------------------------------------------------------------
+// shared memory: the A ring, the B ring, then the barrier region (1024-byte aligned: the swizzle atoms need it)
+__device__ __forceinline__ Smem carve_smem(const ArgsN& a) {
+    extern __shared__ __align__(1024) uint8_t smem[];
+    const uint32_t sA = (smem_u32(smem) + 1023u) & ~1023u, sB = sA + a.na_stages * a.a_slot_bytes;
+    const uint32_t sBar = sB + a.nb_stages * a.b_slot_bytes;       // barriers: A full, A empty, B full, B empty, ...
+    return {sA, sB, sBar, sBar + 8 * kMaxAStages, sBar + 16 * kMaxAStages, sBar + 16 * kMaxAStages + 8 * kMaxBStages};
+}
+
+// the warp index through a shuffle: ptxas then knows it is warp-uniform, and so is every branch on the warp role (a
+// role branch it cannot prove uniform makes it serialise the wgmmas behind it)
+__device__ __forceinline__ int warp_index() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
+
+// Barrier set-up of both kernels.  A ring slot is freed by one arrival of each of the cons consumer warpgroups, a
+// scheduler entry by lane 0 of every consumer warp.  copy_warp, which issues the copies, prefetches the first `maps`
+// tensor maps of every problem.
+__device__ __forceinline__ void start_cta(const ArgsN& a, const Smem& S, int cons, int copy_warp, int maps, int warp, int lane) {
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < a.na_stages; ++i) { mbar_init(S.bar_a_full + 8 * i, 1); mbar_init(S.bar_a_empty + 8 * i, cons); }
+        for (int i = 0; i < a.nb_stages; ++i) { mbar_init(S.bar_b_full + 8 * i, 1); mbar_init(S.bar_b_empty + 8 * i, cons); }
+        for (int i = 0; i < kSchedDepth; ++i) { mbar_init(S.bar_a_full + kOffSchedFull + 8 * i, 1); mbar_init(S.bar_a_full + kOffSchedEmpty + 8 * i, 4 * cons); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    if (warp == copy_warp && lane < a.nprob)
+#pragma unroll
+        for (int i = 0; i < maps; ++i) tma_prefetch_desc(&a.p[lane].tm[i]);
     __syncthreads();
     pdl_launch_dependents();            // the next launch may fill SMs as our CTAs retire
+}
 
-    if constexpr (EX) {
-        // ================= exact mode: four consumer warpgroups over tile pairs; warp 0 also issues every copy =================
-        const int wg = warp >> 2, w4 = warp & 3;
-        const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
-        const bool prod = warp == 0;
-        const Smem S = {sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty};
-        Ring R = {0, 0, 0u, 0u};
-        constexpr int NVMAX = kNtMaxExact / 2;
-        float accs[2 * NVMAX];                 // small terms then main chain
-        float sum[NVMAX];                      // bias + residual + every closed K segment, fp32 round-to-nearest
-        pdl_wait();                            // activations come from the previous kernel; residual reads / output writes
-        if (prod) produce(a, S, 0, 0);         // the first copies and scheduler entries
-        for (int seq = 0;; ++seq) {
-            int pair = 0;
-            if (lane == 0) pair = sched_next(bar_sched_full, bar_sched_empty, sched_ring, seq);
-            pair = __shfl_sync(0xffffffffu, pair, 0);
-            if (pair >= a.total_pairs) break;
-            int pi = 0;
-            while (pair >= a.pair_base[pi] + a.pair_count[pi]) ++pi;
-            const Prob& P = a.p[pi];
-            // warpgroups 0, 1 take the pair's first tile, 2, 3 the second (the same tile of the next image group)
-            const int half = wg >> 1;
-            const TileCoord tc = pair_coord(P, pair - a.pair_base[pi], half);
-#define DANET_NT_CASE(N) case N: consume_tile<EX, N>(a, P, tc, S, R, wg & 1, w4, lane, leader, accs, sum, half, prod); break;
-            switch (P.NT) {
-                DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64)
-                default: __trap();
-            }
-#undef DANET_NT_CASE
+// the last CTA to finish re-arms the scheduler for the next launch (or graph replay) that uses this slot
+__device__ __forceinline__ void sched_rearm(const ArgsN& a) {
+    __syncthreads();
+    if (threadIdx.x == 0 && a.sched) {
+        __threadfence();
+        if (atomicAdd(a.sched + 1, 1u) == gridDim.x - 1) { a.sched[0] = 0u; a.sched[1] = 0u; __threadfence(); }
+    }
+}
+
+// Exact mode: four consumer warpgroups over tile pairs; warp 0 also issues every copy (produce).
+__global__ void __launch_bounds__(kThreadsExact, 1)
+k_conv_tc_exact(const __grid_constant__ ArgsN a) {
+    const Smem S = carve_smem(a);
+    const int warp = warp_index(), lane = threadIdx.x & 31;
+    if (threadIdx.x == 0)                                   // the copy cursor: no pair taken yet
+        for (int f = 0; f < kCurFields; ++f) cur_set(S.bar_a_full + kOffCursor, f, f == kCurPi ? -1 : 0);
+    start_cta(a, S, kConsExact, 0, 2, warp, lane);
+    const int wg = warp >> 2, w4 = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
+    const bool prod = warp == 0;
+    Ring R = {0, 0, 0u, 0u};
+    constexpr int NVMAX = kNtMaxExact / 2;
+    float accs[2 * NVMAX];                 // small terms then main chain
+    float sum[NVMAX];                      // bias + residual + every closed K segment, fp32 round-to-nearest
+    pdl_wait();                            // activations come from the previous kernel; residual reads / output writes
+    if (prod) produce(a, S, 0, 0);         // the first copies and scheduler entries
+    for (int seq = 0;; ++seq) {
+        int pair = 0;
+        if (lane == 0) pair = sched_next(S, seq);
+        pair = __shfl_sync(0xffffffffu, pair, 0);
+        if (pair >= a.total_units) break;
+        const int pi = unit_prob(a, pair);
+        const Prob& P = a.p[pi];
+        // warpgroups 0, 1 take the pair's first tile, 2, 3 the second (the same tile of the next image group)
+        const int half = wg >> 1;
+        const TileCoord tc = pair_coord(P, pair - a.unit_base[pi], half);
+#define DANET_NT_CASE(N) case N: exact_tile<N>(a, P, tc, S, R, wg & 1, w4, lane, leader, half, prod, accs, sum); break;
+        switch (P.NT) {
+            DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64)
+            default: __trap();
         }
-    } else if (warp == kWarpProd) {
+#undef DANET_NT_CASE
+    }
+    sched_rearm(a);
+}
+
+// Fast mode: two consumer warpgroups over tiles and a producer warp that runs the tile scheduler and issues every copy.
+__global__ void __launch_bounds__(kThreadsFast, 1)
+k_conv_tc_fast(const __grid_constant__ ArgsN a) {
+    const Smem S = carve_smem(a);
+    const int warp = warp_index(), lane = threadIdx.x & 31;
+    start_cta(a, S, kConsFast, kWarpProd, 1, warp, lane);
+    if (warp == kWarpProd) {
         // ================= producer: tile scheduler + every TMA / bulk copy, in consumption order =================
         if (lane == 0) {
             int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
-            // Tile scheduler: this thread publishes tile indices kSchedAhead tiles ahead of its own loads.  The first
-            // kSchedStatic tiles of a CTA are its round-robin share (no atomic latency at start-up), later ones come
-            // from the global counter (heaviest problems first): greedy list scheduling over heterogeneous tiles.
+            // tile scheduler: this thread publishes tile indices kSchedAhead tiles ahead of its own loads
             int pub = 0; bool ended = false;
             for (int seq = 0;; ++seq) {
                 while (pub <= seq + kSchedAhead && !ended) {
                     const int slot = pub & (kSchedDepth - 1);
-                    mbar_wait(bar_sched_empty + 8 * slot, ((pub / kSchedDepth) & 1) ^ 1);
-                    int t;
-                    if (pub < kSchedStatic || !a.sched) t = (int)blockIdx.x + pub * (int)gridDim.x;
-                    else t = (int)atomicAdd(a.sched, 1u) + kSchedStatic * (int)gridDim.x;
-                    if (t >= a.total_tiles) { t = a.total_tiles; ended = true; }
-                    asm volatile("st.shared.s32 [%0], %1;" ::"r"(sched_ring + 4 * slot), "r"(t) : "memory");
-                    mbar_arrive(bar_sched_full + 8 * slot);
+                    mbar_wait(S.bar_a_full + kOffSchedEmpty + 8 * slot, ((pub / kSchedDepth) & 1) ^ 1);
+                    const int t = sched_unit(a, pub, [&] { return (int)atomicAdd(a.sched, 1u); });
+                    ended = t == a.total_units;
+                    asm volatile("st.shared.s32 [%0], %1;" ::"r"(S.bar_a_full + kOffSchedRing + 4 * slot), "r"(t) : "memory");
+                    mbar_arrive(S.bar_a_full + kOffSchedFull + 8 * slot);
                     ++pub;
                 }
                 int tile;
-                asm volatile("ld.shared.s32 %0, [%1];" : "=r"(tile) : "r"(sched_ring + 4 * (seq & (kSchedDepth - 1))) : "memory");
-                if (tile >= a.total_tiles) break;
+                asm volatile("ld.shared.s32 %0, [%1];" : "=r"(tile) : "r"(S.bar_a_full + kOffSchedRing + 4 * (seq & (kSchedDepth - 1))) : "memory");
+                if (tile >= a.total_units) break;
                 if (seq == 0) pdl_wait();                            // activations come from the previous kernel
-                int pi = 0;
-                while (tile >= a.p[pi].tile_base + a.p[pi].tile_count) ++pi;
+                const int pi = unit_prob(a, tile);
                 const Prob& P = a.p[pi];
-                const TileCoord tc = decode_tile(P, tile - P.tile_base);
+                const TileCoord tc = decode_tile(P, tile - a.unit_base[pi]);
                 const int h0 = tc.th * kTileH * P.stride - P.pad, w0 = tc.tw * kTileW * P.stride - P.pad;
                 const uint8_t* src = P.wpk + kPackHeader + ((long long)tc.ws * P.blocks_per_set + (long long)tc.nt * P.nblk) * P.b_block_bytes;
                 int b = 0;
                 for (int c = 0; c < P.nchunks; ++c)
                     for (int slot = 0; slot < P.npa; ++slot) {
-                        mbar_wait(bar_a_empty + 8 * as, ((aph >> as) & 1u) ^ 1u);
+                        mbar_wait(S.bar_a_empty + 8 * as, ((aph >> as) & 1u) ^ 1u);
                         if (P.nstack > 1) {
-                            const uint32_t box_bytes = (uint32_t)(P.box_h * P.sbo_a[slot]);
-                            mbar_expect_tx(bar_a_full + 8 * as, box_bytes * P.nstack);
+                            const uint32_t box_bytes = (uint32_t)(P.box_h * P.sbo_a);
+                            mbar_expect_tx(S.bar_a_full + 8 * as, box_bytes * P.nstack);
                             for (int n = 0; n < P.nstack; ++n)       // images beyond N are out of bounds: zero rows
-                                tma_load_4d(sA + as * a.a_slot_bytes + n * P.hs * P.sbo_a[slot], &P.tm[0], c * P.KCH,
-                                            w0 + P.par_px[slot], h0 + P.par_py[slot], tc.img0 + n * P.wsets, bar_a_full + 8 * as);
+                                tma_load_4d(S.sA + as * a.a_slot_bytes + n * P.hs * P.sbo_a, &P.tm[0], c * P.KCH,
+                                            w0 + P.par_px[slot], h0 + P.par_py[slot], tc.img0 + n * P.wsets, S.bar_a_full + 8 * as);
                         } else {
-                            mbar_expect_tx(bar_a_full + 8 * as, (uint32_t)P.stage_bytes[slot]);
-                            tma_load_4d(sA + as * a.a_slot_bytes, &P.tm[0], c * P.KCH, w0 + P.par_px[slot], h0 + P.par_py[slot],
-                                        tc.img0, bar_a_full + 8 * as);
+                            mbar_expect_tx(S.bar_a_full + 8 * as, (uint32_t)P.stage_bytes);
+                            tma_load_4d(S.sA + as * a.a_slot_bytes, &P.tm[0], c * P.KCH, w0 + P.par_px[slot], h0 + P.par_py[slot],
+                                        tc.img0, S.bar_a_full + 8 * as);
                         }
                         aph ^= 1u << as;
                         if (++as == a.na_stages) as = 0;
                         for (int t = 0; t < P.ngrp[slot]; ++t, ++b) {
-                            mbar_wait(bar_b_empty + 8 * bs, ((bph >> bs) & 1u) ^ 1u);
-                            mbar_expect_tx(bar_b_full + 8 * bs, (uint32_t)P.b_block_bytes);
-                            bulk_g2s(sB + bs * a.b_slot_bytes, src + (long long)b * P.b_block_bytes, (uint32_t)P.b_block_bytes, bar_b_full + 8 * bs);
+                            mbar_wait(S.bar_b_empty + 8 * bs, ((bph >> bs) & 1u) ^ 1u);
+                            mbar_expect_tx(S.bar_b_full + 8 * bs, (uint32_t)P.b_block_bytes);
+                            bulk_g2s(S.sB + bs * a.b_slot_bytes, src + (long long)b * P.b_block_bytes, (uint32_t)P.b_block_bytes,
+                                     S.bar_b_full + 8 * bs);
                             bph ^= 1u << bs;
                             if (++bs == a.nb_stages) bs = 0;
                         }
@@ -870,22 +917,20 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
         // ================= consumer warpgroups: wgmma main loop + epilogue =================
         const int wg = warp >> 2, w4 = warp & 3;
         const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
-        const Smem S = {sA, sB, bar_a_full, bar_a_empty, bar_b_full, bar_b_empty};
         Ring R = {0, 0, 0u, 0u};
         float accs[kNtMaxFast / 2];                              // the main chain (the only accumulator set)
         pdl_wait();                                              // residual reads / output writes
         for (int seq = 0;; ++seq) {
             int tile = 0;
-            if (lane == 0) tile = sched_next(bar_sched_full, bar_sched_empty, sched_ring, seq);
+            if (lane == 0) tile = sched_next(S, seq);
             tile = __shfl_sync(0xffffffffu, tile, 0);
-            if (tile >= a.total_tiles) break;
-            int pi = 0;
-            while (tile >= a.p[pi].tile_base + a.p[pi].tile_count) ++pi;
+            if (tile >= a.total_units) break;
+            const int pi = unit_prob(a, tile);
             const Prob& P = a.p[pi];
-            const TileCoord tc = decode_tile(P, tile - P.tile_base);
+            const TileCoord tc = decode_tile(P, tile - a.unit_base[pi]);
             // one tile body per N tile width make_prob can produce; every body uses a prefix of the same accumulator
-            // arrays, so the widths share their registers
-#define DANET_NT_CASE(N) case N: consume_tile<EX, N>(a, P, tc, S, R, wg, w4, lane, leader, accs, nullptr); break;
+            // array, so the widths share their registers
+#define DANET_NT_CASE(N) case N: fast_tile<N>(a, P, tc, S, R, wg, w4, lane, leader, accs); break;
             switch (P.NT) {
                 DANET_NT_CASE(16) DANET_NT_CASE(32) DANET_NT_CASE(48) DANET_NT_CASE(64) DANET_NT_CASE(80) DANET_NT_CASE(96)
                 DANET_NT_CASE(112) DANET_NT_CASE(128) DANET_NT_CASE(144) DANET_NT_CASE(160) DANET_NT_CASE(176) DANET_NT_CASE(192)
@@ -895,41 +940,36 @@ k_conv_tc(const __grid_constant__ ArgsN a) {
 #undef DANET_NT_CASE
         }
     }
-    __syncthreads();
-    if (threadIdx.x == 0 && a.sched) {
-        // the last CTA to finish re-arms the scheduler for the next launch (or graph replay) that uses this slot
-        __threadfence();
-        if (atomicAdd(a.sched + 1, 1u) == gridDim.x - 1) { a.sched[0] = 0u; a.sched[1] = 0u; __threadfence(); }
+    sched_rearm(a);
+}
+
+// pow2_scale (common.cuh): k_absmax leaves the largest finite |x| in word 2 of the header, k_pow2_scale turns it into
+// the power-of-two scale 2^s that brings it into [2^13, 2^14) -- the lo halves (2^-11 of the value) of all but the
+// tiniest values are then normal fp16 numbers and the split keeps its 22 bits -- and writes the header words
+__global__ void k_absmax(long long n, const float* __restrict__ x, unsigned* __restrict__ out) {
+    unsigned m = 0;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const unsigned b = __float_as_uint(fabsf(x[i]));
+        if (b < 0x7f800000u && b > m) m = b;           // finite values only; non-negative floats order like their bit patterns
     }
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);   // a maximum: the same result in any order
+}
+__global__ void k_pow2_scale(float* __restrict__ hdr, int words) {
+    __shared__ float sc;
+    if (threadIdx.x == 0) {
+        const float amax = __uint_as_float(reinterpret_cast<const unsigned*>(hdr)[2]);
+        float scale = 1.0f;
+        if (amax > 0.0f) { int e = 0; frexpf(amax, &e); scale = ldexpf(1.0f, 14 - e); }
+        sc = scale;
+    }
+    __syncthreads();
+    if ((int)threadIdx.x < words) hdr[threadIdx.x] = threadIdx.x == 0 ? sc : (threadIdx.x == 1 ? 1.0f / sc : 0.0f);
 }
 
 // weight packing: SIMT layout [wsets][ks*ks*Cin][Cout] fp32 -> swizzled smem-image blocks of split fp16.
 // block (ws, nt, chunk, parity plane, tap group[, plane]) = [TG taps][rows][SWB bytes]; rows = output channels
-// (exact mode: NT lo rows then NT hi rows)
-__global__ void k_absmax(long long n, const float* __restrict__ w, unsigned* __restrict__ out) {
-    unsigned m = 0;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const unsigned b = __float_as_uint(fabsf(w[i]));
-        if (b < 0x7f800000u && b > m) m = b;           // finite values only; non-negative floats order like their bit patterns
-    }
-    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
-}
-// k_absmax leaves the largest |w| in header word 2; k_pack_header turns it into the power-of-two scale 2^s that brings
-// it into [2^13, 2^14) -- the lo halves (2^-11 of the value) of all but the tiniest weights are then normal fp16 numbers
-// and the split keeps its 22 bits -- and writes the header; k_pack reads the scale back from the header
-__global__ void k_pack_header(float* __restrict__ hdr) {
-    __shared__ float sc;
-    if (threadIdx.x == 0) {
-        const float wmax = __uint_as_float(reinterpret_cast<const unsigned*>(hdr)[2]);
-        float scale = 1.0f;
-        if (wmax > 0.0f) { int e = 0; frexpf(wmax, &e); scale = ldexpf(1.0f, 14 - e); }
-        sc = scale;
-    }
-    __syncthreads();
-    if (threadIdx.x < kPackHeader / 4) hdr[threadIdx.x] = threadIdx.x == 0 ? sc : (threadIdx.x == 1 ? 1.0f / sc : 0.0f);
-}
-
+// (exact mode: NT lo rows then NT hi rows).  The header's scale 2^s (pow2_scale) multiplies every weight.
 __device__ __forceinline__ void pack_one(const Prob& g, const float* __restrict__ w, __half* __restrict__ out, float scale) {
     const int blk_halves = g.b_block_bytes / 2;
     const long long total = (long long)g.wsets * g.blocks_per_set * blk_halves;
@@ -988,27 +1028,15 @@ __global__ void k_act_merge(long long n, const __half* __restrict__ hi, const __
 // ---------------------------------------------------------------------------------------------
 // host: tensor maps + launch
 // ---------------------------------------------------------------------------------------------
-// the input tensor [N][H][W][Cin] fp16 as a 4-D tensor map whose box is the largest parity-plane halo of the problem
-// (all parity planes of a stride-2 problem share one map only if their boxes agree; they are encoded per slot otherwise --
-//  here every slot uses the MAXIMAL box and stage_bytes is that of the maximal box, see make_prob)
-static int encode_x(const Prob& g, const void* base, CUtensorMap* tm) {
-    PFN_encodeTiled fn = encode_fn();
-    DANET_CHECK(fn, "conv_tc: cuTensorMapEncodeTiled is not available from this driver");
-    DANET_CHECK(((uintptr_t)base & 15) == 0, "conv_tc: activation plane must be 16-byte aligned");
-    cuuint64_t gdim[4] = {(cuuint64_t)g.Cin, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.N};
-    cuuint64_t gstr[3] = {(cuuint64_t)g.Cin * 2, (cuuint64_t)g.W * g.Cin * 2, (cuuint64_t)g.H * g.W * g.Cin * 2};
-    const int Wb = g.sbo_a[0] / g.SWB, Hb = g.box_h;
-    cuuint32_t box[4] = {(cuuint32_t)g.KCH, (cuuint32_t)(g.stride * (Wb - 1) + 1), (cuuint32_t)(g.stride * (Hb - 1) + 1), 1u};
-    cuuint32_t estr[4] = {1u, (cuuint32_t)g.stride, (cuuint32_t)g.stride, 1u};
-    const CUtensorMapSwizzle sw = g.SWB == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (g.SWB == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-    const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), gdim, gstr, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    DANET_CHECK(r == CUDA_SUCCESS, "conv_tc: cuTensorMapEncodeTiled failed (%d) for [%d,%d,%d,%d] box [%u,%u,%u]", (int)r,
-                g.N, g.H, g.W, g.Cin, box[0], box[1], box[2]);
+}  // namespace tc
+
+int pow2_scale(const float* x, long long n, float* hdr, int words, cudaStream_t st) {
+    DANET_CUDA(cudaMemsetAsync(hdr + 2, 0, 4, st));
+    tc::k_absmax<<<264, 256, 0, st>>>(n, x, reinterpret_cast<unsigned*>(hdr + 2));
+    tc::k_pow2_scale<<<1, 256, 0, st>>>(hdr, words);
+    DANET_LAUNCH_CHECK();
     return 0;
 }
-
-}  // namespace tc
 
 static int g_sm_count[64];
 static unsigned* g_sched[64];              // per device: kSchedSlots x {tile counter, done counter}, zero-initialised, self-resetting
@@ -1055,7 +1083,7 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         for (int j = i; j > 0 && tcost[j] > tcost[j - 1]; --j) {
             std::swap(a.p[j], a.p[j - 1]); std::swap(tcost[j], tcost[j - 1]); std::swap(order[j], order[j - 1]);
         }
-    int base = 0;
+    int tiles = 0;
     for (int i = 0; i < n; ++i) {
         Prob& P = a.p[i];
         const danet_conv_problem& q = probs[order[i]];
@@ -1065,16 +1093,18 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         P.res_f = q.res.f32; P.res_hi = (const __half*)q.res.hi; P.res_lo = (const __half*)q.res.lo;
         if (P.res_f) { P.res_hi = nullptr; P.res_lo = nullptr; }
         P.y_f = q.y.f32; P.y_hi = (__half*)q.y.hi; P.y_lo = (__half*)q.y.lo;
-        if (encode_x(P, q.x.hi, &P.tm[0]) != 0) return -1;
-        if (P.exact) { if (encode_x(P, q.x.lo, &P.tm[1]) != 0) return -1; }
-        else P.tm[1] = P.tm[0];
-        P.tile_base = base; base += P.tile_count;
-        DANET_CHECK(base < (1 << 24), "danet_conv_tc_group: too many tiles");
-        a.pair_base[i] = a.total_pairs; a.total_pairs += pair_count(P);
-        a.pair_count[i] = a.total_pairs - a.pair_base[i];
+        // the input planes as tensor maps whose box is a parity plane's halo: KCH channels x (sbo_a / SWB) x box_h
+        // pixels.  One map serves every parity plane: make_prob sizes them all with the largest box.
+        const CUtensorMapSwizzle sw = P.SWB == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (P.SWB == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+        for (int h = 0; h < (P.exact ? 2 : 1); ++h)
+            if (encode_nhwc_f16(&P.tm[h], h ? q.x.lo : q.x.hi, P.N, P.H, P.W, P.Cin, P.KCH, P.sbo_a / P.SWB, P.box_h, sw, P.stride) != 0) return -1;
+        if (!P.exact) P.tm[1] = P.tm[0];
+        tiles += P.tile_count;
+        DANET_CHECK(tiles < (1 << 24), "danet_conv_tc_group: too many tiles");
+        a.unit_base[i] = a.total_units;
+        a.unit_count[i] = P.exact ? pair_count(P) : P.tile_count;
+        a.total_units += a.unit_count[i];
     }
-    a.total_tiles = base;
-    const int units = a.p[0].exact ? a.total_pairs : a.total_tiles;          // scheduled work units: tile pairs or tiles
     int dev = 0;
     DANET_CUDA(cudaGetDevice(&dev));
     DANET_CHECK(dev >= 0 && dev < 64, "conv_tc: device ordinal %d out of range", dev);
@@ -1082,8 +1112,8 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
         std::lock_guard<std::mutex> lk(g_tc_mu);
         if (first_use_on_current_device(&g_tc_devs) != 0) {          // function attributes are per device
             DANET_CUDA(cudaDeviceGetAttribute(&g_sm_count[dev], cudaDevAttrMultiProcessorCount, dev));
-            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+            DANET_CUDA(cudaFuncSetAttribute(k_conv_tc_exact, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
             DANET_CUDA(cudaMalloc((void**)&g_sched[dev], kSchedSlots * 2 * sizeof(unsigned)));
             DANET_CUDA(cudaMemset(g_sched[dev], 0, kSchedSlots * 2 * sizeof(unsigned)));
         }
@@ -1092,17 +1122,17 @@ int conv_tc_group_launch(int n, const danet_conv_problem* probs, cudaStream_t st
     }
     const int smem_bytes = kSmemFixed + a.na_stages * a.a_slot_bytes + a.nb_stages * a.b_slot_bytes;
     const int cap = g_sm_count[dev];
-    const int grid = units < cap ? units : cap;
+    const int grid = a.total_units < cap ? a.total_units : cap;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreadsOf(a.p[0].exact));
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(a.p[0].exact ? kThreadsExact : kThreadsFast);
     cfg.dynamicSmemBytes = smem_bytes;
     cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    if (a.p[0].exact) { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<1>, a)); }
-    else { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<0>, a)); }
+    if (a.p[0].exact) { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc_exact, a)); }
+    else { DANET_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc_fast, a)); }
     DANET_LAUNCH_CHECK();
     return 0;
 }
@@ -1137,7 +1167,7 @@ extern "C" int danet_conv_tc_geometry(const danet_conv_desc* d, int64_t* out) {
     }
     for (int s = 0; s < g.npa; ++s) {
         taps += g.ntap[s];
-        a_bytes += g.nstack > 1 ? (int64_t)g.nstack * g.box_h * g.sbo_a[s] : g.stage_bytes[s];
+        a_bytes += g.nstack > 1 ? (int64_t)g.nstack * g.box_h * g.sbo_a : g.stage_bytes;
     }
     out[0] = tc::kTileH; out[1] = tc::kTileW; out[2] = g.tile_count; out[3] = g.nstack;
     out[4] = g.exact ? 3 : 1;                                              // products per MAC (exact: hi*hi + hi*lo + lo*hi)
@@ -1211,11 +1241,9 @@ extern "C" int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt,
     DANET_CHECK(d && tc::make_prob(d, &g), "danet_conv_tc_pack: shape not supported by the tensor-core path");
     DANET_CHECK(w_simt && w_packed, "danet_conv_tc_pack: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    unsigned* d_max = (unsigned*)w_packed + 2;         // header word 2: scratch for the absolute maximum
-    DANET_CUDA(cudaMemsetAsync(d_max, 0, 4, st));
     const long long nw = (long long)d->wsets * d->ksize * d->ksize * d->Cin * d->Cout;
-    tc::k_absmax<<<132, 256, 0, st>>>(nw, w_simt, d_max);
-    tc::k_pack_header<<<1, 256, 0, st>>>((float*)w_packed);
+    const int rc = pow2_scale(w_simt, nw, (float*)w_packed, tc::kPackHeader / 4, st);
+    if (rc != 0) return rc;
     const long long total = (long long)g.wsets * g.blocks_per_set * (g.b_block_bytes / 2);
     tc::k_pack<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(g, w_simt, (__half*)((uint8_t*)w_packed + tc::kPackHeader),
                                                                  (const float*)w_packed);

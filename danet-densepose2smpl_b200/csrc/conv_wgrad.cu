@@ -279,24 +279,9 @@ __global__ void k_db_finish(const double* __restrict__ part, int nchunk, int C, 
 // ---------------------------------------------------------------------------------------------
 // dy as scaled split-fp16 planes
 // ---------------------------------------------------------------------------------------------
-// dy is scaled by the power of two 2^s that brings max |dy| into [2^13, 2^14) before the split, as the packed weights
-// are: without it the lo half of a small gradient is a subnormal (or zero) fp16 number and the split loses its 22 bits.
-// scale[0] = 2^s, scale[1] = 2^-s, scale[2] = scratch for the absolute maximum (float bits)
-__global__ void k_absmax_bits(long long n, const float* __restrict__ x, unsigned* __restrict__ out) {
-    unsigned m = 0;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const unsigned b = __float_as_uint(fabsf(x[i]));
-        if (b < 0x7f800000u && b > m) m = b;           // finite values only; non-negative floats order like their bit patterns
-    }
-    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);   // a maximum: the same result in any order
-}
-__global__ void k_grad_scale(float* __restrict__ scale) {
-    const float amax = __uint_as_float(reinterpret_cast<const unsigned*>(scale)[2]);
-    float sc = 1.0f;
-    if (amax > 0.0f) { int e = 0; frexpf(amax, &e); sc = ldexpf(1.0f, 14 - e); }
-    scale[0] = sc; scale[1] = 1.0f / sc;
-}
+// dy is scaled by the power of two 2^s that brings max |dy| into [2^13, 2^14) before the split (pow2_scale), as the
+// packed weights are: without it the lo half of a small gradient is a subnormal (or zero) fp16 number and the split
+// loses its 22 bits.  scale[0] = 2^s, scale[1] = 2^-s, scale[2] = scratch for the absolute maximum (float bits)
 __global__ void k_split_scaled(int N, int C, int HW, int Cp, const float* __restrict__ x, const float* __restrict__ scale,
                                __half* __restrict__ hi, __half* __restrict__ lo) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -417,21 +402,6 @@ __global__ void k_scatter_nchw(int N, int C, int H, int W, int Cp, int S, int Hc
     }
 }
 
-static int encode_plane(const void* base, int C, int W, int H, int N, int stride, CUtensorMap* tm) {
-    PFN_encodeTiled fn = encode_fn();
-    DANET_CHECK(fn, "conv_wgrad: cuTensorMapEncodeTiled is not available from this driver");
-    DANET_CHECK(base && ((uintptr_t)base & 15) == 0, "conv_wgrad: activation planes must be non-null and 16-byte aligned");
-    cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-    cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)kCh, (cuuint32_t)(stride * (kBox - 1) + 1), (cuuint32_t)(stride * (kBox - 1) + 1), 1u};
-    cuuint32_t estr[4] = {1u, (cuuint32_t)stride, (cuuint32_t)stride, 1u};
-    const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), gdim, gstr, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    DANET_CHECK(r == CUDA_SUCCESS, "conv_wgrad: cuTensorMapEncodeTiled failed (%d) for [%d,%d,%d,%d]", (int)r, N, H, W, C);
-    return 0;
-}
-
 }  // namespace wg
 
 static unsigned long long g_wgrad_devs = 0;
@@ -476,10 +446,11 @@ extern "C" int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout_r, int32_
     wg::Args* a = new wg::Args();
     memset(a, 0, sizeof(*a));
     int rc = 0;
-    rc |= wg::encode_plane(dy->hi, d->Cout, g.Wo, g.Ho, d->N, 1, &a->tm[0]);
-    rc |= wg::encode_plane(dy->lo, d->Cout, g.Wo, g.Ho, d->N, 1, &a->tm[1]);
-    rc |= wg::encode_plane(x->hi, d->Cin, d->W, d->H, d->N, d->stride, &a->tm[2]);
-    rc |= wg::encode_plane(x->lo, d->Cin, d->W, d->H, d->N, d->stride, &a->tm[3]);
+    // boxes of 64 channels x 8 x 8 pixels, 128-byte swizzled: dy hi, dy lo, then x hi, x lo at the convolution's stride
+    const void* planes[4] = {dy->hi, dy->lo, x->hi, x->lo};
+    for (int i = 0; i < 4; ++i)
+        rc |= tc::encode_nhwc_f16(&a->tm[i], planes[i], d->N, i < 2 ? g.Ho : d->H, i < 2 ? g.Wo : d->W, i < 2 ? d->Cout : d->Cin,
+                                  wg::kCh, wg::kBox, wg::kBox, CU_TENSOR_MAP_SWIZZLE_128B, i < 2 ? 1 : d->stride);
     if (rc != 0) { delete a; return -1; }
     a->part = (float*)workspace;
     a->Cin = d->Cin; a->Cout = d->Cout; a->ks = d->ksize; a->stride = d->stride; a->pad = d->pad; a->wsets = d->wsets;
@@ -527,9 +498,8 @@ extern "C" int danet_conv_grad_split(int32_t N, int32_t C, int32_t HW, int32_t C
     DANET_CHECK(N >= 1 && C >= 1 && HW >= 1 && Cp >= C && Cp % 8 == 0 && dy && hi && lo && scale,
                 "danet_conv_grad_split: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
-    DANET_CUDA(cudaMemsetAsync(scale + 2, 0, 4, st));
-    wg::k_absmax_bits<<<264, 256, 0, st>>>((long long)N * C * HW, dy, (unsigned*)(scale + 2));
-    wg::k_grad_scale<<<1, 1, 0, st>>>(scale);
+    const int rc = pow2_scale(dy, (long long)N * C * HW, scale, 2, st);
+    if (rc != 0) return rc;
     wg::k_split_scaled<<<(unsigned)(((long long)N * HW + 255) / 256), 256, 0, st>>>(N, C, HW, Cp, dy, scale, (__half*)hi, (__half*)lo);
     DANET_LAUNCH_CHECK();
     return 0;

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <mutex>
 #include <stdint.h>
+#include "common.cuh"
 
 namespace danet {
 namespace tc {
@@ -120,6 +121,24 @@ static PFN_encodeTiled encode_fn() {
             fn = (PFN_encodeTiled)p;
     });
     return fn;
+}
+
+// An fp16 NHWC tensor [N][H][W][C] as a 4-D tensor map.  A box reads box_c channels of box_w x box_h pixels, taking
+// every stride-th column and row (elementStrides = stride); elements outside the tensor are zero filled.
+static int encode_nhwc_f16(CUtensorMap* tm, const void* base, int N, int H, int W, int C, int box_c, int box_w, int box_h,
+                           CUtensorMapSwizzle sw, int stride) {
+    PFN_encodeTiled fn = encode_fn();
+    DANET_CHECK(fn, "cuTensorMapEncodeTiled is not available from this driver");
+    DANET_CHECK(base && ((uintptr_t)base & 15) == 0, "tensor map: activation planes must be non-null and 16-byte aligned");
+    cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+    cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+    cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)(stride * (box_w - 1) + 1), (cuuint32_t)(stride * (box_h - 1) + 1), 1u};
+    cuuint32_t estr[4] = {1u, (cuuint32_t)stride, (cuuint32_t)stride, 1u};
+    const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), gdim, gstr, box, estr,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    DANET_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) for [%d,%d,%d,%d] box [%u,%u,%u]", (int)r, N, H, W, C,
+                box[0], box[1], box[2]);
+    return 0;
 }
 
 }  // namespace tc

@@ -43,7 +43,7 @@ def _conv_kernels(log):
 
 def test_conv_tc_wgmma_not_serialized(ptxas_log):
     kernels = _conv_kernels(ptxas_log)
-    assert len(kernels) == 2, kernels                     # k_conv_tc<0> (fast) and k_conv_tc<1> (exact)
+    assert len(kernels) == 2, kernels                     # k_conv_tc_fast and k_conv_tc_exact
     bad = [ln for ln in ptxas_log.splitlines() if re.search(r"\(C75\d\d\)", ln) and "serialized" in ln and "k_conv_tc" in ln]
     assert not bad, "\n".join(bad)
 
