@@ -106,11 +106,11 @@ SIGNATURES = {
     "danet_conv_weights_simt": (c_int, [c_int] * 6 + [c_p, c_p, c_p]),
     "danet_conv_dgrad_pieces": (c_int, [c_int, c_int, c_p]),
     "danet_conv_dgrad_weights": (c_int, [c_int] * 5 + [c_p, c_int, c_int, c_p, c_p, c_p]),
-    "danet_conv_dgrad_scatter": (c_int, [c_int] * 9 + [c_p, ctypes.POINTER(c_p), c_p, c_p, c_p]),
+    "danet_conv_dgrad_scatter": (c_int, [c_int] * 9 + [c_p, ctypes.POINTER(c_p), c_p, c_p, c_int, c_p, c_p]),
     "danet_conv_grad_split": (c_int, [c_int] * 4 + [c_p] * 5),
     "danet_conv_wgrad_workspace_bytes": (c_i64, [ctypes.POINTER(ConvDesc)]),
     "danet_conv_wgrad": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_int, ctypes.POINTER(Act), ctypes.POINTER(Act), c_p, c_p,
-                                 c_p, c_p]),
+                                 c_p, c_p, c_p]),
     "danet_conv_bias_grad_workspace_bytes": (c_i64, [c_int, c_int, c_int]),
     "danet_conv_bias_grad": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
     "danet_bn2d_workspace_bytes": (c_i64, [c_int, c_int, c_int]),

@@ -8,9 +8,9 @@ path accepts: kernel size 1 or 3 with stride 1 or 2, or 7 with stride 2; padding
 cover every convolution of the network.  Anything else raises ValueError; there is no fall-back to torch.  Channel counts
 need not be multiples of 8: the op pads them internally.
 
-- Forward: x becomes split-fp16 NHWC planes (danet_nchw_to_nhwc), the current weights are packed on every call
-  (danet_conv_tc_pack: they change every optimiser step), danet_conv_tc_group runs the convolution, and
-  danet_conv_dgrad_scatter writes the fp32 NCHW result.
+- Forward: x becomes scaled split-fp16 NHWC planes (danet_conv_grad_split), the current weights are packed on every
+  call (danet_conv_tc_pack: they change every optimiser step), danet_conv_tc_group runs the convolution without the
+  bias, and danet_conv_dgrad_scatter writes the fp32 NCHW result: x's scale removed, then the bias added.
 - Input gradient: forward problems of the same engine.  Stride 1 is conv(dy, W') with W' the rotated filter.  Stride 2
   splits each output-parity class of dx into 1x1 / 3x3 stride-1 pieces (a 4-tap 7x7/s2 parity becomes a centred 3-tap
   window plus a 1-tap piece read back shifted by one pixel), runs them as multi-problem launches and sums them into dx.
@@ -21,8 +21,10 @@ need not be multiples of 8: the op pads them internally.
 host, and forward + backward can be captured in a CUDA graph.  `groups = G` maps onto the engine's weight sets over the
 (batch, group)-flattened image axis, the lowering the inference plan uses for the reference's grouped convolutions.
 
-Precision: dy is scaled by a power of two found on the device from max |dy| before its fp16 hi + lo split, and the scale
-is removed exactly afterwards, so gradients of any magnitude keep fp32-grade relative precision.  db sums the fp32 dy."""
+Precision: x and dy are each scaled by a power of two found on the device from their max |v| before the fp16 hi + lo
+split (the weights are too, when they are packed), and the scales are removed exactly afterwards, so operands of any
+magnitude keep fp32-grade precision.  The bias never enters a scaled sum.  db sums the fp32 dy.  NaN and +-inf in x, dy
+or the weights stay non-finite in every output they reach."""
 import ctypes
 
 import torch
@@ -59,12 +61,14 @@ def _planes(shape, dev):
     return (torch.empty(shape, dtype=torch.float16, device=dev), torch.empty(shape, dtype=torch.float16, device=dev))
 
 
-def _split_nchw(lib, t, N, C, HW, Cp, shape, dev):
-    """fp32 NCHW [N, C, HW] -> split-fp16 NHWC planes [shape] with Cp >= C channels (pad channels zero)"""
+def _split_scaled(lib, t, N, C, HW, Cp, shape, dev):
+    """fp32 NCHW [N, C, HW] -> split-fp16 NHWC planes [shape] of t * 2^s with Cp >= C channels (pad channels zero), and
+    the scale [2^s, 2^-s, -, -] (danet_conv_grad_split)"""
     hi, lo = _planes(shape, dev)
-    act = _lib.Act(None, hi.data_ptr(), lo.data_ptr())
-    _lib.check(lib.danet_nchw_to_nhwc(N, C, HW, Cp, _lib.ptr(t), ctypes.byref(act), _lib.stream_ptr(dev)), "nchw_to_nhwc")
-    return hi, lo
+    scale = torch.empty(4, dtype=torch.float32, device=dev)
+    _lib.check(lib.danet_conv_grad_split(N, C, HW, Cp, _lib.ptr(t), _lib.ptr(hi), _lib.ptr(lo), _lib.ptr(scale),
+                                         _lib.stream_ptr(dev)), "conv_grad_split")
+    return (hi, lo), scale
 
 
 def _pack(lib, d, w_simt, dev):
@@ -102,12 +106,13 @@ def _pieces(lib, k, stride):
     return _PIECES[key]
 
 
-def _scatter(lib, pieces, n, maps, N, C, H, W, Cp, stride, Hc, Wc, scale, dev):
-    """NHWC piece maps -> fp32 NCHW [N, C, H, W] (summed per class, shifted, cropped, scale removed)"""
+def _scatter(lib, pieces, n, maps, N, C, H, W, Cp, stride, Hc, Wc, scale, dev, bias=None, G=1):
+    """NHWC piece maps -> fp32 NCHW [N, C, H, W] (summed per class, shifted, cropped, scale removed, then the bias
+    [G * C] of image n's group n % G added)"""
     y = torch.empty(N, C, H, W, dtype=torch.float32, device=dev)
     arr = (ctypes.c_void_p * max(n, 1))(*[m.data_ptr() for m in maps])
-    _lib.check(lib.danet_conv_dgrad_scatter(N, C, H, W, Cp, stride, Hc, Wc, n, pieces, arr, _lib.ptr(scale), _lib.ptr(y),
-                                            _lib.stream_ptr(dev)), "conv_dgrad_scatter")
+    _lib.check(lib.danet_conv_dgrad_scatter(N, C, H, W, Cp, stride, Hc, Wc, n, pieces, arr, _lib.ptr(scale), _lib.ptr(bias), G,
+                                            _lib.ptr(y), _lib.stream_ptr(dev)), "conv_dgrad_scatter")
     return y
 
 
@@ -125,29 +130,27 @@ class _Conv2d(torch.autograd.Function):
         d = _desc(N, H, W, Cinp, Coutp, k, stride, G)
         with torch.cuda.device(dev):
             sp = _lib.stream_ptr(dev)
-            xp = _split_nchw(lib, x, N, cin, H * W, Cinp, (N, H, W, Cinp), dev)
+            xp, x_scale = _split_scaled(lib, x, N, cin, H * W, Cinp, (N, H, W, Cinp), dev)
             w_simt = torch.empty(G * k * k * Cinp * Coutp, dtype=torch.float32, device=dev)
             _lib.check(lib.danet_conv_weights_simt(G, cout, cin, k, Coutp, Cinp, _lib.ptr(weight), _lib.ptr(w_simt), sp),
                        "conv_weights_simt")
             pk = _pack(lib, d, w_simt, dev)
-            bp = None
-            if bias is not None:
-                bp = torch.zeros(G, Coutp, dtype=torch.float32, device=dev)
-                bp[:, :cout].copy_(bias.view(G, cout))
+            # the engine's sum is of x * 2^s: the bias joins after the scatter has removed 2^s
             y_nhwc = torch.empty(N, Ho, Wo, Coutp, dtype=torch.float32, device=dev)
-            arr = (_lib.ConvProblem * 1)(_problem(d, xp, pk, bp, y_nhwc))
+            arr = (_lib.ConvProblem * 1)(_problem(d, xp, pk, None, y_nhwc))
             _lib.check(lib.danet_conv_tc_group(1, arr, sp), "conv_tc_group")
             one = (_lib.DgradPiece * 1)(_lib.DgradPiece(0, 0, k, 0, 0, 0, 0, 0, 0))
-            y = _scatter(lib, one, 1, [y_nhwc], N, cout, Ho, Wo, Coutp, 1, Ho, Wo, None, dev)
+            y = _scatter(lib, one, 1, [y_nhwc], N, cout, Ho, Wo, Coutp, 1, Ho, Wo, x_scale, dev, bias, G)
         need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        ctx.save_for_backward(weight if need_dx else None, xp[0] if need_dw else None, xp[1] if need_dw else None)
+        ctx.save_for_backward(weight if need_dx else None, xp[0] if need_dw else None, xp[1] if need_dw else None,
+                              x_scale if need_dw else None)
         ctx.geom = (B, Ct, H, W, Cot, cin, cout, k, stride, G, Ho, Wo)
         return y.view(B, Cot, Ho, Wo)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
-        weight, x_hi, x_lo = ctx.saved_tensors
+        weight, x_hi, x_lo, x_scale = ctx.saved_tensors
         B, Ct, H, W, Cot, cin, cout, k, stride, G, Ho, Wo = ctx.geom
         need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
         N, Cinp, Coutp = B * G, _ceil8(cin), _ceil8(cout)
@@ -159,10 +162,7 @@ class _Conv2d(torch.autograd.Function):
             gy = gy.to(torch.float32).contiguous()
             if need_dx or need_dw:
                 # dy * 2^s as split planes, 2^s from max |dy| on the device: small gradients keep their 22 bits
-                scale = torch.empty(4, dtype=torch.float32, device=dev)
-                dyp = _planes((N, Ho, Wo, Coutp), dev)
-                _lib.check(lib.danet_conv_grad_split(N, cout, Ho * Wo, Coutp, _lib.ptr(gy), _lib.ptr(dyp[0]), _lib.ptr(dyp[1]),
-                                                     _lib.ptr(scale), sp), "conv_grad_split")
+                dyp, scale = _split_scaled(lib, gy, N, cout, Ho * Wo, Coutp, (N, Ho, Wo, Coutp), dev)
             if need_dx:
                 pieces, n = _pieces(lib, k, stride)
                 probs, outs, keep = [], [], []
@@ -189,7 +189,7 @@ class _Conv2d(torch.autograd.Function):
                 xa = _lib.Act(None, x_hi.data_ptr(), x_lo.data_ptr())
                 da = _lib.Act(None, dyp[0].data_ptr(), dyp[1].data_ptr())
                 _lib.check(lib.danet_conv_wgrad(ctypes.byref(d), cout, cin, ctypes.byref(xa), ctypes.byref(da), _lib.ptr(scale),
-                                                _lib.ptr(dw), _lib.ptr(ws), sp), "conv_wgrad")
+                                                _lib.ptr(x_scale), _lib.ptr(dw), _lib.ptr(ws), sp), "conv_wgrad")
             if need_db:
                 # from the fp32 dy itself
                 ws = torch.empty(int(lib.danet_conv_bias_grad_workspace_bytes(B, Cot, Ho * Wo)), dtype=torch.uint8, device=dev)

@@ -945,7 +945,9 @@ k_conv_tc_fast(const __grid_constant__ ArgsN a) {
 
 // pow2_scale (common.cuh): k_absmax leaves the largest finite |x| in word 2 of the header, k_pow2_scale turns it into
 // the power-of-two scale 2^s that brings it into [2^13, 2^14) -- the lo halves (2^-11 of the value) of all but the
-// tiniest values are then normal fp16 numbers and the split keeps its 22 bits -- and writes the header words
+// tiniest values are then normal fp16 numbers and the split keeps its 22 bits -- and writes the header words.  s is
+// clamped to [-126, 126] so that 2^s and 2^-s are both finite, normal fp32 numbers: a maximum below 2^-112 gets the
+// largest scale there is instead of an infinite one (and a zero inverse).
 __global__ void k_absmax(long long n, const float* __restrict__ x, unsigned* __restrict__ out) {
     unsigned m = 0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -960,7 +962,7 @@ __global__ void k_pow2_scale(float* __restrict__ hdr, int words) {
     if (threadIdx.x == 0) {
         const float amax = __uint_as_float(reinterpret_cast<const unsigned*>(hdr)[2]);
         float scale = 1.0f;
-        if (amax > 0.0f) { int e = 0; frexpf(amax, &e); scale = ldexpf(1.0f, 14 - e); }
+        if (amax > 0.0f) { int e = 0; frexpf(amax, &e); scale = ldexpf(1.0f, min(max(14 - e, -126), 126)); }
         sc = scale;
     }
     __syncthreads();
@@ -1002,7 +1004,8 @@ __device__ __forceinline__ void pack_one(const Prob& g, const float* __restrict_
             if (co < g.Cout && cin < g.Cin) v = w[((size_t)ws * taps * g.Cin + (size_t)t * g.Cin + cin) * g.Cout + co] * scale;
         }
     }
-    v = fminf(fmaxf(v, -65504.f), 65504.f);
+    // every finite v is below 2^14 after the scale, so no clamp: NaN and +-inf stay NaN and +-inf (their lo half is NaN),
+    // and a diverging weight makes the convolution's output non-finite as torch's would be
     const __half h = __float2half_rn(v);
     out[i] = want_lo ? __float2half_rn(v - __half2float(h)) : h;
 }

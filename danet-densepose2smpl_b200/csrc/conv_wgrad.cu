@@ -16,9 +16,10 @@
 //       k_wgrad_finish adds the chunks in chunk order in double.  There are no float atomics, so the results repeat bit
 //       for bit.  db (channel sums of the fp32 dy) uses the same scheme: k_db_partial / k_db_finish.
 //
-// dy scale.  Gradients can be orders of magnitude below 1, where the lo half of an fp16 split is subnormal or zero.  So
-// dy is scaled by a power of two 2^s, found on the device from max |dy| (no host synchronisation), before the split
-// (k_split_scaled), and the scale is removed exactly in k_wgrad_finish and k_scatter_nchw.
+// Operand scales.  Gradients can be orders of magnitude below 1, where the lo half of an fp16 split is subnormal or zero,
+// and activations can lie far from 1 either way (past 65504 the split saturates).  So dy, and the forward's x, are each
+// scaled by a power of two 2^s, found on the device from the tensor's max |v| (no host synchronisation), before the split
+// (k_split_scaled), and the scales are removed exactly in k_wgrad_finish (both) and k_scatter_nchw (one per output).
 //
 // Input gradient.  For stride 1, dx = conv(dy, W') with W' the filter rotated by 180 degrees and Cin / Cout swapped,
 // padding k/2: a forward problem of the engine.  For stride 2, output-parity class (a, b) of dx is a stride-1
@@ -211,9 +212,11 @@ k_wgrad(const __grid_constant__ Args a) {
 }
 
 // dW in the layout of nn.Conv2d.weight with groups = wsets: [wsets * cout_r][cin_r][k][k]; chunks added in order, in
-// double, then the dy scale removed (a power of two: exact) before the one rounding to fp32
+// double, then the dy and x scales removed one after the other (powers of two: exact in double, where their product
+// could underflow in fp32) before the one rounding to fp32
 __global__ void k_wgrad_finish(const float* __restrict__ part, int nchunk, int wsets, int taps, int Cout, int Cin, int cout_r,
-                               int cin_r, const float* __restrict__ dy_scale, float* __restrict__ dW) {
+                               int cin_r, const float* __restrict__ dy_scale, const float* __restrict__ x_scale,
+                               float* __restrict__ dW) {
     const long long total = (long long)wsets * cout_r * cin_r * taps;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
@@ -226,6 +229,7 @@ __global__ void k_wgrad_finish(const float* __restrict__ part, int nchunk, int w
     double acc = 0.0;
     for (int c = 0; c < nchunk; ++c) acc += (double)p[(size_t)c * step];
     if (dy_scale) acc *= (double)__ldg(dy_scale + 1);
+    if (x_scale) acc *= (double)__ldg(x_scale + 1);
     dW[i] = (float)acc;
 }
 
@@ -277,25 +281,33 @@ __global__ void k_db_finish(const double* __restrict__ part, int nchunk, int C, 
 }
 
 // ---------------------------------------------------------------------------------------------
-// dy as scaled split-fp16 planes
+// dy (and the forward's x) as scaled split-fp16 planes
 // ---------------------------------------------------------------------------------------------
-// dy is scaled by the power of two 2^s that brings max |dy| into [2^13, 2^14) before the split (pow2_scale), as the
-// packed weights are: without it the lo half of a small gradient is a subnormal (or zero) fp16 number and the split
-// loses its 22 bits.  scale[0] = 2^s, scale[1] = 2^-s, scale[2] = scratch for the absolute maximum (float bits)
+// v is scaled by the power of two 2^s that brings max |v| into [2^13, 2^14) before the split (pow2_scale), as the
+// packed weights are: without it the lo half of a small value is a subnormal (or zero) fp16 number and the split loses
+// its 22 bits, and a value past 65504 saturates.  scale[0] = 2^s, scale[1] = 2^-s, scale[2] = scratch for the absolute
+// maximum (float bits).  Every finite scaled value is below 2^14, so the conversion does not saturate: NaN and +-inf
+// stay non-finite (a diverging step shows in every output it reaches, as it does in torch).
+__device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
 __global__ void k_split_scaled(int N, int C, int HW, int Cp, const float* __restrict__ x, const float* __restrict__ scale,
                                __half* __restrict__ hi, __half* __restrict__ lo) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)N * HW) return;
     const int n = (int)(i / HW), p = (int)(i % HW);
     const float sc = __ldg(scale);
-    ActV y; y.f = nullptr; y.hi = hi; y.lo = lo;
     for (int c = 0; c < Cp; c += 4) {                 // Cp % 8 == 0; reads coalesced across pixels
         float4 v;
         v.x = c + 0 < C ? x[((size_t)n * C + c + 0) * HW + p] * sc : 0.0f;
         v.y = c + 1 < C ? x[((size_t)n * C + c + 1) * HW + p] * sc : 0.0f;
         v.z = c + 2 < C ? x[((size_t)n * C + c + 2) * HW + p] * sc : 0.0f;
         v.w = c + 3 < C ? x[((size_t)n * C + c + 3) * HW + p] * sc : 0.0f;
-        act_st4(y, i * Cp + c, v);
+        const uint32_t h0 = pack_h2(v.x, v.y), h1 = pack_h2(v.z, v.w);
+        const float2 a = h2_to_f2(h0), b = h2_to_f2(h1);
+        *reinterpret_cast<uint2*>(hi + i * Cp + c) = make_uint2(h0, h1);
+        *reinterpret_cast<uint2*>(lo + i * Cp + c) = make_uint2(pack_h2(v.x - a.x, v.y - a.y), pack_h2(v.z - b.x, v.w - b.y));
     }
 }
 
@@ -369,19 +381,21 @@ __global__ void k_dgrad_weights(int wsets, int cout_r, int cin_r, int k, int str
 }
 
 // y[n][c][h][w] (NCHW, C real channels) = sum, in piece order, over the pieces of class (h % S, w % S) of the piece's map
-// at [n][h / S + tr][w / S + tc][c] (NHWC, Cp channels; 0 outside the map), times scale[1] when a scale is given.  A block
-// moves a 32-channel x 32-column tile of one output row through shared memory, so both the reads (channels) and the
-// writes (columns) are coalesced.
+// at [n][h / S + tr][w / S + tc][c] (NHWC, Cp channels; 0 outside the map), times scale[1] when a scale is given, plus
+// bias[(n % G) * C + c] when a bias is given (after the scale: a bias never enters a scaled sum).  A block moves a
+// 32-channel x 32-column tile of one output row through shared memory, so both the reads (channels) and the writes
+// (columns) are coalesced.
 constexpr int kMaxPieces = 9;
 struct Pieces { const float* p[kMaxPieces]; int cls[kMaxPieces], tr[kMaxPieces], tc[kMaxPieces]; int n; };
 __global__ void k_scatter_nchw(int N, int C, int H, int W, int Cp, int S, int Hc, int Wc, const __grid_constant__ Pieces pc,
-                               const float* __restrict__ scale, float* __restrict__ y) {
+                               const float* __restrict__ scale, const float* __restrict__ bias, int G, float* __restrict__ y) {
     __shared__ float tile[32][33];
     const int nh = blockIdx.x, n = nh / H, h = nh - n * H;
     const int w0 = blockIdx.y * 32, c0 = blockIdx.z * 32;
     const int tx = threadIdx.x, ty = threadIdx.y;
     const int a = h % S, u = h / S;
     const float inv = scale ? __ldg(scale + 1) : 1.0f;
+    const float* bn = bias ? bias + (size_t)(n % G) * C : nullptr;
     for (int wl = ty; wl < 32; wl += 8) {
         const int w = w0 + wl, c = c0 + tx;
         float v = 0.0f;
@@ -393,7 +407,9 @@ __global__ void k_scatter_nchw(int N, int C, int H, int W, int Cp, int S, int Hc
                     v += __ldg(pc.p[i] + (((size_t)n * Hc + uu) * Wc + vi) * Cp + c);
             }
         }
-        tile[wl][tx] = v * inv;
+        v *= inv;
+        if (bn && c < C) v += __ldg(bn + c);
+        tile[wl][tx] = v;
     }
     __syncthreads();
     for (int cl = ty; cl < 32; cl += 8) {
@@ -431,7 +447,8 @@ extern "C" int64_t danet_conv_wgrad_workspace_bytes(const danet_conv_desc* d) {
 }
 
 extern "C" int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout_r, int32_t cin_r, const danet_act* x,
-                                const danet_act* dy, const float* dy_scale, float* dW, void* workspace, danet_stream_t stream) {
+                                const danet_act* dy, const float* dy_scale, const float* x_scale, float* dW, void* workspace,
+                                danet_stream_t stream) {
     wg::Geo g;
     DANET_CHECK(d && wg::make_geo(d, &g), "danet_conv_wgrad: shape not supported (k in {1,3,7}, pad k/2, stride 1|2, "
                                           "channels %% 8, N %% wsets == 0)");
@@ -469,7 +486,7 @@ extern "C" int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout_r, int32_
     DANET_CUDA(e);
     const long long total = (long long)d->wsets * cout_r * cin_r * g.taps;
     wg::k_wgrad_finish<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float*)workspace, g.nchunk, d->wsets, g.taps, d->Cout,
-                                                                      d->Cin, cout_r, cin_r, dy_scale, dW);
+                                                                      d->Cin, cout_r, cin_r, dy_scale, x_scale, dW);
     DANET_LAUNCH_CHECK();
     return 0;
 }
@@ -551,9 +568,9 @@ extern "C" int danet_conv_dgrad_weights(int32_t wsets, int32_t cout_r, int32_t c
 
 extern "C" int danet_conv_dgrad_scatter(int32_t N, int32_t C, int32_t H, int32_t W, int32_t Cp, int32_t stride, int32_t Hc,
                                         int32_t Wc, int32_t npieces, const danet_dgrad_piece* pieces, const float* const* maps,
-                                        const float* scale, float* y, danet_stream_t stream) {
+                                        const float* scale, const float* bias, int32_t groups, float* y, danet_stream_t stream) {
     DANET_CHECK(pieces && maps && y && N >= 1 && C >= 1 && Cp >= C && H >= 1 && W >= 1 && (stride == 1 || stride == 2) &&
-                npieces >= 0 && npieces <= wg::kMaxPieces, "danet_conv_dgrad_scatter: bad arguments");
+                npieces >= 0 && npieces <= wg::kMaxPieces && groups >= 1, "danet_conv_dgrad_scatter: bad arguments");
     DANET_CHECK(Hc >= (H + stride - 1) / stride && Wc >= (W + stride - 1) / stride, "danet_conv_dgrad_scatter: maps too small");
     DANET_CHECK((long long)N * H < (1LL << 31), "danet_conv_dgrad_scatter: too many rows");
     wg::Pieces p = {};
@@ -564,7 +581,8 @@ extern "C" int danet_conv_dgrad_scatter(int32_t N, int32_t C, int32_t H, int32_t
         p.p[i] = maps[i]; p.cls[i] = pieces[i].a * stride + pieces[i].b; p.tr[i] = pieces[i].tr; p.tc[i] = pieces[i].tc;
     }
     const dim3 grid((unsigned)(N * H), (unsigned)cdiv(W, 32), (unsigned)cdiv(C, 32));
-    wg::k_scatter_nchw<<<grid, dim3(32, 8), 0, (cudaStream_t)stream>>>(N, C, H, W, Cp, stride, Hc, Wc, p, scale, y);
+    wg::k_scatter_nchw<<<grid, dim3(32, 8), 0, (cudaStream_t)stream>>>(N, C, H, W, Cp, stride, Hc, Wc, p, scale, bias, groups,
+                                                                       y);
     DANET_LAUNCH_CHECK();
     return 0;
 }

@@ -293,24 +293,26 @@ int danet_conv_dgrad_weights(int32_t wsets, int32_t cout, int32_t cin, int32_t k
                              danet_stream_t stream);
 /* interleave / crop / sum: y NCHW [N,C,H,W] (fp32) with y[n][c][h][w] = sum in piece order over the pieces of class
  * (h % stride, w % stride) of maps[i] at [n][h / stride + tr][w / stride + tc][c] (0 outside), times scale[1] when
- * scale (device) is not NULL.  maps is a HOST array of npieces device pointers, each NHWC fp32 [N,Hc,Wc,Cp].  With
- * stride 1 and the piece {0} it is the NHWC -> NCHW conversion. */
+ * scale (device) is not NULL, plus bias[(n % groups) * C + c] when bias (device, [groups][C]) is not NULL.  maps is a
+ * HOST array of npieces device pointers, each NHWC fp32 [N,Hc,Wc,Cp].  With stride 1 and the piece {0} it is the
+ * NHWC -> NCHW conversion (the forward's epilogue: the x scale removed, then the bias added). */
 int danet_conv_dgrad_scatter(int32_t N, int32_t C, int32_t H, int32_t W, int32_t Cp, int32_t stride, int32_t Hc, int32_t Wc,
                              int32_t npieces, const danet_dgrad_piece* pieces, const float* const* maps,
-                             const float* scale, float* y, danet_stream_t stream);
-/* dy NCHW [N,C,HW] fp32 -> split-fp16 NHWC planes [N,HW,Cp] (Cp % 8 == 0, pad channels 0) of dy * 2^s, where the power
- * of two 2^s brings max |dy| into [2^13, 2^14) (1 when dy is 0): gradients far below 1 keep their 22 bits.
+                             const float* scale, const float* bias, int32_t groups, float* y, danet_stream_t stream);
+/* v NCHW [N,C,HW] fp32 (dy, or the forward's x) -> split-fp16 NHWC planes [N,HW,Cp] (Cp % 8 == 0, pad channels 0) of
+ * v * 2^s, where the power of two 2^s brings max finite |v| into [2^13, 2^14) (1 when there is none; s is clamped to
+ * [-126, 126]): values far from 1 keep their 22 bits.  NaN and +-inf stay non-finite in the planes.
  * scale: device float[3]; receives scale[0] = 2^s, scale[1] = 2^-s (scale[2] is scratch).  No host synchronisation. */
 int danet_conv_grad_split(int32_t N, int32_t C, int32_t HW, int32_t Cp, const float* dy, void* hi, void* lo, float* scale,
                           danet_stream_t stream);
 /* Weight gradient of the forward problem d (flags ignored; N % wsets == 0): x [N,H,W,Cin] and dy [N,Ho,Wo,Cout] as hi +
- * lo split-fp16 planes; dy_scale = the scale danet_conv_grad_split wrote for dy (or NULL: unscaled).  dW
+ * lo split-fp16 planes; dy_scale / x_scale = the scales danet_conv_grad_split wrote for dy / x (or NULL: unscaled).  dW
  * [wsets*cout][cin][k][k] from a wgmma implicit GEMM over the pixels in split-fp16 exact arithmetic; split K over pixel
- * chunks, partials in the workspace (16-byte aligned), chunks added in a fixed order in double, dy_scale removed
- * exactly. */
+ * chunks, partials in the workspace (16-byte aligned), chunks added in a fixed order in double, both scales removed
+ * exactly (one after the other, in double). */
 int64_t danet_conv_wgrad_workspace_bytes(const danet_conv_desc* d);
 int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout, int32_t cin, const danet_act* x, const danet_act* dy,
-                     const float* dy_scale, float* dW, void* workspace, danet_stream_t stream);
+                     const float* dy_scale, const float* x_scale, float* dW, void* workspace, danet_stream_t stream);
 /* Bias gradient: db[c] = sum over n and the HW pixels of the fp32 NCHW dy [N,C,HW]; image chunks summed in double with
  * a fixed order, then added in chunk order.  Workspace 8-byte aligned. */
 int64_t danet_conv_bias_grad_workspace_bytes(int32_t N, int32_t C, int32_t HW);

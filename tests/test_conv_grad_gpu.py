@@ -1,42 +1,14 @@
-"""GPU tests of the differentiable convolution (danet_b200.conv.conv2d): y, dx, dW and db against torch fp64 autograd on
-the same inputs for every distinct convolution of body_net, limb_net and limb_reslayer plus two HRNet shapes, gradients
-scaled far from 1, then repeatability, CUDA-graph replay, batch independence of dx, needs_input_grad subsets, the
-input-gradient pieces against the restatement and argument errors."""
+"""GPU tests of the differentiable convolution (danet_b200.conv.conv2d) beyond its numbers: repeatability, CUDA-graph
+replay, batch independence of dx, needs_input_grad subsets, the input-gradient pieces against the restatement and
+argument errors.  y, dx, dW and db against fp64 autograd, element by element, are the sweep's
+(tests/test_conv_grad_sweep_gpu.py)."""
 import pytest
 import torch
-import torch.nn.functional as F
+
+from conv_grad_sweep_common import NET_SHAPES as SHAPES
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
-
-# (name, cin, cout, H, k, stride, groups): per-group channels
-SHAPES = [
-    ("body_in_1x1_75-64", 75, 64, 56, 1, 1, 1),
-    ("limb_in_1x1_21-64", 21, 64, 56, 1, 1, 1),
-    ("stem_7x7s2_64-64", 64, 64, 56, 7, 2, 1),
-    ("layer1_3x3_64-64", 64, 64, 14, 3, 1, 1),
-    ("layer2_3x3s2_64-128", 64, 128, 14, 3, 2, 1),
-    ("layer2_down_1x1s2_64-128", 64, 128, 14, 1, 2, 1),
-    ("layer2_3x3_128-128", 128, 128, 7, 3, 1, 1),
-    ("layer3_3x3s2_128-256_7to4", 128, 256, 7, 3, 2, 1),
-    ("layer3_down_1x1s2_128-256_7to4", 128, 256, 7, 1, 2, 1),
-    ("layer3_3x3_256-256", 256, 256, 4, 3, 1, 1),
-    ("layer4_3x3s2_256-512_4to2", 256, 512, 4, 3, 2, 1),
-    ("layer4_down_1x1s2_256-512", 256, 512, 4, 1, 2, 1),
-    ("layer4_3x3_512-512", 512, 512, 2, 3, 1, 1),
-    ("limb_reslayer_3x3s2_g24", 256, 128, 4, 3, 2, 24),
-    ("limb_reslayer_3x3_g24", 128, 128, 2, 3, 1, 24),
-    ("limb_reslayer_down_1x1s2_g24", 256, 128, 4, 1, 2, 24),
-    ("hrnet_3x3_96-96", 96, 96, 28, 3, 1, 1),
-    ("hrnet_3x3s2_48-96", 48, 96, 56, 3, 2, 1),
-]
-# relative Frobenius-norm bounds: y and dx, dW and db
-TOL_Y, TOL_W = 1e-5, 2e-5
-
-
-def rel(a, b):
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / b.norm().clamp_min(1e-300))
 
 
 def make(shape, B, bias, seed=0):
@@ -58,53 +30,6 @@ def run(x, w, b, gy, s, G, need=(True, True, True)):
     y = conv2d(x, w, b, s, w.shape[-1] // 2, 1, G)
     y.backward(gy)
     return y.detach(), x.grad, w.grad, (b.grad if b is not None else None)
-
-
-def reference(x, w, b, gy, s, G):
-    x, w = x.double().requires_grad_(), w.double().requires_grad_()
-    b = b.double().requires_grad_() if b is not None else None
-    y = F.conv2d(x, w, b, stride=s, padding=w.shape[-1] // 2, groups=G)
-    y.backward(gy.double())
-    return y.detach(), x.grad, w.grad, (b.grad if b is not None else None)
-
-
-@pytest.mark.parametrize("bias", [False, True], ids=["nobias", "bias"])
-@pytest.mark.parametrize("B", [2, 16])
-@pytest.mark.parametrize("shape", SHAPES, ids=[s[0] for s in SHAPES])
-def test_against_fp64_autograd(shape, B, bias):
-    s, G = shape[5], shape[6]
-    x, w, b, gy = make(shape, B, bias)
-    got = run(x, w, b, gy, s, G)
-    ref = reference(x, w, b, gy, s, G)
-    errs = check(got, ref)
-    print("%s B=%d bias=%d %s" % (shape[0], B, bias, " ".join("%s %.2e" % kv for kv in errs.items())))
-
-
-def check(got, ref):
-    errs = {}
-    for name, gt, rf, tol in zip(("y", "dx", "dW", "db"), got, ref, (TOL_Y, TOL_Y, TOL_W, TOL_W)):
-        if rf is None:
-            assert gt is None
-            continue
-        assert gt.shape == rf.shape and gt.dtype == torch.float32, name
-        errs[name] = rel(gt, rf)
-        assert errs[name] <= tol, (name, errs)
-    return errs
-
-
-SCALED = [SHAPES[2], SHAPES[7], SHAPES[13], SHAPES[17]]
-
-
-@pytest.mark.parametrize("gscale", [1e-8, 1e-4, 1e3])
-@pytest.mark.parametrize("shape", SCALED, ids=[s[0] for s in SCALED])
-def test_gradient_scale(shape, gscale):
-    """Gradients far from 1 (mean-reduced losses over many pixels give ~1e-8) meet the same bounds: dy is scaled by a
-    power of two before its fp16 split."""
-    s, G = shape[5], shape[6]
-    x, w, b, gy = make(shape, 4, True)
-    gy = gy * gscale
-    errs = check(run(x, w, b, gy, s, G), reference(x, w, b, gy, s, G))
-    print("%s gy*%g %s" % (shape[0], gscale, " ".join("%s %.2e" % kv for kv in errs.items())))
 
 
 def test_pieces_match_the_restatement():
