@@ -120,6 +120,11 @@ SIGNATURES = {
     "danet_maxpool3x3s2_nchw_backward": (c_int, [c_int] * 4 + [c_p] * 4),
     "danet_global_avgpool_backward": (c_int, [c_int, c_int, c_p, c_p, c_p]),
     "danet_linear_backward": (c_int, [c_int] * 3 + [c_p] * 7),
+    "danet_hr_fuse_forward": (c_int, [c_int] * 5 + [c_p, c_p, c_int, c_p, c_p]),
+    "danet_hr_fuse_backward": (c_int, [c_int] * 5 + [c_p] * 4),
+    "danet_part_crops_forward": (c_int, [c_int] * 3 + [c_p, c_p, c_int, c_p, c_p]),
+    "danet_part_crops_backward": (c_int, [c_int] * 3 + [c_p, c_p, c_int, c_p, c_p]),
+    "danet_part_thetas": (c_int, [c_int] * 3 + [c_p] * 4 + [c_f, c_p, c_f, c_p, c_f, c_int, c_p, c_p, c_p]),
     "danet_act_split": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_act_merge": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_nchw_to_nhwc": (c_int, [c_int, c_int, c_int, c_int, c_p, ctypes.POINTER(Act), c_p]),

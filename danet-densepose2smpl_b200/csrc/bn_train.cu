@@ -21,6 +21,10 @@
 // and NaN wins over numbers (torch's rule, so the slots equal its indices).  The backward is a gather: an input pixel
 // adds, in row-major window order, the dy of the windows (at most four) whose slot points at it.
 //
+// HRNet fuse: the forward adds the nearest-upsampled terms in list order, so it is bit-identical to the reference's
+// F.interpolate + add + relu chain.  The backward of a term upsampled by f is a gather: one thread per term element
+// sums dy * [y > 0] over its f x f block in row-major order (fp32: within (f^2 - 1) 2^-24 sum |dy| of the exact sum).
+//
 // Branch tails (their forwards are danet_global_avgpool and danet_linear of glue.cu): the average pool's backward
 // spreads dy / HW over the plane; the linear layer's backward sums dx = dy W, dW = dy^T x and db = sum dy in double, in
 // index order.
@@ -279,6 +283,116 @@ k_linear_bwd(int N, int In, int Out, long long ndx, long long ndw, long long ndb
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// HRNet fuse (hr_module.py:161-179): y = relu(up(t_0) + up(t_1) + ...), nearest upsampling by 1, 2, 4 or 8
+// ------------------------------------------------------------------------------------------------
+struct FuseArgs { const float* t[4]; int sh[4]; int n; };     // sh = log2 of the upsample factor
+
+__device__ __forceinline__ float relu_fwd(float v) { return (v > 0.f || v != v) ? v : 0.f; }     // torch: NaN stays
+
+// Forward: a thread writes V consecutive outputs of one row (V = 4: 16-byte stores, and 16-/8-byte loads of the
+// terms at factor 1 / 2).  The terms are added in list order, each sum rounded on its own, as the reference's
+// y = y + term chain.
+template <int V>
+__global__ void __launch_bounds__(kThreads)
+k_hr_fuse_fwd(long long items, int H, int W, const FuseArgs a, int relu, float* __restrict__ y) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= items) return;
+    const int WV = W / V;
+    const long long row = i / WV;                    // (n * C + c) * H + h
+    const int w = (int)(i - row * WV) * V;
+    const long long nc = row / H;
+    const int h = (int)(row - nc * H);
+    float acc[V];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        if (j >= a.n) break;
+        const int sh = a.sh[j], Wj = W >> sh;
+        const float* src = a.t[j] + (size_t)(nc * (H >> sh) + (h >> sh)) * Wj;
+        float v[V];
+        if (V == 4 && sh == 0) {
+            const float4 t = __ldg(reinterpret_cast<const float4*>(src + w));
+            v[0] = t.x; v[1 % V] = t.y; v[2 % V] = t.z; v[3 % V] = t.w;
+        } else if (V == 4 && sh == 1) {
+            const float2 t = __ldg(reinterpret_cast<const float2*>(src + (w >> 1)));
+            v[0] = t.x; v[1 % V] = t.x; v[2 % V] = t.y; v[3 % V] = t.y;
+        } else {
+#pragma unroll
+            for (int k = 0; k < V; ++k) v[k] = __ldg(src + ((w + k) >> sh));
+        }
+#pragma unroll
+        for (int k = 0; k < V; ++k) acc[k] = j == 0 ? v[k] : __fadd_rn(acc[k], v[k]);
+    }
+    if (relu) {
+#pragma unroll
+        for (int k = 0; k < V; ++k) acc[k] = relu_fwd(acc[k]);
+    }
+    float* o = y + (size_t)row * W + w;
+    if (V == 4) *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1 % V], acc[2 % V], acc[3 % V]);
+    else o[0] = acc[0];
+}
+
+// dy masked by the ReLU: torch's rule on the output, no gradient where y <= 0 (an exact 0 sum included)
+__device__ __forceinline__ float relu_bwd(float g, const float* y, size_t e) { return (y && !(__ldg(y + e) > 0.f)) ? 0.f : g; }
+
+// Backward of one term upsampled by F: a thread owns one element of dterm and sums dy * [y > 0] over its F x F block in
+// row-major order (fp32).  VEC: the block's rows are read as 8- (F = 2) or 16-byte (F = 4, 8) vectors.
+template <int F, bool VEC>
+__global__ void __launch_bounds__(kThreads)
+k_hr_fuse_bwd(long long items, int Hj, int Wj, const float* __restrict__ dy, const float* __restrict__ y, float* __restrict__ dt) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= items) return;
+    const long long row = i / Wj;                    // (n * C + c) * Hj + hj
+    const int wj = (int)(i - row * Wj);
+    const long long nc = row / Hj;
+    const int hj = (int)(row - nc * Hj), W = Wj * F;
+    float acc = 0.f;
+#pragma unroll
+    for (int r = 0; r < F; ++r) {
+        const size_t e = (size_t)((nc * Hj + hj) * F + r) * W + (size_t)wj * F;
+        if (VEC && F == 2) {
+            const float2 g = __ldg(reinterpret_cast<const float2*>(dy + e));
+            float2 m = make_float2(1.f, 1.f);
+            if (y) { const float2 t = __ldg(reinterpret_cast<const float2*>(y + e)); m = make_float2(t.x > 0.f, t.y > 0.f); }
+            acc += m.x != 0.f ? g.x : 0.f;
+            acc += m.y != 0.f ? g.y : 0.f;
+        } else if (VEC && F >= 4) {
+#pragma unroll
+            for (int q = 0; q < F; q += 4) {
+                const float4 g = __ldg(reinterpret_cast<const float4*>(dy + e + q));
+                float4 t = make_float4(1.f, 1.f, 1.f, 1.f);
+                if (y) t = __ldg(reinterpret_cast<const float4*>(y + e + q));
+                acc += t.x > 0.f ? g.x : 0.f;
+                acc += t.y > 0.f ? g.y : 0.f;
+                acc += t.z > 0.f ? g.z : 0.f;
+                acc += t.w > 0.f ? g.w : 0.f;
+            }
+        } else {
+#pragma unroll
+            for (int q = 0; q < F; ++q) acc += relu_bwd(__ldg(dy + e + q), y, e + q);
+        }
+    }
+    dt[i] = acc;
+}
+
+// Backward of a term at factor 1: dterm = dy * [y > 0], 16-byte vectors when aligned
+__global__ void __launch_bounds__(kThreads)
+k_hr_fuse_bwd1(long long total, int vec, const float* __restrict__ dy, const float* __restrict__ y, float* __restrict__ dt) {
+    const long long e = 4 * ((long long)blockIdx.x * kThreads + threadIdx.x);
+    if (e >= total) return;
+    if (vec && e + 3 < total) {
+        const float4 g = __ldg(reinterpret_cast<const float4*>(dy + e));
+        float4 o = g;
+        if (y) {
+            const float4 t = __ldg(reinterpret_cast<const float4*>(y + e));
+            o = make_float4(t.x > 0.f ? g.x : 0.f, t.y > 0.f ? g.y : 0.f, t.z > 0.f ? g.z : 0.f, t.w > 0.f ? g.w : 0.f);
+        }
+        *reinterpret_cast<float4*>(dt + e) = o;
+        return;
+    }
+    for (long long k = e; k < e + 4 && k < total; ++k) dt[k] = relu_bwd(__ldg(dy + k), y, (size_t)k);
+}
+
 static unsigned grid_of(long long work) { return (unsigned)((work + kThreads - 1) / kThreads); }
 static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
@@ -378,6 +492,62 @@ extern "C" int danet_maxpool3x3s2_nchw_backward(int32_t N, int32_t C, int32_t H,
     const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
     const long long total = (long long)N * C * H * W;
     bn::k_maxpool3x3s2_bwd<<<bn::grid_of(total), bn::kThreads, 0, (cudaStream_t)stream>>>(total, H, W, Ho, Wo, dy, slot, dx);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+static bool fuse_factor_ok(int32_t f, int32_t H, int32_t W) {
+    return (f == 1 || f == 2 || f == 4 || f == 8) && H % f == 0 && W % f == 0;
+}
+
+static int fuse_shift(int32_t f) { return f == 8 ? 3 : f == 4 ? 2 : f == 2 ? 1 : 0; }
+
+extern "C" int danet_hr_fuse_forward(int32_t N, int32_t C, int32_t H, int32_t W, int32_t nterms, const float* const* terms,
+                                     const int32_t* factors, int32_t relu, float* y, danet_stream_t stream) {
+    DANET_CHECK(pool_shape_ok(N, C, H, W), "danet_hr_fuse_forward: bad sizes N=%d C=%d H=%d W=%d", N, C, H, W);
+    DANET_CHECK(nterms >= 1 && nterms <= 4, "danet_hr_fuse_forward: %d terms (1 to 4 are supported)", nterms);
+    DANET_CHECK(terms && factors && y, "danet_hr_fuse_forward: terms, factors and y must be non-null");
+    bn::FuseArgs a;
+    a.n = nterms;
+    bool vec = (W % 4) == 0 && bn::aligned16(y);
+    for (int j = 0; j < 4; ++j) {
+        a.t[j] = nullptr; a.sh[j] = 0;
+        if (j >= nterms) continue;
+        DANET_CHECK(terms[j], "danet_hr_fuse_forward: term %d is null", j);
+        DANET_CHECK(fuse_factor_ok(factors[j], H, W), "danet_hr_fuse_forward: factor %d of term %d must be 1, 2, 4 or 8 and "
+                    "divide H=%d and W=%d", factors[j], j, H, W);
+        a.t[j] = terms[j]; a.sh[j] = fuse_shift(factors[j]);
+        vec = vec && (a.sh[j] == 0 ? bn::aligned16(terms[j]) : a.sh[j] == 1 ? ((uintptr_t)terms[j] & 7) == 0 : true);
+    }
+    const long long total = (long long)N * C * H * W;
+    if (vec) bn::k_hr_fuse_fwd<4><<<bn::grid_of(total / 4), bn::kThreads, 0, (cudaStream_t)stream>>>(total / 4, H, W, a, relu, y);
+    else bn::k_hr_fuse_fwd<1><<<bn::grid_of(total), bn::kThreads, 0, (cudaStream_t)stream>>>(total, H, W, a, relu, y);
+    DANET_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int danet_hr_fuse_backward(int32_t N, int32_t C, int32_t H, int32_t W, int32_t factor, const float* dy,
+                                      const float* y, float* dterm, danet_stream_t stream) {
+    DANET_CHECK(pool_shape_ok(N, C, H, W), "danet_hr_fuse_backward: bad sizes N=%d C=%d H=%d W=%d", N, C, H, W);
+    DANET_CHECK(fuse_factor_ok(factor, H, W), "danet_hr_fuse_backward: factor %d must be 1, 2, 4 or 8 and divide H=%d and "
+                "W=%d", factor, H, W);
+    DANET_CHECK(dy && dterm, "danet_hr_fuse_backward: dy and dterm must be non-null");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int Hj = H / factor, Wj = W / factor;
+    const long long items = (long long)N * C * Hj * Wj;
+    const bool vec = bn::aligned16(dy) && (!y || bn::aligned16(y));
+    switch (factor) {
+        case 1: bn::k_hr_fuse_bwd1<<<bn::grid_of((items + 3) / 4), bn::kThreads, 0, st>>>(items, vec && bn::aligned16(dterm), dy, y, dterm); break;
+        case 2: if (vec) bn::k_hr_fuse_bwd<2, true><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
+                else bn::k_hr_fuse_bwd<2, false><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
+                break;
+        case 4: if (vec) bn::k_hr_fuse_bwd<4, true><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
+                else bn::k_hr_fuse_bwd<4, false><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
+                break;
+        default: if (vec) bn::k_hr_fuse_bwd<8, true><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
+                 else bn::k_hr_fuse_bwd<8, false><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
+                 break;
+    }
     DANET_LAUNCH_CHECK();
     return 0;
 }

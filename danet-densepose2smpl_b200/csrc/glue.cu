@@ -1,35 +1,11 @@
 // Memory-bound fp32 glue kernels of the DaNet network half (NHWC activations).
 // Each replaces a chain of small ATen launches in the reference; citations per kernel.
 #include "common.cuh"
+#include "stn_common.cuh"
 #include <cuda_fp16.h>
 #include <math.h>
 
 namespace danet {
-
-// utils/smpl_utlis.py:13-17,29-53 (structure tables used by iuv_estimator.py:176-184,262-301)
-__constant__ int c_parents0[24] = {0, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21};
-__constant__ int c_children1[24] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 10, 11, 15, 16, 17, 15, 18, 19, 20, 21, 22, 23, 22, 23};
-// smpl2dp_part as 25-bit masks over DensePose part ids
-__constant__ unsigned c_part_mask[24] = {
-    (1u << 1) | (1u << 2), (1u << 8) | (1u << 10), (1u << 7) | (1u << 9), (1u << 1) | (1u << 2),
-    (1u << 8) | (1u << 10) | (1u << 12) | (1u << 14), (1u << 7) | (1u << 9) | (1u << 11) | (1u << 13),
-    (1u << 1) | (1u << 2), (1u << 12) | (1u << 14) | (1u << 5), (1u << 11) | (1u << 13) | (1u << 6),
-    (1u << 1) | (1u << 2), (1u << 12) | (1u << 14) | (1u << 5), (1u << 11) | (1u << 13) | (1u << 6),
-    (1u << 1) | (1u << 2) | (1u << 23) | (1u << 24), (1u << 15) | (1u << 17), (1u << 16) | (1u << 18),
-    (1u << 23) | (1u << 24), (1u << 15) | (1u << 17), (1u << 16) | (1u << 18),
-    (1u << 15) | (1u << 17) | (1u << 19) | (1u << 21), (1u << 16) | (1u << 18) | (1u << 20) | (1u << 22),
-    (1u << 19) | (1u << 21) | (1u << 4), (1u << 20) | (1u << 22) | (1u << 3),
-    (1u << 19) | (1u << 21) | (1u << 4), (1u << 20) | (1u << 22) | (1u << 3)};
-
-// torch.argmax semantics: first maximal value; NaN counts as maximal
-__device__ __forceinline__ int argmax_first(const float* v, int n) {
-    int best = 0; float bv = v[0];
-    for (int c = 1; c < n; ++c) {
-        const float x = v[c];
-        if ((x > bv) || (x != x && bv == bv)) { bv = x; best = c; }
-    }
-    return best;
-}
 
 // ------------------------------------------------------------------------------------------
 // NCHW image -> NHWC padded (input boundary of the network; demo.py:106 / eval.py:147 tensors)

@@ -9,6 +9,7 @@
 // fixed order -- bit-for-bit repeatable, no float atomics.  The per-point / per-pixel arithmetic is __host__ __device__
 // so that the DANET_LOSSES_HOST_CHECK build walks it on the CPU against the reference-generated golden.
 #include "common.cuh"
+#include "stn_common.cuh"
 
 namespace danet {
 
@@ -26,12 +27,6 @@ namespace danet {
 
 __host__ __device__ inline float sl1(float d) { const float a = fabsf(d); return a < 1.f ? 0.5f * d * d : a - 0.5f; }
 __host__ __device__ inline float sl1_grad(float d) { return fminf(fmaxf(d, -1.f), 1.f); }
-
-// grid coordinate in [-1, 1] -> source pixel coordinate (torch grid_sampler_compute_source_index, no padding clip)
-__host__ __device__ inline float unnormalize(float g, int S, int align_corners) {
-    return align_corners ? RN_MUL(RN_MUL(RN_ADD(g, 1.f), 0.5f), (float)(S - 1))
-                         : RN_MUL(RN_ADD(RN_MUL(RN_ADD(g, 1.f), (float)S), -1.f), 0.5f);
-}
 
 // bilinear footprint of one sample point: north-west corner and the four weights (nw, ne, sw, se).  Points whose
 // corners are all outside the map (or NaN coordinates) get x0 = y0 = -2: nothing is read or written for them.
@@ -85,7 +80,7 @@ __host__ __device__ inline Foot dp_foot(const DpArgs& a, int n, int p) {
     const size_t o = (size_t)n * a.P + p;
     const float hs = 0.5f * (float)a.S, sc = 2.f / (float)a.S;
     const float gx = RN_MUL(RN_ADD(a.X[o], -hs), sc), gy = RN_MUL(RN_ADD(a.Y[o], -hs), sc);
-    return make_foot(unnormalize(gx, a.S, a.align), unnormalize(gy, a.S, a.align), a.S);
+    return make_foot(grid_unnormalize(gx, a.S, a.align), grid_unnormalize(gy, a.S, a.align), a.S);
 }
 // the point's class label: int64 of the float label (truncation toward zero); -1 if outside [0, 25)
 __host__ __device__ inline int dp_label(float l, int C) { return (l > -1.f && l < (float)C) ? (int)l : -1; }
@@ -407,15 +402,6 @@ __constant__ signed char c_dp2smpl[24][6] = DANET_DP2SMPL_MAPPING;
 static const signed char h_dp2smpl[24][6] = DANET_DP2SMPL_MAPPING;
 #endif
 
-// base grid coordinate i of affine_grid, rounded like torch's: linspace(-1, 1, S) (start + i*step on the first half,
-// end - (S-1-i)*step on the second), times (S-1)/S when align_corners is off (AffineGridGenerator.cpp)
-__host__ __device__ inline float affine_base(int i, int S, int align) {
-    const float step = 2.f / (float)(S - 1);
-    float v = i < S / 2 ? RN_ADD(-1.f, RN_MUL(step, (float)i)) : RN_ADD(1.f, -RN_MUL(step, (float)(S - 1 - i)));
-    if (!align) v = RN_MUL(v, (float)(S - 1)) / (float)S;
-    return v;
-}
-
 // the 21 channels (U, V, I x [background, 6 mapped]) of part `i`'s crop at output pixel (px, py) of image b:
 // affine_grid + grid_sample (bilinear, zeros) of part_iuv_simp's maps.  The I background (sum of the 6 mapped I
 // channels < 0.5, repeats counted twice) is evaluated at the source pixels and then interpolated, like the reference.
@@ -425,7 +411,7 @@ __host__ __device__ inline void part_target_pixel(const float* U, const float* V
     const float xb = affine_base(px, S, align), yb = affine_base(py, S, align);
     const float gx = RN_ADD(RN_ADD(RN_MUL(th[0], xb), RN_MUL(th[1], yb)), th[2]);
     const float gy = RN_ADD(RN_ADD(RN_MUL(th[3], xb), RN_MUL(th[4], yb)), th[5]);
-    const Foot f = make_foot(unnormalize(gx, S, align), unnormalize(gy, S, align), S);
+    const Foot f = make_foot(grid_unnormalize(gx, S, align), grid_unnormalize(gy, S, align), S);
     const size_t HW = (size_t)S * S;
     float acc[3][7];
 #pragma unroll

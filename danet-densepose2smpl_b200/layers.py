@@ -7,6 +7,7 @@
     y = max_pool2d(x, 3, 2, 1)                     # F.max_pool2d(x, kernel_size=3, stride=2, padding=1)
     y = adaptive_avg_pool2d(x, 1)                  # F.adaptive_avg_pool2d(x, 1)
     y = linear(x, weight, bias, add=None)          # F.linear(x, weight, bias) + add (add: a constant [Out] term)
+    y = hr_fuse([t0, t1, ...], [f0, f1, ...])      # relu(up(t0, f0) + up(t1, f1) + ...), nearest upsampling
 
 `batch_norm` has the meaning and argument order of torch.nn.functional.batch_norm.  Training mode normalises with the
 biased batch variance over (N, H, W) and updates running_mean / running_var in place with `momentum` and the unbiased
@@ -310,3 +311,74 @@ def linear(input, weight, bias=None, *, add=None):
             tensors.append((name, t))
     _check_cuda(fn, tensors, input.device)
     return _Linear.apply(input, weight, bias, add.detach() if add is not None else None)
+
+
+class _HrFuse(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, relu, factors, *terms):
+        lib = _lib.load()
+        t0, f0 = terms[0], factors[0]
+        dev = t0.device
+        N, C, H, W = t0.shape[0], t0.shape[1], t0.shape[2] * f0, t0.shape[3] * f0
+        n = len(terms)
+        with torch.cuda.device(dev):
+            y = torch.empty(N, C, H, W, dtype=torch.float32, device=dev)
+            ptrs = (ctypes.c_void_p * 4)(*[t.data_ptr() for t in terms])
+            facs = (ctypes.c_int32 * 4)(*factors)
+            _lib.check(lib.danet_hr_fuse_forward(N, C, H, W, n, ptrs, facs, int(relu), _lib.ptr(y), _lib.stream_ptr(dev)),
+                       "hr_fuse_forward")
+        ctx.save_for_backward(y if relu else None)
+        ctx.factors, ctx.shape = factors, (N, C, H, W)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        (y,) = ctx.saved_tensors
+        N, C, H, W = ctx.shape
+        lib = _lib.load()
+        dev = gy.device
+        grads = []
+        with torch.cuda.device(dev):
+            gy = gy.to(torch.float32).contiguous()
+            for f, need in zip(ctx.factors, ctx.needs_input_grad[2:]):
+                if not need:
+                    grads.append(None)
+                    continue
+                dt = torch.empty(N, C, H // f, W // f, dtype=torch.float32, device=dev)
+                _lib.check(lib.danet_hr_fuse_backward(N, C, H, W, f, _lib.ptr(gy), _lib.ptr(y), _lib.ptr(dt),
+                                                      _lib.stream_ptr(dev)), "hr_fuse_backward")
+                grads.append(dt)
+        return (None, None) + tuple(grads)
+
+
+def hr_fuse(terms, factors, relu=True):
+    """One HRNet fuse output (hr_module.py:161-179) on the GPU, differentiable w.r.t. every term:
+    relu(up(terms[0], factors[0]) + up(terms[1], factors[1]) + ...), up = nearest upsampling by 1, 2, 4 or 8.
+
+    terms: 1 to 4 fp32 contiguous NCHW CUDA tensors [N, C, H / f, W / f] with t.H * f == H and t.W * f == W for one
+    (H, W).  The terms are added in list order, the reference's `y = y + ...` order, so the forward is bit-identical
+    to the fp32 sequence F.interpolate(t, scale_factor=f, mode='nearest') + ... + relu.  The backward of a term is
+    the sum of dy * [y > 0] over each f x f block in row-major order (torch's ReLU rule: an exact 0 gets no gradient),
+    in fp32: within (f^2 - 1) 2^-24 sum |dy| of the exact block sum."""
+    fn = "hr_fuse"
+    if not isinstance(terms, (list, tuple)) or not 1 <= len(terms) <= 4:
+        raise ValueError("danet_b200.layers.hr_fuse: terms must be a list of 1 to 4 tensors")
+    if not isinstance(factors, (list, tuple)) or len(factors) != len(terms):
+        raise ValueError("danet_b200.layers.hr_fuse: factors must be a list with one factor per term")
+    for f in factors:
+        if isinstance(f, bool) or not isinstance(f, int) or f not in (1, 2, 4, 8):
+            raise ValueError("danet_b200.layers.hr_fuse: factors must be 1, 2, 4 or 8 (got %r)" % (f,))
+    for j, t in enumerate(terms):
+        _check_tensor(fn, "terms[%d]" % j, t)
+        if t.dim() != 4 or min(t.shape) < 1:
+            raise ValueError("danet_b200.layers.hr_fuse: terms[%d] must be a non-empty 4-D NCHW tensor (got %s)"
+                             % (j, tuple(t.shape)))
+    N, C = terms[0].shape[:2]
+    H, W = terms[0].shape[2] * factors[0], terms[0].shape[3] * factors[0]
+    for j, (t, f) in enumerate(zip(terms, factors)):
+        if tuple(t.shape) != (N, C, H // f, W // f) or H % f or W % f:
+            raise ValueError("danet_b200.layers.hr_fuse: terms[%d] %s upsampled by %d is not [%d, %d, %d, %d]"
+                             % (j, tuple(t.shape), f, N, C, H, W))
+    _check_cuda(fn, [("terms[%d]" % j, t) for j, t in enumerate(terms)], terms[0].device)
+    return _HrFuse.apply(bool(relu), tuple(int(f) for f in factors), *terms)

@@ -362,6 +362,34 @@ int danet_global_avgpool_backward(int32_t NC, int32_t HW, const float* dy, float
 int danet_linear_backward(int32_t N, int32_t In, int32_t Out, const float* x, const float* w, const float* dy, float* dx,
                           float* dw, float* db, danet_stream_t stream);
 
+/* HRNet fuse (models/module/hr_module.py:161-179, the training form of danet_fuse_sum): fp32 NCHW
+ * y [N,C,H,W] = relu?(up(t_0) + up(t_1) + ...), term j [N,C,H/f_j,W/f_j] upsampled nearest by f_j in {1,2,4,8},
+ * added in list order (bit-identical to the F.interpolate + add + relu chain).  terms / factors: host arrays of
+ * nterms (1..4) entries.  The backward writes one term's gradient: dterm = the f x f block sums of dy * [y > 0]
+ * (y NULL: no ReLU), row-major. */
+int danet_hr_fuse_forward(int32_t N, int32_t C, int32_t H, int32_t W, int32_t nterms, const float* const* terms,
+                          const int32_t* factors, int32_t relu, float* y, danet_stream_t stream);
+int danet_hr_fuse_backward(int32_t N, int32_t C, int32_t H, int32_t W, int32_t factor, const float* dy, const float* y,
+                           float* dterm, danet_stream_t stream);
+
+/* STN part crops in training (models/danet/iuv_estimator.py:193-204): 24x F.affine_grid(theta_i, xd.size()) +
+ * F.grid_sample(xd, grid) (bilinear, zeros), cat on dim 1.  xd [B,C,S,S], theta [B,24,2,3] with zero off-diagonal
+ * entries (not read), crops [B,24*C,S,S], all fp32 NCHW.  The backward is the exact adjoint of the forward w.r.t. xd,
+ * a gather summed in double. */
+int danet_part_crops_forward(int32_t B, int32_t C, int32_t S, const float* xd, const float* theta, int32_t align_corners,
+                             float* crops, danet_stream_t stream);
+int danet_part_crops_backward(int32_t B, int32_t C, int32_t S, const float* dcrops, const float* theta,
+                              int32_t align_corners, float* dxd, danet_stream_t stream);
+/* Training-mode thetas (iuv_estimator.py:137-140,172-191,262-301): soft-argmax centres of 10 * hm [B,24,Sh,Sh], the
+ * centre jitter center_jitter * (center_noise [B,24,2] - 0.5), part visibility (bilinear sample of
+ * 1[argmax index_pred [B,25,Si,Si] in the part's set] < vis_score; off when vis_score <= 0) and affine_para with the
+ * scale jitters scale_jitter * (scale_noise [24,2,B] - 0.5).  NULL noise: no jitter.  centers [B,24,2] (jittered),
+ * theta [B,24,2,3] = [[s, 0, cx], [0, s, cy]]. */
+int danet_part_thetas(int32_t B, int32_t Sh, int32_t Si, const float* hm, const float* index_pred,
+                      const float* learned_ratio, const float* learned_offset, float vis_score, const float* center_noise,
+                      float center_jitter, const float* scale_noise, float scale_jitter, int32_t align_corners,
+                      float* centers, float* theta, danet_stream_t stream);
+
 /* input boundary: x NCHW [N,C,HW] -> y NHWC [N,HW,Cp] with Cp >= C zero-padded channels
  * (images arrive NCHW: demo.py:106, eval.py:147) */
 int danet_nchw_to_nhwc(int32_t N, int32_t C, int32_t HW, int32_t Cp, const float* x, const danet_act* y,
