@@ -637,23 +637,28 @@ __global__ void k_smpl_joints(int B, SmplView m, const float* __restrict__ posed
 // backward of the SMPL layer (the piece of the training step, train/trainer.py:148-215 + smpl_regressor.py:131-221,
 // that has a hard oracle): given dL/dverts and dL/d(smpl joints), dL/dbetas and dL/dR (R = the 24 rotation matrices
 // the layer consumed, pose2rot=False).  fp32 SIMT; everything is recomputed from (betas, R), nothing is kept from
-// the forward pass.
+// the forward pass.  No float atomics: every sum has a fixed order, so the result is bit-for-bit repeatable and a
+// body's gradient does not depend on the rest of the batch.
 //   k_smpl_pose          (forward kernel) -> G (world transforms), A (skinning transforms), pose feature
-//   k_lbs_bwd_verts      grid (vertex tile, body): recompute v_posed, dv_posed = T_v^T g, dA += w (g x [v_posed;1])
+//   k_lbs_bwd_verts      grid (vertex tile, body): recompute v_posed, dv_posed = T_v^T g, and the tile's partial
+//                        dA = sum_v w (g x [v_posed;1]), each of the 24 x 12 entries summed in vertex order
+//   k_lbs_bwd_dA         dA = the tile partials summed in tile order
 //   k_lbs_bwd_blend      dpf = P dv_posed (207 rows), dbeta_shape = S dv_posed: one warp per (body, row)
 //   k_lbs_bwd_chain      one thread per body: reverse kinematic chain -> dR, dJ -> dbeta
 // ---------------------------------------------------------------------------------------------
+constexpr int kTileS = kTileV + 1;      // row stride of the staged [joint][vertex] and [entry][vertex] planes (no bank conflicts)
 __global__ void __launch_bounds__(kTileV)
 k_lbs_bwd_verts(int B, const float* __restrict__ betas, const float* __restrict__ pf, const float* __restrict__ A,
-                SmplView m, const float* __restrict__ gverts, float* __restrict__ dvp, float* __restrict__ dA) {
+                SmplView m, const float* __restrict__ gverts, float* __restrict__ dvp, float* __restrict__ dA_tiles) {
     __shared__ float s_pf[kPF];
     __shared__ float s_A[kJ * 12];
-    __shared__ float s_dA[kJ * 12];
     __shared__ float s_v[kTileC];
     __shared__ float s_beta[kMaxBetas];
+    __shared__ float s_w[kJ * kTileS];      // skinning weight of (joint, vertex), 0 past nv
+    __shared__ float s_gv[12 * kTileS];     // g[r] * [v_posed; 1][c] of (entry r * 4 + c, vertex)
     const int tile = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     for (int i = tid; i < kPF; i += kTileV) s_pf[i] = pf[(size_t)b * kPF + i];
-    for (int i = tid; i < kJ * 12; i += kTileV) { s_A[i] = A[(size_t)b * kJ * 12 + i]; s_dA[i] = 0.f; }
+    for (int i = tid; i < kJ * 12; i += kTileV) s_A[i] = A[(size_t)b * kJ * 12 + i];
     if (tid < kMaxBetas) s_beta[tid] = tid < m.nbetas ? betas[(size_t)b * m.nbetas + tid] : 0.f;
     __syncthreads();
     // v_posed of the tile (coordinate-parallel, like the forward pass)
@@ -687,12 +692,14 @@ k_lbs_bwd_verts(int B, const float* __restrict__ betas, const float* __restrict_
         } else {
             w = __ldg(m.skin_dense + (size_t)j * m.nvpad + v);
         }
-        if (w == 0.f || v >= m.nv) continue;
-        for (int r = 0; r < 3; ++r) {
+        if (v >= m.nv) w = 0.f;
+        s_w[j * kTileS + tid] = w;
+        if (w == 0.f) continue;
+        for (int r = 0; r < 3; ++r)
             for (int c = 0; c < 3; ++c) T[r * 3 + c] = fmaf(w, s_A[j * 12 + r * 4 + c], T[r * 3 + c]);
-            for (int c = 0; c < 4; ++c) atomicAdd(&s_dA[j * 12 + r * 4 + c], w * g[r] * vh[c]);
-        }
     }
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 4; ++c) s_gv[(r * 4 + c) * kTileS + tid] = g[r] * vh[c];
     // dv_posed = T^T g
     if (v < m.nv)
         for (int c = 0; c < 3; ++c)
@@ -700,7 +707,26 @@ k_lbs_bwd_verts(int B, const float* __restrict__ betas, const float* __restrict_
     else if (3 * v + 2 < m.npad)
         for (int c = 0; c < 3; ++c) dvp[(size_t)b * m.npad + 3 * v + c] = 0.f;
     __syncthreads();
-    for (int i = tid; i < kJ * 12; i += kTileV) if (s_dA[i] != 0.f) atomicAdd(&dA[(size_t)b * kJ * 12 + i], s_dA[i]);
+    // the tile's partial dA: thread = (joint, entry) output, summed over the tile's vertices in order
+    float* out = dA_tiles + ((size_t)b * m.ntiles + tile) * (kJ * 12);
+    for (int o = tid; o < kJ * 12; o += kTileV) {
+        const float* wj = s_w + (o / 12) * kTileS;
+        const float* ge = s_gv + (o % 12) * kTileS;
+        float s = 0.f;
+        for (int u = 0; u < kTileV; ++u) s = fmaf(wj[u], ge[u], s);
+        out[o] = s;
+    }
+}
+
+// dA[b] = sum over the vertex tiles, in tile order, of the partials of k_lbs_bwd_verts
+__global__ void k_lbs_bwd_dA(int B, int ntiles, const float* __restrict__ dA_tiles, float* __restrict__ dA) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * kJ * 12) return;
+    const int b = i / (kJ * 12), o = i - b * (kJ * 12);
+    const float* p = dA_tiles + (size_t)b * ntiles * (kJ * 12) + o;
+    float s = 0.f;
+    for (int t = 0; t < ntiles; ++t) s += p[(size_t)t * (kJ * 12)];
+    dA[i] = s;
 }
 
 // rows 0..206: dL/dpose_feature; rows 207..207+nbetas-1: dL/dbeta through the shape blend shapes
@@ -1055,6 +1081,7 @@ extern "C" int64_t danet_smpl_backward_workspace_bytes(danet_smpl_t h, int32_t B
     ws_off(cur, (int64_t)B * h->v.npad * 4);        // dL/dv_posed
     ws_off(cur, (int64_t)B * kJ * 12 * 4);          // dL/dA
     ws_off(cur, (int64_t)B * kPF * 4);              // dL/dpose_feature
+    ws_off(cur, (int64_t)B * h->v.ntiles * kJ * 12 * 4);   // per-tile partials of dL/dA
     return cur;
 }
 
@@ -1075,10 +1102,12 @@ extern "C" int danet_smpl_backward(danet_smpl_t h, int32_t B, const float* betas
     float* dvp = (float*)(ws + ws_off(cur, (int64_t)B * m.npad * 4));
     float* dA = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 12 * 4));
     float* dpf = (float*)(ws + ws_off(cur, (int64_t)B * kPF * 4));
-    DANET_CUDA(cudaMemsetAsync(dA, 0, (size_t)B * kJ * 12 * 4, stream));
+    float* dA_tiles = (float*)(ws + ws_off(cur, (int64_t)B * m.ntiles * kJ * 12 * 4));
     k_smpl_pose<<<cdiv(B, kPoseWarps), kPoseWarps * 32, 0, stream>>>(B, DANET_POSE_ROTMAT, betas, rotmats, m, nullptr, G, A, pf, posed, nullptr, nullptr);
     DANET_LAUNCH_CHECK();
-    k_lbs_bwd_verts<<<dim3(m.ntiles, B), kTileV, 0, stream>>>(B, betas, pf, A, m, grad_verts, dvp, dA);
+    k_lbs_bwd_verts<<<dim3(m.ntiles, B), kTileV, 0, stream>>>(B, betas, pf, A, m, grad_verts, dvp, dA_tiles);
+    DANET_LAUNCH_CHECK();
+    k_lbs_bwd_dA<<<cdiv(B * kJ * 12, 256), 256, 0, stream>>>(B, m.ntiles, dA_tiles, dA);
     DANET_LAUNCH_CHECK();
     const int nrow = 207 + m.nbetas;
     k_lbs_bwd_blend<<<cdiv((int64_t)B * nrow * 32, 256), 256, 0, stream>>>(B, m, dvp, dpf, grad_betas);

@@ -75,7 +75,8 @@ int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas, const floa
  * models/danet/smpl_regressor.py:131-221).  rotmats [B,24,3,3] are the matrices the forward consumed (pose2rot=False,
  * treated as free 3x3 inputs); grad_verts [B,V,3]; grad_smpl_joints [B,24,3] or NULL (gradients w.r.t. the regressed
  * joints are folded into grad_verts by the caller: J_regressor^T g); outputs grad_betas [B,num_betas],
- * grad_rotmats [B,24,3,3].  Recomputes the forward intermediates; fp32. */
+ * grad_rotmats [B,24,3,3].  Recomputes the forward intermediates; fp32, with no float atomics: every sum runs in a
+ * fixed order, so the result is bit-for-bit repeatable and a body's gradient does not depend on the rest of the batch. */
 int64_t danet_smpl_backward_workspace_bytes(danet_smpl_t h, int32_t B);
 int danet_smpl_backward(danet_smpl_t h, int32_t B, const float* betas, const float* rotmats,
                         const float* grad_verts, const float* grad_smpl_joints, float* grad_betas,
