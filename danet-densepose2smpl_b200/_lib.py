@@ -189,10 +189,22 @@ def stream_ptr(device=None):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def call(name, *args, device=None):
+    """danet_<name>(*args, stream): the stream is the current torch stream of `device` (default: the current device),
+    and a failure raises RuntimeError labelled `name`."""
+    check(getattr(load(), "danet_" + name)(*args, stream_ptr(device)), name)
+
+
+def workspace(nbytes, device):
+    """uint8 scratch of `nbytes` on `device`: at least 16 bytes, so its pointer is never NULL."""
+    import torch
+    return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
+
+
 def ptr(t):
-    """Device pointer of a torch tensor (None -> NULL)."""
-    if t is None:
-        return ctypes.c_void_p(0)
+    """Device pointer of a torch tensor or an integer address (None and 0 -> NULL)."""
+    if t is None or isinstance(t, int):
+        return ctypes.c_void_p(t or 0)
     return ctypes.c_void_p(t.data_ptr())
 
 

@@ -30,20 +30,10 @@ import ctypes
 import torch
 from torch.autograd.function import once_differentiable
 
-from . import _lib
+from . import _args, _lib
 
 EXACT = 4                         # DANET_CONV_EXACT
 _MAX_PROBLEMS = 6                 # problems per danet_conv_tc_group launch
-
-
-def _pair(v, name):
-    if isinstance(v, (tuple, list)):
-        if len(v) != 2 or v[0] != v[1]:
-            raise ValueError("danet_b200.conv.conv2d: %s must be one int or an equal pair (got %r)" % (name, v))
-        v = v[0]
-    if isinstance(v, bool) or not isinstance(v, int):
-        raise ValueError("danet_b200.conv.conv2d: %s must be an int (got %r)" % (name, v))
-    return v
 
 
 def _ceil8(c):
@@ -61,22 +51,21 @@ def _planes(shape, dev):
     return (torch.empty(shape, dtype=torch.float16, device=dev), torch.empty(shape, dtype=torch.float16, device=dev))
 
 
-def _split_scaled(lib, t, N, C, HW, Cp, shape, dev):
+def _split_scaled(t, N, C, HW, Cp, shape, dev):
     """fp32 NCHW [N, C, HW] -> split-fp16 NHWC planes [shape] of t * 2^s with Cp >= C channels (pad channels zero), and
     the scale [2^s, 2^-s, -, -] (danet_conv_grad_split)"""
     hi, lo = _planes(shape, dev)
     scale = torch.empty(4, dtype=torch.float32, device=dev)
-    _lib.check(lib.danet_conv_grad_split(N, C, HW, Cp, _lib.ptr(t), _lib.ptr(hi), _lib.ptr(lo), _lib.ptr(scale),
-                                         _lib.stream_ptr(dev)), "conv_grad_split")
+    _lib.call("conv_grad_split", N, C, HW, Cp, _lib.ptr(t), _lib.ptr(hi), _lib.ptr(lo), _lib.ptr(scale), device=dev)
     return (hi, lo), scale
 
 
-def _pack(lib, d, w_simt, dev):
-    nbytes = int(lib.danet_conv_tc_packed_bytes(ctypes.byref(d)))
+def _pack(d, w_simt, dev):
+    nbytes = int(_lib.load().danet_conv_tc_packed_bytes(ctypes.byref(d)))
     if nbytes <= 0:
         raise ValueError("danet_b200.conv.conv2d: shape not supported by the tensor-core path")
     pk = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    _lib.check(lib.danet_conv_tc_pack(ctypes.byref(d), _lib.ptr(w_simt), _lib.ptr(pk), _lib.stream_ptr(dev)), "conv_tc_pack")
+    _lib.call("conv_tc_pack", ctypes.byref(d), _lib.ptr(w_simt), _lib.ptr(pk), device=dev)
     return pk
 
 
@@ -94,32 +83,31 @@ def _problem(d, x_planes, pk, bias, y):
 _PIECES = {}
 
 
-def _pieces(lib, k, stride):
+def _pieces(k, stride):
     """the input-gradient pieces of a (k, stride) convolution (danet_conv_dgrad_pieces), cached"""
     key = (k, stride)
     if key not in _PIECES:
         arr = (_lib.DgradPiece * 9)()
-        n = int(lib.danet_conv_dgrad_pieces(k, stride, arr))
+        n = int(_lib.load().danet_conv_dgrad_pieces(k, stride, arr))
         if n < 0:
             raise ValueError("danet_b200.conv.conv2d: no input gradient for k=%d stride=%d" % (k, stride))
         _PIECES[key] = ((_lib.DgradPiece * max(n, 1))(*arr[:n]), n)
     return _PIECES[key]
 
 
-def _scatter(lib, pieces, n, maps, N, C, H, W, Cp, stride, Hc, Wc, scale, dev, bias=None, G=1):
+def _scatter(pieces, n, maps, N, C, H, W, Cp, stride, Hc, Wc, scale, dev, bias=None, G=1):
     """NHWC piece maps -> fp32 NCHW [N, C, H, W] (summed per class, shifted, cropped, scale removed, then the bias
     [G * C] of image n's group n % G added)"""
     y = torch.empty(N, C, H, W, dtype=torch.float32, device=dev)
     arr = (ctypes.c_void_p * max(n, 1))(*[m.data_ptr() for m in maps])
-    _lib.check(lib.danet_conv_dgrad_scatter(N, C, H, W, Cp, stride, Hc, Wc, n, pieces, arr, _lib.ptr(scale), _lib.ptr(bias), G,
-                                            _lib.ptr(y), _lib.stream_ptr(dev)), "conv_dgrad_scatter")
+    _lib.call("conv_dgrad_scatter", N, C, H, W, Cp, stride, Hc, Wc, n, pieces, arr, _lib.ptr(scale), _lib.ptr(bias), G,
+              _lib.ptr(y), device=dev)
     return y
 
 
 class _Conv2d(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, stride, groups):
-        lib = _lib.load()
         dev = x.device
         B, Ct, H, W = x.shape
         Cot, cin, k, _ = weight.shape
@@ -129,18 +117,16 @@ class _Conv2d(torch.autograd.Function):
         Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
         d = _desc(N, H, W, Cinp, Coutp, k, stride, G)
         with torch.cuda.device(dev):
-            sp = _lib.stream_ptr(dev)
-            xp, x_scale = _split_scaled(lib, x, N, cin, H * W, Cinp, (N, H, W, Cinp), dev)
+            xp, x_scale = _split_scaled(x, N, cin, H * W, Cinp, (N, H, W, Cinp), dev)
             w_simt = torch.empty(G * k * k * Cinp * Coutp, dtype=torch.float32, device=dev)
-            _lib.check(lib.danet_conv_weights_simt(G, cout, cin, k, Coutp, Cinp, _lib.ptr(weight), _lib.ptr(w_simt), sp),
-                       "conv_weights_simt")
-            pk = _pack(lib, d, w_simt, dev)
+            _lib.call("conv_weights_simt", G, cout, cin, k, Coutp, Cinp, _lib.ptr(weight), _lib.ptr(w_simt), device=dev)
+            pk = _pack(d, w_simt, dev)
             # the engine's sum is of x * 2^s: the bias joins after the scatter has removed 2^s
             y_nhwc = torch.empty(N, Ho, Wo, Coutp, dtype=torch.float32, device=dev)
             arr = (_lib.ConvProblem * 1)(_problem(d, xp, pk, None, y_nhwc))
-            _lib.check(lib.danet_conv_tc_group(1, arr, sp), "conv_tc_group")
+            _lib.call("conv_tc_group", 1, arr, device=dev)
             one = (_lib.DgradPiece * 1)(_lib.DgradPiece(0, 0, k, 0, 0, 0, 0, 0, 0))
-            y = _scatter(lib, one, 1, [y_nhwc], N, cout, Ho, Wo, Coutp, 1, Ho, Wo, x_scale, dev, bias, G)
+            y = _scatter(one, 1, [y_nhwc], N, cout, Ho, Wo, Coutp, 1, Ho, Wo, x_scale, dev, bias, G)
         need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         ctx.save_for_backward(weight if need_dx else None, xp[0] if need_dw else None, xp[1] if need_dw else None,
                               x_scale if need_dw else None)
@@ -154,25 +140,23 @@ class _Conv2d(torch.autograd.Function):
         B, Ct, H, W, Cot, cin, cout, k, stride, G, Ho, Wo = ctx.geom
         need_dx, need_dw, need_db = ctx.needs_input_grad[:3]
         N, Cinp, Coutp = B * G, _ceil8(cin), _ceil8(cout)
-        lib = _lib.load()
         dev = gy.device
         dx = dw = db = None
         with torch.cuda.device(dev):
-            sp = _lib.stream_ptr(dev)
             gy = gy.to(torch.float32).contiguous()
             if need_dx or need_dw:
                 # dy * 2^s as split planes, 2^s from max |dy| on the device: small gradients keep their 22 bits
-                dyp, scale = _split_scaled(lib, gy, N, cout, Ho * Wo, Coutp, (N, Ho, Wo, Coutp), dev)
+                dyp, scale = _split_scaled(gy, N, cout, Ho * Wo, Coutp, (N, Ho, Wo, Coutp), dev)
             if need_dx:
-                pieces, n = _pieces(lib, k, stride)
+                pieces, n = _pieces(k, stride)
                 probs, outs, keep = [], [], []
                 for i in range(n):
                     pc = pieces[i]
                     dd = _desc(N, Ho, Wo, Coutp, Cinp, pc.K, 1, G)
                     wc = torch.empty(G * pc.K * pc.K * Coutp * Cinp, dtype=torch.float32, device=dev)
-                    _lib.check(lib.danet_conv_dgrad_weights(G, cout, cin, k, stride, ctypes.byref(pc), Coutp, Cinp,
-                                                            _lib.ptr(weight), _lib.ptr(wc), sp), "conv_dgrad_weights")
-                    pk = _pack(lib, dd, wc, dev)
+                    _lib.call("conv_dgrad_weights", G, cout, cin, k, stride, ctypes.byref(pc), Coutp, Cinp, _lib.ptr(weight),
+                              _lib.ptr(wc), device=dev)
+                    pk = _pack(dd, wc, dev)
                     o = torch.empty(N, Ho, Wo, Cinp, dtype=torch.float32, device=dev)
                     probs.append(_problem(dd, dyp, pk, None, o))
                     outs.append(o)
@@ -180,43 +164,39 @@ class _Conv2d(torch.autograd.Function):
                 for i in range(0, n, _MAX_PROBLEMS):          # the engine runs up to 6 problems per launch
                     grp = probs[i:i + _MAX_PROBLEMS]
                     arr = (_lib.ConvProblem * len(grp))(*grp)
-                    _lib.check(lib.danet_conv_tc_group(len(grp), arr, sp), "conv_tc_group (dgrad)")
-                dx = _scatter(lib, pieces, n, outs, N, cin, H, W, Cinp, stride, Ho, Wo, scale, dev).view(B, Ct, H, W)
+                    _lib.call("conv_tc_group", len(grp), arr, device=dev)
+                dx = _scatter(pieces, n, outs, N, cin, H, W, Cinp, stride, Ho, Wo, scale, dev).view(B, Ct, H, W)
             if need_dw:
                 d = _desc(N, H, W, Cinp, Coutp, k, stride, G)
-                ws = torch.empty(int(lib.danet_conv_wgrad_workspace_bytes(ctypes.byref(d))), dtype=torch.uint8, device=dev)
+                ws = _lib.workspace(_lib.load().danet_conv_wgrad_workspace_bytes(ctypes.byref(d)), dev)
                 dw = torch.empty(Cot, cin, k, k, dtype=torch.float32, device=dev)
                 xa = _lib.Act(None, x_hi.data_ptr(), x_lo.data_ptr())
                 da = _lib.Act(None, dyp[0].data_ptr(), dyp[1].data_ptr())
-                _lib.check(lib.danet_conv_wgrad(ctypes.byref(d), cout, cin, ctypes.byref(xa), ctypes.byref(da), _lib.ptr(scale),
-                                                _lib.ptr(x_scale), _lib.ptr(dw), _lib.ptr(ws), sp), "conv_wgrad")
+                _lib.call("conv_wgrad", ctypes.byref(d), cout, cin, ctypes.byref(xa), ctypes.byref(da), _lib.ptr(scale),
+                          _lib.ptr(x_scale), _lib.ptr(dw), _lib.ptr(ws), device=dev)
             if need_db:
                 # from the fp32 dy itself
-                ws = torch.empty(int(lib.danet_conv_bias_grad_workspace_bytes(B, Cot, Ho * Wo)), dtype=torch.uint8, device=dev)
+                ws = _lib.workspace(_lib.load().danet_conv_bias_grad_workspace_bytes(B, Cot, Ho * Wo), dev)
                 db = torch.empty(Cot, dtype=torch.float32, device=dev)
-                _lib.check(lib.danet_conv_bias_grad(B, Cot, Ho * Wo, _lib.ptr(gy), _lib.ptr(db), _lib.ptr(ws), sp),
-                           "conv_bias_grad")
+                _lib.call("conv_bias_grad", B, Cot, Ho * Wo, _lib.ptr(gy), _lib.ptr(db), _lib.ptr(ws), device=dev)
         return dx, dw, db, None, None
 
 
 def conv2d(x, weight, bias=None, stride=1, padding=0, dilation=1, groups=1):
     """torch.nn.functional.conv2d on the tensor-core engine (exact mode), differentiable.  See the module docstring."""
-    stride, padding, dilation = _pair(stride, "stride"), _pair(padding, "padding"), _pair(dilation, "dilation")
+    where = "danet_b200.conv.conv2d"
+    stride = _args.int_pair(where, "stride", stride)
+    padding = _args.int_pair(where, "padding", padding)
+    dilation = _args.int_pair(where, "dilation", dilation)
     if isinstance(groups, bool) or not isinstance(groups, int) or groups < 1:
-        raise ValueError("danet_b200.conv.conv2d: groups must be a positive int (got %r)" % (groups,))
-    for name, t in (("x", x), ("weight", weight), ("bias", bias)):
-        if t is None:
-            continue
-        if not isinstance(t, torch.Tensor):
-            raise ValueError("danet_b200.conv.conv2d: %s must be a tensor" % name)
-        if not t.is_cuda:
-            raise ValueError("danet_b200.conv.conv2d: %s must be a CUDA tensor (there is no CPU path)" % name)
-        if t.dtype != torch.float32:
-            raise ValueError("danet_b200.conv.conv2d: %s must be float32 (got %s)" % (name, t.dtype))
+        raise ValueError("%s: groups must be a positive int (got %r)" % (where, groups))
+    tensors = [(name, t) for name, t in (("x", x), ("weight", weight), ("bias", bias)) if t is not None]
+    for name, t in tensors:                     # each tensor in turn: type, CUDA, dtype
+        _args.cuda(where, [(name, t)])
+        _args.tensor(where, name, t, contiguous=False)
     if x.dim() != 4 or weight.dim() != 4:
         raise ValueError("danet_b200.conv.conv2d: x and weight must be 4-D (NCHW, OIHW)")
-    if weight.device != x.device or (bias is not None and bias.device != x.device):
-        raise ValueError("danet_b200.conv.conv2d: x, weight and bias must be on one device")
+    _args.cuda(where, tensors)                  # one device
     Cot, cin, kh, kw = weight.shape
     if kh != kw or kh not in (1, 3, 7):
         raise ValueError("danet_b200.conv.conv2d: kernel size must be 1, 3 or 7 and square (got %dx%d)" % (kh, kw))

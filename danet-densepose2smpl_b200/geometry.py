@@ -17,7 +17,7 @@ def rot6d_to_rotmat(x):
     n = xc.shape[0]
     out = torch.empty(n, 3, 3, device=xc.device)
     with torch.cuda.device(xc.device):
-        _lib.check(_lib.load().danet_rot6d_to_rotmat(n, _lib.ptr(xc), _lib.ptr(out), _lib.stream_ptr()), "rot6d")
+        _lib.call("rot6d_to_rotmat", n, _lib.ptr(xc), _lib.ptr(out))
     return out
 
 
@@ -29,8 +29,7 @@ def batch_rodrigues(theta, flavor="quat"):
     n = tc.shape[0]
     out = torch.empty(n, 3, 3, device=tc.device)
     with torch.cuda.device(tc.device):
-        _lib.check(_lib.load().danet_batch_rodrigues(n, _lib.ptr(tc), _lib.ptr(out),
-                                                     1 if flavor == "smplx" else 0, _lib.stream_ptr()), "rodrigues")
+        _lib.call("batch_rodrigues", n, _lib.ptr(tc), _lib.ptr(out), 1 if flavor == "smplx" else 0)
     return out
 
 
@@ -48,6 +47,6 @@ def perspective_projection(points, rotation, translation, focal_length, camera_c
     c = camera_center.detach().to(dev).float().contiguous()
     out = torch.empty(B, N, 2, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(_lib.load().danet_perspective_projection(B, N, _lib.ptr(p), _lib.ptr(r), _lib.ptr(t), _lib.ptr(f),
-                                                            _lib.ptr(c), _lib.ptr(out), _lib.stream_ptr()), "persp")
+        _lib.call("perspective_projection", B, N, _lib.ptr(p), _lib.ptr(r), _lib.ptr(t), _lib.ptr(f), _lib.ptr(c),
+                  _lib.ptr(out))
     return out

@@ -16,10 +16,8 @@ def iuvmap_clean(U_uv, V_uv, Index_UV, AnnIndex=None):
     oU, oV, oI = torch.empty_like(U), torch.empty_like(V), torch.empty_like(I)
     oA = torch.empty_like(A) if A is not None else None
     with torch.cuda.device(dev):
-        _lib.check(_lib.load().danet_iuvmap_clean_nchw(B, C, A.shape[1] if A is not None else 0, H * W,
-                                                       _lib.ptr(U), _lib.ptr(V), _lib.ptr(I), _lib.ptr(A),
-                                                       _lib.ptr(oU), _lib.ptr(oV), _lib.ptr(oI), _lib.ptr(oA),
-                                                       _lib.stream_ptr()), "iuvmap_clean")
+        _lib.call("iuvmap_clean_nchw", B, C, A.shape[1] if A is not None else 0, H * W,
+                  *map(_lib.ptr, (U, V, I, A, oU, oV, oI, oA)))
     return oU, oV, oI, oA
 
 
@@ -33,8 +31,7 @@ def iuv_img2map(uvimages, uv_rois=None, new_size=None):
     assert S == S2
     outs = [torch.empty(B, c, S, S, device=x.device) for c in (25, 25, 25, 15)]
     with torch.cuda.device(x.device):
-        _lib.check(_lib.load().danet_iuv_img2map(B, S, _lib.ptr(x), *[_lib.ptr(o) for o in outs],
-                                                 _lib.stream_ptr()), "iuv_img2map")
+        _lib.call("iuv_img2map", B, S, _lib.ptr(x), *map(_lib.ptr, outs))
     return tuple(outs)
 
 

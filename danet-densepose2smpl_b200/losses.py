@@ -29,20 +29,22 @@ POINT_REGRESSION_WEIGHTS = 0.5                  # configs/danet_default.yaml:23 
 def _launch(N, C, Cann, HW, pred_stride, map_stride, u, v, idx, ann, U, V, I, A, has, batch_size, point_weight, dev,
             gu, gv, gi, ga):
     """Pointers are integer device addresses (or None); returns losses [4] on `dev`."""
-    lib = _lib.load()
-    p = lambda x: _lib.c_p(x if x else 0)
     with torch.cuda.device(dev):
-        ws = torch.empty(int(lib.danet_body_uv_losses_workspace_bytes(N, HW)), dtype=torch.uint8, device=dev)
+        ws = _lib.workspace(_lib.load().danet_body_uv_losses_workspace_bytes(N, HW), dev)
         losses = torch.empty(4, device=dev)
-        _lib.check(lib.danet_body_uv_losses(N, C, Cann, HW, pred_stride, map_stride, p(u), p(v), p(idx), p(ann), p(U), p(V),
-                                            p(I), p(A), p(has), float(batch_size), float(point_weight), _lib.ptr(losses),
-                                            p(gu), p(gv), p(gi), p(ga), _lib.ptr(ws), _lib.stream_ptr(dev)),
-                   "body_uv_losses")
+        _lib.call("body_uv_losses", N, C, Cann, HW, pred_stride, map_stride, *map(_lib.ptr, (u, v, idx, ann, U, V, I, A, has)),
+                  float(batch_size), float(point_weight), _lib.ptr(losses), *map(_lib.ptr, (gu, gv, gi, ga)), _lib.ptr(ws),
+                  device=dev)
     return losses
 
 
 def _f32(t, dev):
     return t.detach().to(device=dev, dtype=torch.float32).contiguous()
+
+
+def _d(t):
+    """integer device address of t (None -> 0): what the launch functions take"""
+    return t.data_ptr() if t is not None else 0
 
 
 def _has_u8(has_iuv, dev, repeat=1):
@@ -72,9 +74,8 @@ class _BodyUvLosses(torch.autograd.Function):
         gv = torch.empty_like(v_) if need[1] else None
         gi = torch.empty_like(i_) if need[2] else None
         ga = torch.empty_like(a_) if (ann is not None and need[3]) else None
-        d = lambda t: t.data_ptr() if t is not None else 0
-        losses = _launch(B, C, a_.shape[1] if a_ is not None else 0, HW, 0, 0, d(u_), d(v_), d(i_), d(a_), d(U_), d(V_),
-                         d(I_), d(A_), d(has), float(B), point_weight, dev, d(gu), d(gv), d(gi), d(ga))
+        losses = _launch(B, C, a_.shape[1] if a_ is not None else 0, HW, 0, 0, _d(u_), _d(v_), _d(i_), _d(a_), _d(U_),
+                         _d(V_), _d(I_), _d(A_), _d(has), float(B), point_weight, dev, _d(gu), _d(gv), _d(gi), _d(ga))
         ctx.grads = (gu, gv, gi, ga)
         ctx.dtypes = (u.dtype, v.dtype, idx.dtype, ann.dtype if ann is not None else None)
         return losses
@@ -122,10 +123,10 @@ class _PartIuvLosses(torch.autograd.Function):
         p_, g_ = _f32(pred, dev), _f32(gt, dev)
         grad = torch.empty_like(p_) if ctx.needs_input_grad[0] else None
         step = C * HW * 4                                         # bytes between the u, v and index groups of a row
-        pb, gb, qb = p_.data_ptr(), g_.data_ptr(), (grad.data_ptr() if grad is not None else 0)
+        pb, gb, qb = p_.data_ptr(), g_.data_ptr(), _d(grad)
         q = lambda k: qb + k * step if qb else 0
         losses = _launch(B * P, C, 0, HW, three * C * HW, three * C * HW, pb, pb + step, pb + 2 * step, 0,
-                         gb, gb + step, gb + 2 * step, 0, has.data_ptr() if has is not None else 0, float(B * P),
+                         gb, gb + step, gb + 2 * step, 0, _d(has), float(B * P),
                          point_weight, dev, q(0), q(1), q(2), 0)
         ctx.grad = grad
         ctx.dtype = pred.dtype
@@ -165,42 +166,29 @@ STN_HM_WEIGHTS = 0.0                            # configs/danet_default.yaml:36 
 NUM_UV_CHANNELS = 25                            # cfg.DANET.NUM_PATCHES + 1
 
 
-def _ws(nbytes, dev):
-    return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=dev)
-
-
-_d = lambda t: t.data_ptr() if t is not None else 0
-_P = lambda x: _lib.c_p(x if x else 0)
-
-
 def _dp_launch(N, S, Cann, P, preds, pts, has, align, pw, part_w, index_w, dev, grads):
     """preds / pts / grads: integer device addresses (0 = NULL); returns losses [4] on `dev`."""
-    lib = _lib.load()
     with torch.cuda.device(dev):
-        ws = _ws(lib.danet_dp_uvia_losses_workspace_bytes(N, S * S), dev)
+        ws = _lib.workspace(_lib.load().danet_dp_uvia_losses_workspace_bytes(N, S * S), dev)
         losses = torch.empty(4, device=dev)
-        _lib.check(lib.danet_dp_uvia_losses(N, S, Cann, P, *map(_P, preds), *map(_P, pts), _P(has), align, float(pw),
-                                            float(part_w), float(index_w), _lib.ptr(losses), *map(_P, grads),
-                                            _lib.ptr(ws), _lib.stream_ptr(dev)), "dp_uvia_losses")
+        _lib.call("dp_uvia_losses", N, S, Cann, P, *map(_lib.ptr, preds), *map(_lib.ptr, pts), _lib.ptr(has), align,
+                  float(pw), float(part_w), float(index_w), _lib.ptr(losses), *map(_lib.ptr, grads), _lib.ptr(ws),
+                  device=dev)
     return losses
 
 
 def _stn_launch(B, J, S, hm, kps, cols, kps_weight, hm_weight, dev, groi, ghm):
-    lib = _lib.load()
     with torch.cuda.device(dev):
-        ws = _ws(lib.danet_stn_kps_losses_workspace_bytes(B, J), dev)
+        ws = _lib.workspace(_lib.load().danet_stn_kps_losses_workspace_bytes(B, J), dev)
         losses = torch.empty(2, device=dev)
-        _lib.check(lib.danet_stn_kps_losses(B, J, S, _P(hm), _P(kps), cols, float(kps_weight), float(hm_weight),
-                                            _lib.ptr(losses), _P(groi), _P(ghm), _lib.ptr(ws), _lib.stream_ptr(dev)),
-                   "stn_kps_losses")
+        _lib.call("stn_kps_losses", B, J, S, _lib.ptr(hm), _lib.ptr(kps), cols, float(kps_weight), float(hm_weight),
+                  _lib.ptr(losses), _lib.ptr(groi), _lib.ptr(ghm), _lib.ptr(ws), device=dev)
     return losses
 
 
 def _part_launch(B, S, C, U, V, I, theta, align, out, dev):
-    lib = _lib.load()
     with torch.cuda.device(dev):
-        _lib.check(lib.danet_part_iuv_targets(B, S, C, _P(U), _P(V), _P(I), _P(theta), align, _P(out),
-                                              _lib.stream_ptr(dev)), "part_iuv_targets")
+        _lib.call("part_iuv_targets", B, S, C, *map(_lib.ptr, (U, V, I, theta)), align, _lib.ptr(out), device=dev)
 
 
 def _check_labels(lab, C, sel, what):

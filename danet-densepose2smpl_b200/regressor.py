@@ -45,7 +45,7 @@ import weakref
 import torch
 from torch.autograd.function import once_differentiable
 
-from . import _lib
+from . import _args, _lib
 
 LAYERS = [("r2p_gcn", 0), ("refine_gcn", 0), ("refine_gcn", 1), ("refine_gcn", 2), ("p2r_gcn", 0)]
 DIMS = [(128, 128), (128, 256), (256, 256), (256, 128), (128, 128)]
@@ -101,17 +101,15 @@ class _GcnHead(torch.autograd.Function):
     @staticmethod
     def forward(ctx, training, bufs, new_stats, rot_feats, global_para, *params):
         dev, B = rot_feats.device, rot_feats.shape[0]
-        lib = _lib.load()
         with torch.cuda.device(dev):
-            ws = torch.empty(int(lib.danet_gcn_head_train_workspace_bytes(B)), dtype=torch.uint8, device=dev)
+            ws = _lib.workspace(_lib.load().danet_gcn_head_train_workspace_bytes(B), dev)
             para = _empty(B, 229, dev=dev)
             pose0, c0, c1 = (_empty(B, 216, dev=dev), _empty(B, 24, 3, dev=dev), _empty(B, 24, 3, dev=dev)) if training \
                 else (None, None, None)
             p = _pack(params, bufs)
-            _lib.check(lib.danet_gcn_head_train_forward(B, ctypes.byref(p), int(training), _lib.ptr(rot_feats),
-                                                        _lib.ptr(global_para), _lib.ptr(para), _lib.ptr(pose0),
-                                                        _lib.ptr(c0), _lib.ptr(c1), _lib.ptr(new_stats), _lib.ptr(ws),
-                                                        _lib.stream_ptr(dev)), "gcn_head_train_forward")
+            _lib.call("gcn_head_train_forward", B, ctypes.byref(p), int(training), _lib.ptr(rot_feats), _lib.ptr(global_para),
+                      _lib.ptr(para), _lib.ptr(pose0), _lib.ptr(c0), _lib.ptr(c1), _lib.ptr(new_stats), _lib.ptr(ws),
+                      device=dev)
         ctx.save_for_backward(rot_feats, *params)
         ctx.bufs, ctx.ws, ctx.training = bufs, ws, training
         return (para, pose0, c0, c1) if training else para
@@ -127,14 +125,12 @@ class _GcnHead(torch.autograd.Function):
         g_pose0, g_c0, g_c1 = (f32(t) for t in g[1:4]) if training else (None, None, None)
         grads = [None if (not training and name in TRAINING_ONLY) else torch.empty_like(t)
                  for name, t in zip(PARAM_NAMES, params)]
-        lib = _lib.load()
         with torch.cuda.device(dev):
             g_rot, g_gp = torch.empty_like(rot_feats), _empty(B, 13, dev=dev)
             p = _pack(params, ctx.bufs, grads)
-            _lib.check(lib.danet_gcn_head_train_backward(B, ctypes.byref(p), int(training), _lib.ptr(rot_feats),
-                                                         _lib.ptr(g_para), _lib.ptr(g_pose0), _lib.ptr(g_c0),
-                                                         _lib.ptr(g_c1), _lib.ptr(g_rot), _lib.ptr(g_gp),
-                                                         _lib.ptr(ctx.ws), _lib.stream_ptr(dev)), "gcn_head_train_backward")
+            _lib.call("gcn_head_train_backward", B, ctypes.byref(p), int(training), _lib.ptr(rot_feats), _lib.ptr(g_para),
+                      _lib.ptr(g_pose0), _lib.ptr(g_c0), _lib.ptr(g_c1), _lib.ptr(g_rot), _lib.ptr(g_gp), _lib.ptr(ctx.ws),
+                      device=dev)
         return (None, None, None, g_rot, g_gp, *grads)
 
 
@@ -148,6 +144,7 @@ def gcn_head(model, rot_feats, global_para):
     """smpl_regressor.py:844-895 (+ the concatenation of :924) in model.training's BatchNorm mode.  rot_feats [B,24,128],
     global_para [B,13] on the model's CUDA device.  Returns {'para': [B,229], 'joint_rotation': [pose0] or [],
     'joint_position': [coord0, coord1] or []}; differentiable w.r.t. the inputs and the head's 29 parameters."""
+    where = "danet_b200.regressor.gcn_head"
     mod = head_module(model)
     params = [_attr(mod, n) for n in PARAM_NAMES]
     dev = params[0].device
@@ -156,21 +153,20 @@ def gcn_head(model, rot_feats, global_para):
     if dev.type != "cuda":
         raise RuntimeError("danet_b200: move the model to a CUDA device (there is no CPU path)")
     if rot_feats.dim() != 3 or tuple(rot_feats.shape[1:]) != (24, 128) or rot_feats.shape[0] < 1:
-        raise ValueError("gcn_head: rot_feats must be [B,24,128] with B >= 1, got %s" % (tuple(rot_feats.shape),))
+        raise ValueError("%s: rot_feats must be [B,24,128] with B >= 1, got %s" % (where, tuple(rot_feats.shape)))
     B = rot_feats.shape[0]
     if tuple(global_para.shape) != (B, 13):
-        raise ValueError("gcn_head: global_para must be [B,13] = [%d,13], got %s" % (B, tuple(global_para.shape)))
-    if rot_feats.device != dev or global_para.device != dev:
-        raise ValueError("gcn_head: rot_feats and global_para must be on the model's device %s" % dev)
+        raise ValueError("%s: global_para must be [B,13] = [%d,13], got %s" % (where, B, tuple(global_para.shape)))
+    _args.cuda(where, (("rot_feats", rot_feats), ("global_para", global_para)), dev)
     for (name, i), (di, do) in zip(LAYERS, DIMS):
         if tuple(_attr(mod, "%s.gc.%d.weight" % (name, i)).shape) != (di, do):
-            raise ValueError("gcn_head: %s.gc.%d.weight must be [%d,%d]" % (name, i, di, do))
+            raise ValueError("%s: %s.gc.%d.weight must be [%d,%d]" % (where, name, i, di, do))
     training = bool(model.training)
     bn = [_attr(mod, n) for n in BN_NAMES]
     bufs = [m.running_mean for m in bn] + [m.running_var for m in bn] + \
         [_attr(mod, k).reshape(-1) for k in ("r2p_A", "p2r_A", "I_n", "A_mask")] + [mod.mean_pose.reshape(-1)]
     if any(t.dtype != torch.float32 or not t.is_contiguous() for t in params + bufs):
-        raise ValueError("gcn_head: the head's parameters and buffers must be contiguous fp32")
+        raise ValueError("%s: the head's parameters and buffers must be contiguous fp32" % where)
     new_stats = torch.empty(2, 5, 24, device=dev) if training else None
     out = _GcnHead.apply(training, bufs, new_stats, rot_feats.float().contiguous(), global_para.float().contiguous(),
                          *params)
@@ -195,12 +191,10 @@ class _HeadLosses(torch.autograd.Function):
         f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
         p_, c0_, c1_, t_, g_ = (f32(t) for t in (pose0, coord0, coord1, target, gt))
         grads = [torch.empty_like(t) for t in (p_, c0_, c1_)]
-        lib = _lib.load()
         with torch.cuda.device(dev):
             losses = _empty(3, dev=dev)
-            _lib.check(lib.danet_gcn_head_losses(B, _lib.ptr(p_), _lib.ptr(c0_), _lib.ptr(c1_), _lib.ptr(t_), _lib.ptr(g_),
-                                                 _lib.ptr(has), float(rot_w), float(pos_w), _lib.ptr(losses),
-                                                 *(_lib.ptr(t) for t in grads), _lib.stream_ptr(dev)), "gcn_head_losses")
+            _lib.call("gcn_head_losses", B, _lib.ptr(p_), _lib.ptr(c0_), _lib.ptr(c1_), _lib.ptr(t_), _lib.ptr(g_),
+                      _lib.ptr(has), float(rot_w), float(pos_w), _lib.ptr(losses), *map(_lib.ptr, grads), device=dev)
         ctx.grads = grads
         ctx.dtypes = (pose0.dtype, coord0.dtype, coord1.dtype)
         return losses
@@ -362,24 +356,21 @@ def _model_state(model, branch):
     return low, state, dev
 
 
-def _check_input(fn, name, t, dev, shape_tail, desc):
-    if not isinstance(t, torch.Tensor):
-        raise ValueError("danet_b200.regressor.%s: %s must be a tensor (got %s)" % (fn, name, type(t).__name__))
-    if t.dtype != torch.float32:
-        raise ValueError("danet_b200.regressor.%s: %s must be float32 (got %s)" % (fn, name, t.dtype))
-    if t.device != dev:
-        raise ValueError("danet_b200.regressor.%s: %s is on %s, the model on %s" % (fn, name, t.device, dev))
+def _branch_input(where, name, t, dev, shape_tail, desc):
+    """t is fp32 on the model's device `dev`, of shape [B, *shape_tail, S, S] with B, S >= 1"""
+    _args.tensor(where, name, t, contiguous=False)
+    _args.cuda(where, [(name, t)], dev)
     n = len(shape_tail)
     if t.dim() != n + 3 or tuple(t.shape[1:n + 1]) != shape_tail or t.shape[0] < 1 or t.shape[-1] < 1 or \
             t.shape[-1] != t.shape[-2]:
-        raise ValueError("danet_b200.regressor.%s: %s must be %s with B >= 1 (got %s)" % (fn, name, desc, tuple(t.shape)))
+        raise ValueError("%s: %s must be %s with B >= 1 (got %s)" % (where, name, desc, tuple(t.shape)))
 
 
 def body_branch(model, body_iuv):
     """global_para [B,13] = body_net(body_iuv) + mean_cam_shape (smpl_regressor.py:688,696) in model.training's
     BatchNorm mode, differentiable w.r.t. body_iuv and body_net's parameters."""
     low, state, dev = _model_state(model, "body")
-    _check_input("body_branch", "body_iuv", body_iuv, dev, (75,), "[B,75,S,S]")
+    _branch_input("danet_b200.regressor.body_branch", "body_iuv", body_iuv, dev, (75,), "[B,75,S,S]")
     return run_branch(low, state, body_iuv.contiguous(), bool(model.training), _cuda_ops())
 
 
@@ -388,7 +379,7 @@ def limb_branch(model, part_iuv):
     pool (smpl_regressor.py:713-725) in model.training's BatchNorm mode, differentiable w.r.t. part_iuv and the
     parameters of limb_net and limb_reslayer."""
     low, state, dev = _model_state(model, "limb")
-    _check_input("limb_branch", "part_iuv", part_iuv, dev, (24, 3, 7), "[B,24,3,7,S,S]")
+    _branch_input("danet_b200.regressor.limb_branch", "part_iuv", part_iuv, dev, (24, 3, 7), "[B,24,3,7,S,S]")
     B, S = part_iuv.shape[0], part_iuv.shape[-1]
     y = run_branch(low, state, part_iuv.reshape(B * 24, 21, S, S).contiguous(), bool(model.training), _cuda_ops())
     return y.reshape(B, 24, -1)

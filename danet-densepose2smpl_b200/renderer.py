@@ -99,20 +99,18 @@ class IUV_Renderer(object):
         if B == 0:                                       # empty batch: empty outputs, nothing to launch
             return (torch.empty(0, 3, S, S, device=dev), torch.empty(0, S, S, dtype=torch.int32, device=dev) if want_face_idx else None,
                     [torch.empty(0, c, S, S, device=dev) for c in (25, 25, 25, 15)] if want_maps else [None] * 4)
-        lib = _lib.load()
         with torch.cuda.device(dev):
             h = self._handle(dev)
-            need = int(lib.danet_raster_workspace_bytes(h, B))
+            need = int(_lib.load().danet_raster_workspace_bytes(h, B))
             ws = self._ws.get(dev.index)
             if ws is None or ws.numel() < need:
-                ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                ws = _lib.workspace(need, dev)
                 self._ws[dev.index] = ws
             img = torch.empty(B, 3, S, S, device=dev)
             fidx = torch.empty(B, S, S, dtype=torch.int32, device=dev) if want_face_idx else None
             maps = [torch.empty(B, c, S, S, device=dev) for c in (25, 25, 25, 15)] if want_maps else [None] * 4
-            _lib.check(lib.danet_raster_iuv(h, B, _lib.ptr(verts_c), _lib.ptr(cam_c), _lib.ptr(img), _lib.ptr(fidx),
-                                            _lib.ptr(maps[0]), _lib.ptr(maps[1]), _lib.ptr(maps[2]), _lib.ptr(maps[3]),
-                                            _lib.ptr(ws), _lib.stream_ptr()), "raster_iuv")
+            _lib.call("raster_iuv", h, B, _lib.ptr(verts_c), _lib.ptr(cam_c), _lib.ptr(img), _lib.ptr(fidx),
+                      *map(_lib.ptr, maps), _lib.ptr(ws))
         return img, fidx, maps
 
     def verts2uvimg(self, verts, cam):

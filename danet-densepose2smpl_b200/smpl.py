@@ -141,7 +141,6 @@ class SMPL(nn.Module):
         key = device.index if device.index is not None else torch.cuda.current_device()
         if key in self._handles:
             return self._handles[key]
-        lib = _lib.load()
         keep = []
 
         def host(t, dt):
@@ -173,7 +172,7 @@ class SMPL(nn.Module):
         d.joint_map = host(self.joint_map, np.int32)
         h = ctypes.c_void_p()
         with torch.cuda.device(key):
-            _lib.check(lib.danet_smpl_create(ctypes.byref(d), ctypes.byref(h)), "smpl_create")
+            _lib.check(_lib.load().danet_smpl_create(ctypes.byref(d), ctypes.byref(h)), "smpl_create")
         self._handles[key] = h
         return h
 
@@ -207,7 +206,7 @@ class SMPL(nn.Module):
         key = (device.index, )
         ws = self._ws.get(key)
         if ws is None or ws.numel() < need:
-            ws = torch.empty(int(need), dtype=torch.uint8, device=device)
+            ws = _lib.workspace(need, device)
             self._ws[key] = ws
         return ws
 
@@ -289,7 +288,6 @@ class SMPL(nn.Module):
             return self.ModelOutput(vertices=z(0, self.v_template.shape[0], 3) if return_verts else None, global_orient=go_in,
                                     body_pose=bp_in, joints=z(0, len(self.joint_map), 3), joints_J19=z(0, 19, 3),
                                     smpl_joints=z(0, 24, 3), betas=betas, full_pose=None)
-        lib = _lib.load()
         with torch.cuda.device(dev):
             h = self._handle(dev)
             V = self.v_template.shape[0]
@@ -300,10 +298,8 @@ class SMPL(nn.Module):
             jh = torch.empty(B, nh, 3, device=dev) if nh else None
             rot = torch.empty(B, 24, 3, 3, device=dev) if kind != 0 else None
             ws = self._workspace(h, B, dev)
-            _lib.check(lib.danet_smpl_forward(h, B, _lib.ptr(betas), _lib.ptr(pose), kind, _lib.ptr(verts),
-                                              _lib.ptr(joints), _lib.ptr(smpl_joints), _lib.ptr(jh),
-                                              _lib.ptr(rot), _lib.ptr(ws), int(bodies_per_cta),
-                                              _lib.stream_ptr()), "smpl_forward")
+            _lib.call("smpl_forward", h, B, _lib.ptr(betas), _lib.ptr(pose), kind, _lib.ptr(verts), _lib.ptr(joints),
+                      _lib.ptr(smpl_joints), _lib.ptr(jh), _lib.ptr(rot), _lib.ptr(ws), int(bodies_per_cta))
         if transl is not None:
             # smplx adds the translation to joints and vertices; models/smpl.py:27-46 takes smpl_joints from the
             # translated joints, and eval.py regresses the H36M joints from the translated vertices
@@ -337,14 +333,13 @@ class SMPL(nn.Module):
         f = lambda t: t.detach().to(dev, torch.float32).contiguous()
         betas, R, gv = f(betas), f(rotmats).reshape(B, 24, 3, 3), f(grad_vertices)
         gj = f(grad_smpl_joints) if grad_smpl_joints is not None else None
-        lib = _lib.load()
         with torch.cuda.device(dev):
             h = self._handle(dev)
-            ws = torch.empty(int(lib.danet_smpl_backward_workspace_bytes(h, B)), dtype=torch.uint8, device=dev)
+            ws = _lib.workspace(_lib.load().danet_smpl_backward_workspace_bytes(h, B), dev)
             gb = torch.empty(B, betas.shape[1], device=dev)
             gR = torch.empty(B, 24, 3, 3, device=dev)
-            _lib.check(lib.danet_smpl_backward(h, B, _lib.ptr(betas), _lib.ptr(R), _lib.ptr(gv), _lib.ptr(gj), _lib.ptr(gb),
-                                               _lib.ptr(gR), _lib.ptr(ws), _lib.stream_ptr(dev)), "smpl_backward")
+            _lib.call("smpl_backward", h, B, _lib.ptr(betas), _lib.ptr(R), _lib.ptr(gv), _lib.ptr(gj), _lib.ptr(gb),
+                      _lib.ptr(gR), _lib.ptr(ws), device=dev)
         return gb, gR
 
     def joints_h36m(self):
@@ -438,7 +433,6 @@ def mpjpe_h36m(pred_j17, gt_j14):
     B = pred_j17.shape[0]
     out = torch.empty(B, device=pred_j17.device)
     with torch.cuda.device(pred_j17.device):
-        _lib.check(_lib.load().danet_mpjpe_h36m(B, _lib.ptr(pred_j17.float().contiguous()),
-                                               _lib.ptr(gt_j14.float().contiguous()), _lib.ptr(out),
-                                               _lib.stream_ptr()), "mpjpe_h36m")
+        pred, gt = pred_j17.float().contiguous(), gt_j14.float().contiguous()      # locals: they must outlive the launch
+        _lib.call("mpjpe_h36m", B, _lib.ptr(pred), _lib.ptr(gt), _lib.ptr(out))
     return out

@@ -16,47 +16,23 @@ part_crops is iuv_estimator.py:193-204: 24x F.affine_grid(theta_i.detach(), xd.s
 concatenated on dim 1.  Inputs are fp32, contiguous NCHW CUDA tensors; anything else raises ValueError (there is no
 fall-back to torch).  Nothing synchronises with the host and no float atomics are used: results repeat bit for bit, and
 forward + backward can be captured in a CUDA graph."""
-import numbers
-
 import torch
 from torch.autograd.function import once_differentiable
 
-from . import _lib
+from . import _args, _lib
 
 NUM_PARTS = 24
-
-
-def _check(fn, name, t, dim, dev=None):
-    if not isinstance(t, torch.Tensor):
-        raise ValueError("danet_b200.stn.%s: %s must be a tensor (got %s)" % (fn, name, type(t).__name__))
-    if t.dtype != torch.float32:
-        raise ValueError("danet_b200.stn.%s: %s must be float32 (got %s)" % (fn, name, t.dtype))
-    if t.dim() != dim:
-        raise ValueError("danet_b200.stn.%s: %s must be %d-D (got %s)" % (fn, name, dim, tuple(t.shape)))
-    if not t.is_contiguous():
-        raise ValueError("danet_b200.stn.%s: %s must be contiguous" % (fn, name))
-    if not t.is_cuda:
-        raise ValueError("danet_b200.stn.%s: %s must be a CUDA tensor (there is no CPU path)" % (fn, name))
-    if dev is not None and t.device != dev:
-        raise ValueError("danet_b200.stn.%s: %s is on %s, expected %s" % (fn, name, t.device, dev))
-
-
-def _number(fn, name, v):
-    if isinstance(v, bool) or not isinstance(v, numbers.Real):
-        raise ValueError("danet_b200.stn.%s: %s must be a number (got %r)" % (fn, name, v))
-    return float(v)
 
 
 class _PartCrops(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xd, thetas, align):
-        lib = _lib.load()
         dev = xd.device
         B, C, S, _ = xd.shape
         with torch.cuda.device(dev):
             crops = torch.empty(B, NUM_PARTS * C, S, S, dtype=torch.float32, device=dev)
-            _lib.check(lib.danet_part_crops_forward(B, C, S, _lib.ptr(xd), _lib.ptr(thetas), int(align), _lib.ptr(crops),
-                                                    _lib.stream_ptr(dev)), "part_crops_forward")
+            _lib.call("part_crops_forward", B, C, S, _lib.ptr(xd), _lib.ptr(thetas), int(align), _lib.ptr(crops),
+                      device=dev)
         ctx.save_for_backward(thetas)
         ctx.shape, ctx.align = (B, C, S), align
         return crops
@@ -68,13 +44,12 @@ class _PartCrops(torch.autograd.Function):
             return None, None, None
         (thetas,) = ctx.saved_tensors
         B, C, S = ctx.shape
-        lib = _lib.load()
         dev = thetas.device
         with torch.cuda.device(dev):
             gcrops = gcrops.to(torch.float32).contiguous()
             dxd = torch.empty(B, C, S, S, dtype=torch.float32, device=dev)
-            _lib.check(lib.danet_part_crops_backward(B, C, S, _lib.ptr(gcrops), _lib.ptr(thetas), int(ctx.align),
-                                                     _lib.ptr(dxd), _lib.stream_ptr(dev)), "part_crops_backward")
+            _lib.call("part_crops_backward", B, C, S, _lib.ptr(gcrops), _lib.ptr(thetas), int(ctx.align), _lib.ptr(dxd),
+                      device=dev)
         return dxd, None, None
 
 
@@ -88,14 +63,16 @@ def part_crops(xd, thetas, align_corners=False):
     given align_corners, rounded step by step in fp32 without fused multiply-adds.  Each output is a 4-term fp32 sum
     (within 2^-22 sum |w x| of exact).  The backward is the exact adjoint of the forward as executed, a gather summed
     in double: within 2^-24 |dxd| + 2^-45 sum |w dcrops| of the exact adjoint."""
-    fn = "part_crops"
-    _check(fn, "xd", xd, 4)
+    where = "danet_b200.stn.part_crops"
+    _args.tensor(where, "xd", xd, dim=4)
+    _args.cuda(where, [("xd", xd)])
     B, C, S, S2 = xd.shape
     if S != S2 or S < 2 or B < 1 or C < 1:
-        raise ValueError("danet_b200.stn.part_crops: xd must be [B, C, S, S] with S >= 2 (got %s)" % (tuple(xd.shape),))
-    _check(fn, "thetas", thetas, 4, xd.device)
+        raise ValueError("%s: xd must be [B, C, S, S] with S >= 2 (got %s)" % (where, tuple(xd.shape)))
+    _args.tensor(where, "thetas", thetas, dim=4)
+    _args.cuda(where, [("thetas", thetas)], xd.device)
     if tuple(thetas.shape) != (B, NUM_PARTS, 2, 3):
-        raise ValueError("danet_b200.stn.part_crops: thetas must be [%d, 24, 2, 3] (got %s)" % (B, tuple(thetas.shape)))
+        raise ValueError("%s: thetas must be [%d, 24, 2, 3] (got %s)" % (where, B, tuple(thetas.shape)))
     return _PartCrops.apply(xd, thetas.detach(), bool(align_corners))
 
 
@@ -111,39 +88,42 @@ def part_thetas(hm, index_pred, learned_ratio, learned_offset, *, vis_score=0.5,
     * (1 + scale_jitter (r1 - 0.5)), the hidden override 0.8 scale_box (parts 1..23), * (1 + scale_jitter (r2 - 0.5))
     with (r1, r2) = scale_noise[i, :, b] when scale_noise [24, 2, B] is given.  theta = [[s, 0, cx], [0, s, cy]].
     stn_centers are the jittered centres (the reference's stn_kps_pred)."""
-    fn = "part_thetas"
-    _check(fn, "hm", hm, 4)
+    where = "danet_b200.stn.part_thetas"
+    _args.tensor(where, "hm", hm, dim=4)
+    _args.cuda(where, [("hm", hm)])
     dev = hm.device
     B, J, Sh, Sh2 = hm.shape
     if J != NUM_PARTS or Sh != Sh2 or B < 1 or Sh < 1:
-        raise ValueError("danet_b200.stn.part_thetas: hm must be [B, 24, S, S] (got %s)" % (tuple(hm.shape),))
-    _check(fn, "index_pred", index_pred, 4, dev)
+        raise ValueError("%s: hm must be [B, 24, S, S] (got %s)" % (where, tuple(hm.shape)))
+    _args.tensor(where, "index_pred", index_pred, dim=4)
+    _args.cuda(where, [("index_pred", index_pred)], dev)
     if index_pred.shape[0] != B or index_pred.shape[1] != 25 or index_pred.shape[2] != index_pred.shape[3] \
             or index_pred.shape[2] < 2:
-        raise ValueError("danet_b200.stn.part_thetas: index_pred must be [%d, 25, S, S] with S >= 2 (got %s)"
-                         % (B, tuple(index_pred.shape)))
+        raise ValueError("%s: index_pred must be [%d, 25, S, S] with S >= 2 (got %s)"
+                         % (where, B, tuple(index_pred.shape)))
     for name, t in (("learned_ratio", learned_ratio), ("learned_offset", learned_offset)):
-        _check(fn, name, t, 1, dev)
+        _args.tensor(where, name, t, dim=1)
+        _args.cuda(where, [(name, t)], dev)
         if t.shape[0] != NUM_PARTS:
-            raise ValueError("danet_b200.stn.part_thetas: %s must be [24] (got %s)" % (name, tuple(t.shape)))
-    vis = _number(fn, "vis_score", vis_score)
-    cj, sj = _number(fn, "center_jitter", center_jitter), _number(fn, "scale_jitter", scale_jitter)
+            raise ValueError("%s: %s must be [24] (got %s)" % (where, name, tuple(t.shape)))
+    vis = _args.number(where, "vis_score", vis_score)
+    cj, sj = _args.number(where, "center_jitter", center_jitter), _args.number(where, "scale_jitter", scale_jitter)
     if center_noise is not None:
-        _check(fn, "center_noise", center_noise, 3, dev)
+        _args.tensor(where, "center_noise", center_noise, dim=3)
+        _args.cuda(where, [("center_noise", center_noise)], dev)
         if tuple(center_noise.shape) != (B, NUM_PARTS, 2):
-            raise ValueError("danet_b200.stn.part_thetas: center_noise must be [%d, 24, 2] (got %s)"
-                             % (B, tuple(center_noise.shape)))
+            raise ValueError("%s: center_noise must be [%d, 24, 2] (got %s)"
+                             % (where, B, tuple(center_noise.shape)))
     if scale_noise is not None:
-        _check(fn, "scale_noise", scale_noise, 3, dev)
+        _args.tensor(where, "scale_noise", scale_noise, dim=3)
+        _args.cuda(where, [("scale_noise", scale_noise)], dev)
         if tuple(scale_noise.shape) != (NUM_PARTS, 2, B):
-            raise ValueError("danet_b200.stn.part_thetas: scale_noise must be [24, 2, %d] (got %s)"
-                             % (B, tuple(scale_noise.shape)))
-    lib = _lib.load()
+            raise ValueError("%s: scale_noise must be [24, 2, %d] (got %s)"
+                             % (where, B, tuple(scale_noise.shape)))
     with torch.cuda.device(dev):
         centers = torch.empty(B, NUM_PARTS, 2, dtype=torch.float32, device=dev)
         thetas = torch.empty(B, NUM_PARTS, 2, 3, dtype=torch.float32, device=dev)
-        _lib.check(lib.danet_part_thetas(B, Sh, index_pred.shape[2], _lib.ptr(hm), _lib.ptr(index_pred),
-                                         _lib.ptr(learned_ratio), _lib.ptr(learned_offset), vis, _lib.ptr(center_noise), cj,
-                                         _lib.ptr(scale_noise), sj, int(bool(align_corners)), _lib.ptr(centers),
-                                         _lib.ptr(thetas), _lib.stream_ptr(dev)), "part_thetas")
+        _lib.call("part_thetas", B, Sh, index_pred.shape[2], _lib.ptr(hm), _lib.ptr(index_pred), _lib.ptr(learned_ratio),
+                  _lib.ptr(learned_offset), vis, _lib.ptr(center_noise), cj, _lib.ptr(scale_noise), sj,
+                  int(bool(align_corners)), _lib.ptr(centers), _lib.ptr(thetas), device=dev)
     return centers, thetas

@@ -134,3 +134,12 @@ def test_argument_errors():
     w7 = torch.randn(8, 8, 7, 7, device=DEV)
     with pytest.raises(ValueError):
         conv2d(x, w7, None, 1, 3)                                  # 7x7 stride 1: not an engine shape
+    # each tensor in turn (type, CUDA, dtype), then rank, then one device
+    with pytest.raises(ValueError, match="x must be float32"):
+        conv2d(x.double(), w.cpu(), None, 1, 1)
+    with pytest.raises(ValueError, match="weight must be a CUDA tensor"):
+        conv2d(x, w.cpu().double(), None, 1, 1)
+    with pytest.raises(ValueError, match="bias must be float32"):
+        conv2d(x, w, torch.zeros(8, dtype=torch.float64, device=DEV), 1, 1)
+    with pytest.raises(ValueError, match="4-D"):
+        conv2d(x[0], w, None, 1, 1)
