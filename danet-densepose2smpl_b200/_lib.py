@@ -48,12 +48,6 @@ class DgradPiece(ctypes.Structure):
                 ("jc0", c_int), ("jc1", c_int)]
 
 
-class GcnParams(ctypes.Structure):
-    _fields_ = [("adj", c_p), ("W", c_p * 5), ("b", c_p * 5), ("bn_scale", c_p * 5),
-                ("bn_shift", c_p * 5), ("dim_in", c_int * 5), ("dim_out", c_int * 5),
-                ("head_w", c_p), ("head_b", c_p), ("mean_pose", c_p)]
-
-
 class GcnTrainParams(ctypes.Structure):
     """danet_gcn_train_params: raw head parameters and their gradient pointers."""
     _fields_ = [("W", c_p * 5), ("b", c_p * 5), ("bn_weight", c_p * 5), ("bn_bias", c_p * 5),
@@ -94,7 +88,6 @@ SIGNATURES = {
     "danet_raster_workspace_bytes": (c_i64, [c_p, c_int]),
     "danet_raster_iuv": (c_int, [c_p, c_int, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
     "danet_iuv_img2map": (c_int, [c_int, c_int, c_p, c_p, c_p, c_p, c_p, c_p]),
-    "danet_conv2d": (c_int, [ctypes.POINTER(ConvDesc), c_int, c_p, c_p, c_p, c_p, c_p, c_p]),
     "danet_conv_tc_packed_bytes": (c_i64, [ctypes.POINTER(ConvDesc)]),
     "danet_conv_tc_pack": (c_int, [ctypes.POINTER(ConvDesc), c_p, c_p, c_p]),
     "danet_conv_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),
@@ -127,18 +120,9 @@ SIGNATURES = {
     "danet_part_thetas": (c_int, [c_int] * 3 + [c_p] * 4 + [c_f, c_p, c_f, c_p, c_f, c_int, c_p, c_p, c_p]),
     "danet_act_split": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
     "danet_act_merge": (c_int, [c_i64, c_p, c_p, c_p, c_p]),
-    "danet_nchw_to_nhwc": (c_int, [c_int, c_int, c_int, c_int, c_p, ctypes.POINTER(Act), c_p]),
-    "danet_fuse_sum": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(Act), c_p, c_int, ctypes.POINTER(Act), c_p]),
-    "danet_maxpool3x3s2": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(Act), ctypes.POINTER(Act), c_p]),
     "danet_global_avgpool": (c_int, [c_int, c_int, c_int, ctypes.POINTER(Act), c_p, c_p]),
     "danet_linear": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_p, c_p]),
-    "danet_iuv_clean_global": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
-                                       c_p, ctypes.POINTER(Act), c_p, c_p, c_p, c_p, c_p, c_p]),
     "danet_iuvmap_clean_nchw": (c_int, [c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
-    "danet_iuv_clean_parts": (c_int, [c_int, c_int, c_int, c_int, c_p, ctypes.POINTER(Act), c_p, c_p]),
-    "danet_stn_params": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_f, c_int, c_p, c_p, c_p]),
-    "danet_stn_sample": (c_int, [c_int, c_int, c_int, ctypes.POINTER(Act), c_p, c_int, ctypes.POINTER(Act), c_p]),
-    "danet_gcn_pose_head": (c_int, [c_int, ctypes.POINTER(GcnParams), c_p, c_p, c_p, c_p]),
     "danet_gcn_head_train_workspace_bytes": (c_i64, [c_int]),
     "danet_gcn_head_train_forward": (c_int, [c_int, ctypes.POINTER(GcnTrainParams), c_int] + [c_p] * 9),
     "danet_gcn_head_train_backward": (c_int, [c_int, ctypes.POINTER(GcnTrainParams), c_int] + [c_p] * 9),

@@ -13,8 +13,11 @@ void set_error(const char* fmt, ...) {
 
 extern "C" const char* danet_last_error(void) { return danet::g_err; }
 // 3: danet_act views, danet_conv_tc_group (split-fp16 tensor-core engine); 4: one weight packer
-// (danet_conv_tc_pack is stream-ordered, danet_conv_tc_pack_async is gone), danet_conv_tc_config without sub-tiles
-extern "C" int danet_version(void) { return 4; }
+// (danet_conv_tc_pack is stream-ordered, danet_conv_tc_pack_async is gone), danet_conv_tc_config without sub-tiles;
+// 5: the network's inference launches (danet_conv2d, danet_fuse_sum, danet_maxpool3x3s2, danet_nchw_to_nhwc,
+// danet_iuv_clean_global / _parts, danet_stn_params / _sample, danet_gcn_pose_head) are internal: network programs
+// and danet_net_run_step are their entry
+extern "C" int danet_version(void) { return 5; }
 extern "C" int danet_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     int dev = 0;
     DANET_CUDA(cudaGetDevice(&dev));

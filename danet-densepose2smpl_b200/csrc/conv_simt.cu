@@ -1,5 +1,5 @@
-// fp32 implicit-GEMM convolution on the FMA pipe (NHWC) -- the exact-parity path of the
-// network half and the fallback for shapes the wgmma kernel does not take.
+// fp32 implicit-GEMM convolution on the FMA pipe (NHWC) -- the independent fp32 check path of the network half
+// (conv_algo='simt'); its launcher (launchers.cuh) runs the network program's conv2d steps.
 // Replaces nn.Conv2d (+ folded BatchNorm2d + ReLU + residual add) of models/module/hr_module.py,
 // models/module/res_module.py; grouped convolutions (res_module.py:335-342,500-535) are expressed
 // as `wsets` weight sets over the (batch,part)-flattened image axis (see include/danet_b200.h).
@@ -7,7 +7,7 @@
 // CTA tile: 64 (image, output pixel) rows of one weight set x 64 output channels, 256 threads, 4x4 outputs per
 // thread (32 x 32, 2x2 per thread, when the 64 x 64 grid would have fewer than 120 CTAs), K streamed in
 // (tap, 16-channel) chunks through shared memory with register prefetch.
-#include "common.cuh"
+#include "launchers.cuh"
 
 namespace danet {
 
@@ -140,13 +140,22 @@ k_conv_simt(ConvArgs a) {
     }
 }
 
-int conv_simt_launch(const danet_conv_desc* d, const float* x, const float* w, const float* bias,
-                     const float* residual, float* y, cudaStream_t stream) {
+int conv2d(const danet_conv_desc& d, const float* x, const float* w, const float* bias, const float* residual, float* y,
+           cudaStream_t stream) {
+    DANET_CHECK(d.N >= 0 && d.H > 0 && d.W > 0 && d.Cin > 0 && d.Cout > 0, "danet_conv2d: bad sizes");
+    DANET_CHECK(d.Cin % 4 == 0 && d.Cout % 4 == 0, "danet_conv2d: Cin (%d) and Cout (%d) must be multiples of 4 (pad channels)", d.Cin, d.Cout);
+    DANET_CHECK(d.ksize >= 1 && d.ksize <= 7 && d.stride >= 1 && d.stride <= 2 && d.pad >= 0, "danet_conv2d: bad ksize/stride/pad");
+    DANET_CHECK(d.wsets >= 1, "danet_conv2d: wsets must be >= 1");
+    DANET_CHECK(d.H + 2 * d.pad >= d.ksize && d.W + 2 * d.pad >= d.ksize, "danet_conv2d: kernel larger than padded input");
+    DANET_CHECK(d.wsets <= 65535, "danet_conv2d: wsets=%d exceeds 65535", d.wsets);
+    if (d.N == 0) return 0;
+    DANET_CHECK(x && w && y, "danet_conv2d: null pointer");
+    DANET_CHECK(d.flags == 0, "danet_conv2d: flags are only taken by the tensor-core path");
     ConvArgs a;
-    a.N = d->N; a.H = d->H; a.W = d->W; a.Cin = d->Cin; a.Cout = d->Cout; a.ks = d->ksize;
-    a.stride = d->stride; a.pad = d->pad; a.wsets = d->wsets; a.relu = d->relu;
-    a.Ho = (d->H + 2 * d->pad - d->ksize) / d->stride + 1;
-    a.Wo = (d->W + 2 * d->pad - d->ksize) / d->stride + 1;
+    a.N = d.N; a.H = d.H; a.W = d.W; a.Cin = d.Cin; a.Cout = d.Cout; a.ks = d.ksize;
+    a.stride = d.stride; a.pad = d.pad; a.wsets = d.wsets; a.relu = d.relu;
+    a.Ho = (d.H + 2 * d.pad - d.ksize) / d.stride + 1;
+    a.Wo = (d.W + 2 * d.pad - d.ksize) / d.stride + 1;
     a.x = x; a.w = w; a.bias = bias; a.res = residual; a.y = y;
     const int rows = cdiv(a.N, a.wsets) * a.Ho * a.Wo;
     const long long ctas64 = (long long)cdiv(rows, 64) * cdiv(a.Cout, 64) * a.wsets;
@@ -162,26 +171,3 @@ int conv_simt_launch(const danet_conv_desc* d, const float* x, const float* w, c
 }
 
 }  // namespace danet
-
-using namespace danet;
-
-static int check_conv_desc(const danet_conv_desc* d) {
-    DANET_CHECK(d, "danet_conv2d: null descriptor");
-    DANET_CHECK(d->N >= 0 && d->H > 0 && d->W > 0 && d->Cin > 0 && d->Cout > 0, "danet_conv2d: bad sizes");
-    DANET_CHECK(d->Cin % 4 == 0 && d->Cout % 4 == 0, "danet_conv2d: Cin (%d) and Cout (%d) must be multiples of 4 (pad channels)", d->Cin, d->Cout);
-    DANET_CHECK(d->ksize >= 1 && d->ksize <= 7 && d->stride >= 1 && d->stride <= 2 && d->pad >= 0, "danet_conv2d: bad ksize/stride/pad");
-    DANET_CHECK(d->wsets >= 1, "danet_conv2d: wsets must be >= 1");
-    DANET_CHECK(d->H + 2 * d->pad >= d->ksize && d->W + 2 * d->pad >= d->ksize, "danet_conv2d: kernel larger than padded input");
-    DANET_CHECK(d->wsets <= 65535, "danet_conv2d: wsets=%d exceeds 65535", d->wsets);
-    return 0;
-}
-
-extern "C" int danet_conv2d(const danet_conv_desc* d, int32_t algo, const void* x, const float* w,
-                            const float* bias, const float* residual, void* y, danet_stream_t stream) {
-    if (check_conv_desc(d) != 0) return -1;
-    if (d->N == 0) return 0;
-    DANET_CHECK(x && w && y, "danet_conv2d: null pointer");
-    DANET_CHECK(algo == DANET_CONV_SIMT, "danet_conv2d: algo %d -- the tensor-core path is danet_conv_tc_group (split-fp16 activations)", algo);
-    DANET_CHECK(d->flags == 0, "danet_conv2d: flags are only taken by the tensor-core path");
-    return conv_simt_launch(d, (const float*)x, w, bias, residual, (float*)y, (cudaStream_t)stream);
-}

@@ -1,6 +1,9 @@
 // Memory-bound fp32 glue kernels of the DaNet network half (NHWC activations).
 // Each replaces a chain of small ATen launches in the reference; citations per kernel.
-#include "common.cuh"
+// Their launchers (launchers.cuh) are internal, run by the network program's step decoder (net.cu); the
+// activations are padded to 8 channels, so the pools, the fuse and the STN sampler only have 8-channel kernels.
+// danet_global_avgpool, danet_linear and danet_iuvmap_clean_nchw are C ABI entries of their own.
+#include "launchers.cuh"
 #include "stn_common.cuh"
 #include <cuda_fp16.h>
 #include <math.h>
@@ -27,49 +30,6 @@ __global__ void k_nchw_to_nhwc(int N, int C, int HW, int Cp, const float* __rest
         return;
     }
     for (int c = 0; c < Cp; ++c) act_st1(y, i * Cp + c, c < C ? x[((size_t)n * C + c) * HW + p] : 0.0f);
-}
-
-// ------------------------------------------------------------------------------------------
-// iuvmap_clean, global heads (utils/iuvmap.py:6-38 via danet.py:79 / iuv_estimator.py:127)
-// ------------------------------------------------------------------------------------------
-__global__ void k_iuv_clean_global(int B, int HW, int Chead, int off_u, int off_v, int off_i, int off_a,
-                                   int Cb, const float* __restrict__ heads, ActV body,
-                                   uint8_t* __restrict__ amax, float* un, float* vn, float* in_, float* an) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= B * HW) return;
-    const int b = i / HW, pix = i % HW;
-    const float* h = heads + (size_t)i * Chead;
-    float I[25], A[15];
-#pragma unroll
-    for (int c = 0; c < 25; ++c) I[c] = h[off_i + c];
-    const int best = argmax_first(I, 25);
-    amax[i] = (uint8_t)best;
-    const size_t o = (size_t)i * Cb;
-    // the cleaned row [U*onehot 25 | V*onehot 25 | onehot 25 | pad] (the products keep the reference's NaN/Inf
-    // propagation of `U * mask`), written as 4-channel vectors to every view
-    auto elem = [&](int cc) -> float {
-        if (cc < 25) return ((cc == best) ? 1.0f : 0.0f) * h[off_u + cc];
-        if (cc < 50) return ((cc - 25 == best) ? 1.0f : 0.0f) * h[off_v + cc - 25];
-        if (cc < 75) return (cc - 50 == best) ? 1.0f : 0.0f;
-        return 0.0f;
-    };
-    if ((Cb & 3) == 0) {
-        for (int c = 0; c < Cb; c += 4) act_st4(body, o + c, make_float4(elem(c), elem(c + 1), elem(c + 2), elem(c + 3)));
-    } else {
-        for (int c = 0; c < Cb; ++c) act_st1(body, o + c, elem(c));
-    }
-    for (int c = 0; c < 25; ++c) {
-        const float oh = (c == best) ? 1.0f : 0.0f;
-        if (un) un[((size_t)b * 25 + c) * HW + pix] = oh * h[off_u + c];
-        if (vn) vn[((size_t)b * 25 + c) * HW + pix] = oh * h[off_v + c];
-        if (in_) in_[((size_t)b * 25 + c) * HW + pix] = oh;
-    }
-    if (an) {
-#pragma unroll
-        for (int c = 0; c < 15; ++c) A[c] = h[off_a + c];
-        const int ba = argmax_first(A, 15);
-        for (int c = 0; c < 15; ++c) an[((size_t)b * 15 + c) * HW + pix] = (c == ba) ? 1.0f : 0.0f;
-    }
 }
 
 // 24 per-part iuvmap_clean calls of danet.py:93-98 in one pass (one thread per pixel; rows are read and
@@ -234,10 +194,10 @@ k_stn_params(int B, int S, int Chm, const float* __restrict__ hm, const uint8_t*
     }
 }
 
-// 24x affine_grid + grid_sample (iuv_estimator.py:193-204), C % 4 == 0
-// grid = one block per (crop b*24+part, output row py); threads run over (px, 4-channel group) of the row: the
+// 24x affine_grid + grid_sample (iuv_estimator.py:193-204), C % 8 == 0
+// grid = one block per (crop b*24+part, output row py); threads run over (px, V-channel group) of the row: the
 // per-element 64-bit div/mod chain of the first version cost more than the 16-byte store it fed
-// V = channels per work item: 8 when C % 8 == 0 (16-byte accesses on the fp16 planes), else 4; same arithmetic per channel
+// V = channels per work item: 8 (16-byte accesses on the fp16 planes)
 template <int V>
 __global__ void __launch_bounds__(256)
 k_stn_sample(int B, int S, int C, ActV xd, const float* __restrict__ theta,
@@ -401,13 +361,6 @@ constexpr int kGcnThreads = 256;
 constexpr int kGcnMaxF = 256;
 constexpr int kGcnTF = 32;                 // input features per streamed weight tile
 
-struct GcnArgs {
-    const float* adj;
-    const float* W[5]; const float* b[5]; const float* bn_s[5]; const float* bn_t[5];
-    int din[5], dout[5];
-    const float* head_w; const float* head_b; const float* mean_pose;
-};
-
 __device__ __forceinline__ void rot6d_cols(const float* x, float* R) {
     const float a1x = x[0], a1y = x[2], a1z = x[4], a2x = x[1], a2y = x[3], a2z = x[5];
     const float n1 = fmaxf(sqrtf(a1x * a1x + a1y * a1y + a1z * a1z), 1e-12f);
@@ -522,28 +475,29 @@ k_gcn_pose_head(int B, GcnArgs g, const float* __restrict__ rot_feats, const flo
 
 using namespace danet;
 
-static int check_act(const danet_act* a, const char* what, bool need_c8 = false, int C = 8) {
+static int check_act(const danet_act* a, const char* what, int C) {
     DANET_CHECK(act_any(a), "%s: activation has neither an fp32 view nor fp16 planes", what);
     DANET_CHECK(!(a->lo && !a->hi), "%s: lo plane without hi plane", what);
     DANET_CHECK(!a->hi || C % 4 == 0, "%s: fp16 planes need C %% 4 == 0 (got %d)", what, C);
-    (void)need_c8;
     return 0;
 }
 
-extern "C" int danet_nchw_to_nhwc(int32_t N, int32_t C, int32_t HW, int32_t Cp, const float* x, const danet_act* y,
-                                  danet_stream_t s) {
+int danet::nchw_to_nhwc(int N, int C, int HW, int Cp, const float* x, const danet_act* y, cudaStream_t s) {
     DANET_CHECK(N >= 0 && C > 0 && Cp >= C && HW > 0, "danet_nchw_to_nhwc: bad sizes");
     if (N == 0) return 0;
     DANET_CHECK(x, "danet_nchw_to_nhwc: null pointer");
-    if (check_act(y, "danet_nchw_to_nhwc", false, 4) != 0) return -1;
-    k_nchw_to_nhwc<<<cdiv(N * HW, 256), 256, 0, (cudaStream_t)s>>>(N, C, HW, Cp, x, actv(y));
+    if (check_act(y, "danet_nchw_to_nhwc", 4) != 0) return -1;
+    k_nchw_to_nhwc<<<cdiv(N * HW, 256), 256, 0, s>>>(N, C, HW, Cp, x, actv(y));
     DANET_LAUNCH_CHECK();
     return 0;
 }
 
-// Staged form of k_iuv_clean_global: a CTA moves PX pixels' head rows through shared memory with coalesced 16-byte
-// loads (the thread-per-pixel form reads each 384-byte row with strided 4-byte loads: 3.3x the DRAM bytes under ncu),
-// computes per pixel from shared memory and writes the NHWC views as one contiguous run.  Same expressions per element.
+// ------------------------------------------------------------------------------------------
+// iuvmap_clean, global heads (utils/iuvmap.py:6-38 via danet.py:79 / iuv_estimator.py:127)
+// ------------------------------------------------------------------------------------------
+// A CTA moves PX pixels' head rows through shared memory with coalesced 16-byte loads (a thread per pixel reading its
+// 384-byte row with strided 4-byte loads moved 3.3x the DRAM bytes under ncu), computes per pixel from shared memory and
+// writes the NHWC views as one contiguous run.  The products keep the reference's NaN / Inf propagation of `U * mask`.
 template <int PX>
 __global__ void __launch_bounds__(128)
 k_iuv_clean_global_staged(int npix_total, int HW, int Chead, int off_u, int off_v, int off_i, int off_a, int Cb,
@@ -606,82 +560,70 @@ k_iuv_clean_global_staged(int npix_total, int HW, int Chead, int off_u, int off_
     }
 }
 
-extern "C" int danet_iuv_clean_global(int32_t B, int32_t HW, int32_t Chead, int32_t off_u, int32_t off_v,
-                                      int32_t off_i, int32_t off_a, int32_t Cbody, const float* heads,
-                                      const danet_act* body_iuv, uint8_t* index_argmax, float* u_nchw, float* v_nchw,
-                                      float* i_nchw, float* ann_nchw, danet_stream_t s) {
+int danet::iuv_clean_global(int B, int HW, int Chead, int off_u, int off_v, int off_i, int off_a, int Cbody,
+                            const float* heads, const danet_act* body_iuv, uint8_t* index_argmax, float* u_nchw,
+                            float* v_nchw, float* i_nchw, float* ann_nchw, cudaStream_t s) {
+    constexpr int kPx = 64;
+    const size_t smem = (size_t)kPx * (Chead + 1 + Cbody + 1) * sizeof(float);
     DANET_CHECK(B >= 0 && HW > 0 && Cbody >= 75, "danet_iuv_clean_global: bad sizes");
     DANET_CHECK(off_u + 25 <= Chead && off_v + 25 <= Chead && off_i + 25 <= Chead && off_a + 15 <= Chead,
                 "danet_iuv_clean_global: head offsets exceed Chead=%d", Chead);
+    DANET_CHECK(Chead % 4 == 0 && Cbody % 4 == 0 && smem <= 48 * 1024,
+                "danet_iuv_clean_global: Chead=%d and Cbody=%d must be multiples of 4 and fit 64 pixels in 48 KB",
+                Chead, Cbody);
     if (B == 0) return 0;
     DANET_CHECK(heads && index_argmax, "danet_iuv_clean_global: null pointer");
-    if (check_act(body_iuv, "danet_iuv_clean_global", false, 4) != 0) return -1;
-    constexpr int kPx = 64;
-    const size_t smem = (size_t)kPx * (Chead + 1 + Cbody + 1) * sizeof(float);
-    if ((Chead & 3) == 0 && (Cbody & 3) == 0 && smem <= 48 * 1024 && ((uintptr_t)heads & 15) == 0) {
-        k_iuv_clean_global_staged<kPx><<<cdiv(B * HW, kPx), 128, smem, (cudaStream_t)s>>>(
-            B * HW, HW, Chead, off_u, off_v, off_i, off_a, Cbody, heads, actv(body_iuv), index_argmax, u_nchw, v_nchw, i_nchw, ann_nchw);
-    } else {
-        k_iuv_clean_global<<<cdiv(B * HW, 128), 128, 0, (cudaStream_t)s>>>(B, HW, Chead, off_u, off_v, off_i, off_a, Cbody,
-                                                                         heads, actv(body_iuv), index_argmax, u_nchw, v_nchw,
-                                                                         i_nchw, ann_nchw);
-    }
+    DANET_CHECK(((uintptr_t)heads & 15) == 0, "danet_iuv_clean_global: heads must be 16-byte aligned");
+    if (check_act(body_iuv, "danet_iuv_clean_global", 4) != 0) return -1;
+    k_iuv_clean_global_staged<kPx><<<cdiv(B * HW, kPx), 128, smem, s>>>(
+        B * HW, HW, Chead, off_u, off_v, off_i, off_a, Cbody, heads, actv(body_iuv), index_argmax, u_nchw, v_nchw, i_nchw, ann_nchw);
     DANET_LAUNCH_CHECK();
     return 0;
 }
 
-extern "C" int danet_iuv_clean_parts(int32_t N, int32_t HW, int32_t Cx, int32_t Cy, const float* x, const danet_act* y,
-                                     float* raw_nchw, danet_stream_t s) {
-    DANET_CHECK(N >= 0 && HW > 0 && Cx >= 21 && Cy >= 21, "danet_iuv_clean_parts: bad sizes");
+int danet::iuv_clean_parts(int N, int HW, int Cx, int Cy, const float* x, const danet_act* y, float* raw_nchw,
+                           cudaStream_t s) {
+    DANET_CHECK(N >= 0 && HW > 0 && Cx >= 24 && Cy >= 24 && Cx % 4 == 0 && Cy % 4 == 0,
+                "danet_iuv_clean_parts: bad sizes (Cx, Cy must be >= 24 and %% 4 == 0)");
     if (N == 0) return 0;
     DANET_CHECK(x, "danet_iuv_clean_parts: null pointer");
-    if (check_act(y, "danet_iuv_clean_parts", false, Cy) != 0) return -1;
-    if (Cx % 4 == 0 && Cy % 4 == 0 && Cx >= 24 && Cy >= 24)
-        k_iuv_clean_parts<true><<<cdiv((int64_t)N * HW, 128), 128, 0, (cudaStream_t)s>>>(N, HW, Cx, Cy, x, actv(y), raw_nchw);
-    else {
-        DANET_CHECK(!y->hi, "danet_iuv_clean_parts: fp16 planes need Cx, Cy >= 24 and %% 4 == 0");
-        k_iuv_clean_parts<false><<<cdiv((int64_t)N * HW, 128), 128, 0, (cudaStream_t)s>>>(N, HW, Cx, Cy, x, actv(y), raw_nchw);
-    }
+    if (check_act(y, "danet_iuv_clean_parts", Cy) != 0) return -1;
+    k_iuv_clean_parts<true><<<cdiv((int64_t)N * HW, 128), 128, 0, s>>>(N, HW, Cx, Cy, x, actv(y), raw_nchw);
     DANET_LAUNCH_CHECK();
     return 0;
 }
 
-extern "C" int danet_stn_params(int32_t B, int32_t S, int32_t Chm, const float* hm, const uint8_t* index_argmax,
-                                const float* learned_ratio, const float* learned_offset, float vis_thresh,
-                                int32_t align_corners, float* centers, float* theta, danet_stream_t s) {
+int danet::stn_params(int B, int S, int Chm, const float* hm, const uint8_t* index_argmax, const float* learned_ratio,
+                      const float* learned_offset, float vis_thresh, int align_corners, float* centers, float* theta,
+                      cudaStream_t s) {
     DANET_CHECK(B >= 0 && S > 1 && Chm >= 24 && Chm % 4 == 0, "danet_stn_params: bad sizes (Chm must be >=24 and %%4==0)");
     if (B == 0) return 0;
     DANET_CHECK(hm && index_argmax && learned_ratio && learned_offset && centers && theta, "danet_stn_params: null pointer");
-    k_stn_params<<<B, kStnThreads, 0, (cudaStream_t)s>>>(B, S, Chm, hm, index_argmax, learned_ratio, learned_offset,
-                                                        vis_thresh, align_corners, centers, theta);
+    k_stn_params<<<B, kStnThreads, 0, s>>>(B, S, Chm, hm, index_argmax, learned_ratio, learned_offset, vis_thresh,
+                                           align_corners, centers, theta);
     DANET_LAUNCH_CHECK();
     return 0;
 }
 
-extern "C" int danet_stn_sample(int32_t B, int32_t S, int32_t C, const danet_act* xd, const float* theta,
-                                int32_t align_corners, const danet_act* crops, danet_stream_t s) {
-    DANET_CHECK(B >= 0 && S > 1 && C > 0 && C % 4 == 0, "danet_stn_sample: bad sizes (C %% 4 must be 0)");
+int danet::stn_sample(int B, int S, int C, const danet_act* xd, const float* theta, int align_corners,
+                      const danet_act* crops, cudaStream_t s) {
+    DANET_CHECK(B >= 0 && S > 1 && C > 0 && C % 8 == 0, "danet_stn_sample: bad sizes (C %% 8 must be 0)");
     if (B == 0) return 0;
     DANET_CHECK(theta, "danet_stn_sample: null pointer");
-    if (check_act(xd, "danet_stn_sample(xd)", false, C) != 0 || check_act(crops, "danet_stn_sample(crops)", false, C) != 0) return -1;
+    if (check_act(xd, "danet_stn_sample(xd)", C) != 0 || check_act(crops, "danet_stn_sample(crops)", C) != 0) return -1;
     DANET_CHECK((int64_t)B * 24 * S < (1LL << 31), "danet_stn_sample: batch too large for one launch");
-    if (C % 8 == 0) {
-        const int items = S * (C / 8);
-        k_stn_sample<8><<<B * 24 * S, items >= 256 ? 256 : (items + 31) / 32 * 32, 0, (cudaStream_t)s>>>(B, S, C, actv(xd), theta, align_corners, actv(crops));
-    } else {
-        const int items = S * (C / 4);
-        k_stn_sample<4><<<B * 24 * S, items >= 256 ? 256 : (items + 31) / 32 * 32, 0, (cudaStream_t)s>>>(B, S, C, actv(xd), theta, align_corners, actv(crops));
-    }
+    const int items = S * (C / 8);
+    k_stn_sample<8><<<B * 24 * S, items >= 256 ? 256 : (items + 31) / 32 * 32, 0, s>>>(B, S, C, actv(xd), theta, align_corners, actv(crops));
     DANET_LAUNCH_CHECK();
     return 0;
 }
 
-extern "C" int danet_fuse_sum(int32_t N, int32_t H, int32_t W, int32_t C, int32_t nterms, const danet_act* terms,
-                              const int32_t* factors, int32_t relu, const danet_act* y, danet_stream_t s) {
-    DANET_CHECK(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "danet_fuse_sum: bad sizes (C %% 4 must be 0)");
+int danet::fuse_sum(int N, int H, int W, int C, int nterms, const danet_act* terms, const int32_t* factors, int relu,
+                    const danet_act* y, cudaStream_t s) {
+    DANET_CHECK(N >= 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "danet_fuse_sum: bad sizes (C %% 8 must be 0)");
     DANET_CHECK(nterms >= 1 && nterms <= 4 && terms && factors, "danet_fuse_sum: 1..4 terms required");
     if (N == 0) return 0;
-    if (check_act(y, "danet_fuse_sum(y)", false, C) != 0) return -1;
+    if (check_act(y, "danet_fuse_sum(y)", C) != 0) return -1;
     FuseArgs a;
     a.n = nterms;
     for (int j = 0; j < 4; ++j) { a.t[j] = actv(nullptr); a.f[j] = 1; }
@@ -689,26 +631,22 @@ extern "C" int danet_fuse_sum(int32_t N, int32_t H, int32_t W, int32_t C, int32_
         const int f = factors[j];
         DANET_CHECK((f == 1 || f == 2 || f == 4 || f == 8) && H % f == 0 && W % f == 0,
                     "danet_fuse_sum: term %d has bad upsample factor %d for %dx%d", j, f, H, W);
-        if (check_act(&terms[j], "danet_fuse_sum(term)", false, C) != 0) return -1;
+        if (check_act(&terms[j], "danet_fuse_sum(term)", C) != 0) return -1;
         a.t[j] = actv(&terms[j]); a.f[j] = f == 1 ? 0 : (f == 2 ? 1 : (f == 4 ? 2 : 3));
     }
     DANET_CHECK((int64_t)N * H < (1LL << 31) && (int64_t)W * (C / 4) < (1 << 24) && C / 4 < (1 << 16), "danet_fuse_sum: tensor too large for one launch");
-    if (C % 8 == 0)
-        k_fuse_sum<8><<<dim3(N * H, cdiv(W * (C / 8), 256)), 256, 0, (cudaStream_t)s>>>(N, H, W, C / 8, (1ull << 40) / (unsigned long long)(C / 8) + 1ull, a, relu, actv(y));
-    else
-        k_fuse_sum<4><<<dim3(N * H, cdiv(W * (C / 4), 256)), 256, 0, (cudaStream_t)s>>>(N, H, W, C / 4, (1ull << 40) / (unsigned long long)(C / 4) + 1ull, a, relu, actv(y));
+    k_fuse_sum<8><<<dim3(N * H, cdiv(W * (C / 8), 256)), 256, 0, s>>>(N, H, W, C / 8, (1ull << 40) / (unsigned long long)(C / 8) + 1ull, a, relu, actv(y));
     DANET_LAUNCH_CHECK();
     return 0;
 }
 
-extern "C" int danet_maxpool3x3s2(int32_t N, int32_t H, int32_t W, int32_t C, const danet_act* x, const danet_act* y, danet_stream_t s) {
-    DANET_CHECK(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "danet_maxpool3x3s2: bad sizes (C %% 4 must be 0)");
+int danet::maxpool3x3s2(int N, int H, int W, int C, const danet_act* x, const danet_act* y, cudaStream_t s) {
+    DANET_CHECK(N >= 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "danet_maxpool3x3s2: bad sizes (C %% 8 must be 0)");
     if (N == 0) return 0;
-    if (check_act(x, "danet_maxpool3x3s2(x)", false, C) != 0 || check_act(y, "danet_maxpool3x3s2(y)", false, C) != 0) return -1;
+    if (check_act(x, "danet_maxpool3x3s2(x)", C) != 0 || check_act(y, "danet_maxpool3x3s2(y)", C) != 0) return -1;
     const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
     DANET_CHECK((int64_t)N * Ho < (1LL << 31) && (int64_t)Wo * (C / 4) <= 65535LL * 256, "danet_maxpool3x3s2: tensor too large for one launch");
-    if (C % 8 == 0) k_maxpool3x3s2<8><<<dim3(N * Ho, cdiv(Wo * (C / 8), 256)), 256, 0, (cudaStream_t)s>>>(N, H, W, C / 8, actv(x), actv(y));
-    else k_maxpool3x3s2<4><<<dim3(N * Ho, cdiv(Wo * (C / 4), 256)), 256, 0, (cudaStream_t)s>>>(N, H, W, C / 4, actv(x), actv(y));
+    k_maxpool3x3s2<8><<<dim3(N * Ho, cdiv(Wo * (C / 8), 256)), 256, 0, s>>>(N, H, W, C / 8, actv(x), actv(y));
     DANET_LAUNCH_CHECK();
     return 0;
 }
@@ -717,7 +655,7 @@ extern "C" int danet_global_avgpool(int32_t N, int32_t HW, int32_t C, const dane
     DANET_CHECK(N >= 0 && HW > 0 && C > 0, "danet_global_avgpool: bad sizes");
     if (N == 0) return 0;
     DANET_CHECK(y, "danet_global_avgpool: null pointer");
-    if (check_act(x, "danet_global_avgpool", false, 4) != 0) return -1;
+    if (check_act(x, "danet_global_avgpool", 4) != 0) return -1;
     k_global_avgpool<<<cdiv(N * C, 256), 256, 0, (cudaStream_t)s>>>(N, HW, C, actv(x), y);
     DANET_LAUNCH_CHECK();
     return 0;
@@ -733,21 +671,17 @@ extern "C" int danet_linear(int32_t N, int32_t In, int32_t Out, const float* x, 
     return 0;
 }
 
-extern "C" int danet_gcn_pose_head(int32_t B, const danet_gcn_params* p, const float* rot_feats,
-                                   const float* global_para, float* para, danet_stream_t s) {
-    DANET_CHECK(B >= 0 && p, "danet_gcn_pose_head: bad arguments");
+int danet::gcn_pose_head(int B, const GcnArgs& g, const float* rot_feats, const float* global_para, float* para,
+                         cudaStream_t s) {
+    DANET_CHECK(B >= 0, "danet_gcn_pose_head: bad arguments");
     if (B == 0) return 0;
-    DANET_CHECK(rot_feats && global_para && para && p->adj && p->head_w && p->head_b && p->mean_pose,
+    DANET_CHECK(rot_feats && global_para && para && g.adj && g.head_w && g.head_b && g.mean_pose,
                 "danet_gcn_pose_head: null pointer");
-    GcnArgs g;
-    g.adj = p->adj; g.head_w = p->head_w; g.head_b = p->head_b; g.mean_pose = p->mean_pose;
     for (int l = 0; l < 5; ++l) {
-        DANET_CHECK(p->W[l] && p->b[l] && p->bn_scale[l] && p->bn_shift[l], "danet_gcn_pose_head: layer %d has null params", l);
-        DANET_CHECK(p->dim_in[l] > 0 && p->dim_in[l] <= kGcnMaxF && p->dim_out[l] > 0 && p->dim_out[l] <= kGcnMaxF &&
-                    p->dim_in[l] % 4 == 0 && p->dim_out[l] % 4 == 0 && ((uintptr_t)p->W[l] & 15) == 0,
-                    "danet_gcn_pose_head: layer %d dims %d->%d must be <= %d, multiples of 4, W 16-byte aligned", l, p->dim_in[l], p->dim_out[l], kGcnMaxF);
-        g.W[l] = p->W[l]; g.b[l] = p->b[l]; g.bn_s[l] = p->bn_scale[l]; g.bn_t[l] = p->bn_shift[l];
-        g.din[l] = p->dim_in[l]; g.dout[l] = p->dim_out[l];
+        DANET_CHECK(g.W[l] && g.b[l] && g.bn_s[l] && g.bn_t[l], "danet_gcn_pose_head: layer %d has null params", l);
+        DANET_CHECK(g.din[l] > 0 && g.din[l] <= kGcnMaxF && g.dout[l] > 0 && g.dout[l] <= kGcnMaxF &&
+                    g.din[l] % 4 == 0 && g.dout[l] % 4 == 0 && ((uintptr_t)g.W[l] & 15) == 0,
+                    "danet_gcn_pose_head: layer %d dims %d->%d must be <= %d, multiples of 4, W 16-byte aligned", l, g.din[l], g.dout[l], kGcnMaxF);
     }
     DANET_CHECK(g.din[0] == 128 && g.dout[0] == 128 && g.dout[3] == 128 && g.din[4] == 128 && g.dout[4] == 128,
                 "danet_gcn_pose_head: expected 128-d r2p / refine-out / p2r features");
@@ -755,7 +689,7 @@ extern "C" int danet_gcn_pose_head(int32_t B, const danet_gcn_params* p, const f
     static unsigned long long attr_devs = 0;
     if (first_use_on_current_device(&attr_devs) != 0)
         DANET_CUDA(cudaFuncSetAttribute(k_gcn_pose_head, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_gcn_pose_head<<<B, kGcnThreads, smem, (cudaStream_t)s>>>(B, g, rot_feats, global_para, para);
+    k_gcn_pose_head<<<B, kGcnThreads, smem, s>>>(B, g, rot_feats, global_para, para);
     DANET_LAUNCH_CHECK();
     return 0;
 }

@@ -2,12 +2,13 @@
 // weights that danet_b200.plan.Plan.export() writes for one batch size) and replays it -- the network half of
 // DaNet.infer_net (models/danet/danet.py:78-98: img2iuv -> iuvmap_clean -> iuv2smpl up to `para`) for hosts without
 // Python.  The Python plan runs each of its launches as one such step through danet_net_run_step, so both decode
-// every launch with the same prepare / run_step and results are identical.
+// every launch with the same prepare / run_step and results are identical.  run_step is the one caller of the
+// inference launchers (launchers.cuh), which check each step's arguments before they reach a kernel.
 //
 // Program layout (little endian, sections 16-byte aligned):
 //   Header | u64 buf_bytes[n_buf] | {u64 off, u64 bytes} consts[n_const] | Out outs[n_out] | step stream | const payload
 //   step = {u32 op, n_i, n_f, n_r} i32[n_i] f32[n_f] Ref[n_r];  Ref = {u32 kind (0 null, 1 buffer, 2 const, 3 input), u32 id, u64 off}
-#include "common.cuh"
+#include "launchers.cuh"
 #include <string.h>
 
 namespace danet {
@@ -33,7 +34,7 @@ struct Step {
     std::vector<void*> p;
     std::vector<danet_conv_problem> probs;     // OP_CONV_GROUP
     std::vector<danet_act> acts;               // OP_FUSE terms
-    danet_gcn_params gcn;                      // OP_GCN_HEAD
+    GcnArgs gcn;                               // OP_GCN_HEAD
 };
 struct Out { std::string name; void* ptr; uint64_t bytes; uint32_t elem_bytes; int32_t dims[4]; };
 
@@ -106,12 +107,12 @@ int prepare(Step& s) {
     case OP_LINEAR: DANET_CHECK(ni == 3 && nr == 5, "net: malformed linear step"); break;
     case OP_GCN_HEAD: {
         DANET_CHECK(ni == 11 && nr == 27, "net: malformed gcn_head step");
-        danet_gcn_params& g = s.gcn;
+        GcnArgs& g = s.gcn;
         g.adj = (const float*)P[0];
         for (int l = 0; l < 5; ++l) {
             g.W[l] = (const float*)P[1 + l]; g.b[l] = (const float*)P[6 + l];
-            g.bn_scale[l] = (const float*)P[11 + l]; g.bn_shift[l] = (const float*)P[16 + l];
-            g.dim_in[l] = I[1 + l]; g.dim_out[l] = I[6 + l];
+            g.bn_s[l] = (const float*)P[11 + l]; g.bn_t[l] = (const float*)P[16 + l];
+            g.din[l] = I[1 + l]; g.dout[l] = I[6 + l];
         }
         g.head_w = (const float*)P[21]; g.head_b = (const float*)P[22]; g.mean_pose = (const float*)P[23];
         break;
@@ -127,20 +128,19 @@ int run_step(const Step& s, cudaStream_t st) {
     switch (s.op) {
     case OP_INPUT: {
         danet_act y = act_of(P + 1);
-        return danet_nchw_to_nhwc(I[0], I[1], I[2], I[3], (const float*)P[0], &y, st);
+        return nchw_to_nhwc(I[0], I[1], I[2], I[3], (const float*)P[0], &y, st);
     }
     case OP_CONV_GROUP: return danet_conv_tc_group(I[0], s.probs.data(), st);
-    case OP_CONV_SIMT: {
-        danet_conv_desc d = desc_of(I);
-        return danet_conv2d(&d, DANET_CONV_SIMT, P[0], (const float*)P[1], (const float*)P[2], (const float*)P[3], P[4], st);
-    }
+    case OP_CONV_SIMT:
+        return conv2d(desc_of(I), (const float*)P[0], (const float*)P[1], (const float*)P[2], (const float*)P[3],
+                      (float*)P[4], st);
     case OP_FUSE: {
         danet_act y = act_of(P + 3 * I[4]);
-        return danet_fuse_sum(I[0], I[1], I[2], I[3], I[4], s.acts.data(), I + 6, I[5], &y, st);
+        return fuse_sum(I[0], I[1], I[2], I[3], I[4], s.acts.data(), I + 6, I[5], &y, st);
     }
     case OP_MAXPOOL: {
         danet_act x = act_of(P), y = act_of(P + 3);
-        return danet_maxpool3x3s2(I[0], I[1], I[2], I[3], &x, &y, st);
+        return maxpool3x3s2(I[0], I[1], I[2], I[3], &x, &y, st);
     }
     case OP_AVGPOOL: {
         danet_act x = act_of(P);
@@ -148,25 +148,25 @@ int run_step(const Step& s, cudaStream_t st) {
     }
     case OP_CLEAN_GLOBAL: {
         danet_act body = act_of(P + 1);
-        return danet_iuv_clean_global(I[0], I[1], I[2], I[3], I[4], I[5], I[6], I[7], (const float*)P[0], &body,
-                                      (uint8_t*)P[4], (float*)P[5], (float*)P[6], (float*)P[7], (float*)P[8], st);
+        return iuv_clean_global(I[0], I[1], I[2], I[3], I[4], I[5], I[6], I[7], (const float*)P[0], &body,
+                                (uint8_t*)P[4], (float*)P[5], (float*)P[6], (float*)P[7], (float*)P[8], st);
     }
     case OP_CLEAN_PARTS: {
         danet_act y = act_of(P + 1);
-        return danet_iuv_clean_parts(I[0], I[1], I[2], I[3], (const float*)P[0], &y, (float*)P[4], st);
+        return iuv_clean_parts(I[0], I[1], I[2], I[3], (const float*)P[0], &y, (float*)P[4], st);
     }
     case OP_STN_PARAMS:
-        return danet_stn_params(I[0], I[1], I[2], (const float*)P[0], (const uint8_t*)P[1], (const float*)P[2],
-                                (const float*)P[3], s.f[0], I[3], (float*)P[4], (float*)P[5], st);
+        return stn_params(I[0], I[1], I[2], (const float*)P[0], (const uint8_t*)P[1], (const float*)P[2],
+                          (const float*)P[3], s.f[0], I[3], (float*)P[4], (float*)P[5], st);
     case OP_STN_SAMPLE: {
         danet_act xd = act_of(P), crops = act_of(P + 4);
-        return danet_stn_sample(I[0], I[1], I[2], &xd, (const float*)P[3], I[3], &crops, st);
+        return stn_sample(I[0], I[1], I[2], &xd, (const float*)P[3], I[3], &crops, st);
     }
     case OP_LINEAR:
         return danet_linear(I[0], I[1], I[2], (const float*)P[0], (const float*)P[1], (const float*)P[2],
                             (const float*)P[3], (float*)P[4], st);
     case OP_GCN_HEAD:
-        return danet_gcn_pose_head(I[0], &s.gcn, (const float*)P[24], (const float*)P[25], (float*)P[26], st);
+        return gcn_pose_head(I[0], s.gcn, (const float*)P[24], (const float*)P[25], (float*)P[26], st);
     }
     set_error("net: unknown step kind %u", s.op);
     return -1;

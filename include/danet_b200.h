@@ -188,12 +188,10 @@ int danet_iuv_img2map(int32_t B, int32_t S, const float* img, float* maps_u, flo
 
 /* ------------------------------------------------------------------------------------------
  * Network half (models/danet/, models/module/).  NHWC activations as danet_act views (fp32 and/or
- * split-fp16 planes): every glue kernel below reads the fp32 view when present, else hi(+lo), and writes
- * every view that is present.
+ * split-fp16 planes): an entry reads the fp32 view when present, else hi(+lo), and writes every view that is
+ * present.  The network's other layers (input conversion, fp32-FMA convolution, HRNet fuse, pools, iuvmap_clean,
+ * STN, GCN head) run as steps of a network program (danet_net_*, below).
  * ------------------------------------------------------------------------------------------ */
-enum { DANET_CONV_SIMT = 0,            /* fp32 FMA implicit GEMM (independent fp32 check path)      */
-       DANET_CONV_TC = 1 };            /* wgmma tensor-core implicit GEMM (danet_conv_tc_group)     */
-
 typedef struct {
     int32_t N, H, W, Cin;              /* input  [N,H,W,Cin]                                      */
     int32_t Cout, ksize, stride, pad;  /* output [N,Ho,Wo,Cout], Ho = (H+2*pad-ksize)/stride+1     */
@@ -216,12 +214,6 @@ typedef struct {
  * Tensor-core convolutions read hi/lo through TMA tensor maps and write any of the views. */
 typedef struct { float* f32; void* hi; void* lo; } danet_act;
 
-/* Weight packing for the SIMT path: w [wsets][ksize*ksize*Cin][Cout] (tap-major, then cin),
- * bias [wsets][Cout] (BN folded by the caller).  residual (or NULL) has the output's shape and is
- * added before the ReLU (res_module.py:40-56,77-97).  fp32 tensors only. */
-int danet_conv2d(const danet_conv_desc* d, int32_t algo, const void* x, const float* w,
-                 const float* bias, const float* residual, void* y, danet_stream_t stream);
-
 /* Tensor-core path.  One launch runs up to 6 independent convolutions (e.g. the parallel branches of an
  * HRNet stage, hr_module.py:165-166) over one persistent grid.  w_packed comes from danet_conv_tc_pack with
  * the SAME descriptor (flags included).  x needs hi (+ lo in exact mode); res: f32, or hi(+lo), or all NULL;
@@ -236,9 +228,10 @@ int danet_conv_tc_group(int32_t n, const danet_conv_problem* problems, danet_str
 /* The depth of the shared activation / weight rings (stages[0], stages[1]) a launch over a group of n problems would
  * get; the rings are sized for the largest member.  Nonzero if the group cannot share one launch. */
 int danet_conv_tc_config(int32_t n, const danet_conv_desc* descs, int32_t* stages);
-/* bytes / packing helper: converts the SIMT layout above into the swizzled shared-memory image blocks of
- * split-fp16 weights the wgmma kernel bulk-copies (device -> device, stream-ordered, no host synchronisation or
- * allocation: capturable in a CUDA graph).  Header word 2 of w_packed is its scratch while it runs. */
+/* bytes / packing helper: converts weights in the SIMT layout w [wsets][ksize*ksize*Cin][Cout] (tap-major, then cin)
+ * into the swizzled shared-memory image blocks of split-fp16 weights the wgmma kernel bulk-copies (device -> device,
+ * stream-ordered, no host synchronisation or allocation: capturable in a CUDA graph).  Header word 2 of w_packed is its
+ * scratch while it runs. */
 int64_t danet_conv_tc_packed_bytes(const danet_conv_desc* d);
 int danet_conv_tc_pack(const danet_conv_desc* d, const float* w_simt, void* w_packed, danet_stream_t stream);
 int danet_conv_tc_supported(const danet_conv_desc* d);
@@ -363,7 +356,7 @@ int danet_global_avgpool_backward(int32_t NC, int32_t HW, const float* dy, float
 int danet_linear_backward(int32_t N, int32_t In, int32_t Out, const float* x, const float* w, const float* dy, float* dx,
                           float* dw, float* db, danet_stream_t stream);
 
-/* HRNet fuse (models/module/hr_module.py:161-179, the training form of danet_fuse_sum): fp32 NCHW
+/* HRNet fuse (models/module/hr_module.py:161-179) in training: fp32 NCHW
  * y [N,C,H,W] = relu?(up(t_0) + up(t_1) + ...), term j [N,C,H/f_j,W/f_j] upsampled nearest by f_j in {1,2,4,8},
  * added in list order (bit-identical to the F.interpolate + add + relu chain).  terms / factors: host arrays of
  * nterms (1..4) entries.  The backward writes one term's gradient: dterm = the f x f block sums of dy * [y > 0]
@@ -391,76 +384,19 @@ int danet_part_thetas(int32_t B, int32_t Sh, int32_t Si, const float* hm, const 
                       float center_jitter, const float* scale_noise, float scale_jitter, int32_t align_corners,
                       float* centers, float* theta, danet_stream_t stream);
 
-/* input boundary: x NCHW [N,C,HW] -> y NHWC [N,HW,Cp] with Cp >= C zero-padded channels
- * (images arrive NCHW: demo.py:106, eval.py:147) */
-int danet_nchw_to_nhwc(int32_t N, int32_t C, int32_t HW, int32_t Cp, const float* x, const danet_act* y,
-                       danet_stream_t stream);
-
-/* hr_module.py:161-179 fuse: y = relu(sum_j up_{f_j}(t_j)); t_j [N,H/f_j,W/f_j,C] nearest-upsampled
- * by f_j in {1,2,4,8}; nterms <= 4; summed in argument order */
-int danet_fuse_sum(int32_t N, int32_t H, int32_t W, int32_t C, int32_t nterms,
-                   const danet_act* terms /*[nterms]*/, const int32_t* factors, int32_t relu, const danet_act* y,
-                   danet_stream_t stream);
-/* nn.MaxPool2d(3,2,1) (res_module.py:409) NHWC */
-int danet_maxpool3x3s2(int32_t N, int32_t H, int32_t W, int32_t C, const danet_act* x, const danet_act* y,
-                       danet_stream_t stream);
 /* nn.AdaptiveAvgPool2d(1) NHWC [N,H,W,C] -> [N,C] */
 int danet_global_avgpool(int32_t N, int32_t HW, int32_t C, const danet_act* x, float* y, danet_stream_t stream);
 /* y[n,o] = sum_i x[n,i] w[o,i] + b[o] (+ add[o])  (SmplResNet.final_layer + mean_cam_shape) */
 int danet_linear(int32_t N, int32_t In, int32_t Out, const float* x, const float* w, const float* b,
                  const float* add, float* y, danet_stream_t stream);
 
-/* utils/iuvmap.py:6-38 iuvmap_clean on the global prediction heads.
- * heads [B,HW,Chead] NHWC with channel blocks (U 25 | V 25 | Index 25 | Ann 15) at offsets
- * off_u/off_v/off_i/off_a.  Writes body_iuv [B,HW,Cbody>=75] NHWC (cat[U,V,I] of danet.py:85,
- * pad channels zeroed) and the
- * uint8 argmax map [B,HW]; optional NCHW outputs u/v/i [B,25,HW], ann [B,15,HW] (danet.py:81). */
-int danet_iuv_clean_global(int32_t B, int32_t HW, int32_t Chead, int32_t off_u, int32_t off_v,
-                           int32_t off_i, int32_t off_a, int32_t Cbody, const float* heads,
-                           const danet_act* body_iuv, uint8_t* index_argmax, float* u_nchw, float* v_nchw,
-                           float* i_nchw, float* ann_nchw, danet_stream_t stream);
 /* utils/iuvmap.py:6-38 with the reference's own signature: NCHW maps U,V,Index [B,C,HW] and
  * optional AnnIndex [B,Ca,HW] (NULL to skip) -> cleaned maps of the same shapes */
 int danet_iuvmap_clean_nchw(int32_t B, int32_t C, int32_t Ca, int32_t HW, const float* U, const float* V,
                             const float* I, const float* A, float* oU, float* oV, float* oI, float* oA,
                             danet_stream_t stream);
-/* danet.py:93-98: 24 per-part iuvmap_clean calls.  x [N,HW,Cx] NHWC with (U 7|V 7|I 7) in the
- * first 21 channels (N = batch*24) -> y [N,HW,Cy>=21] cleaned (pad channels zeroed); optional raw
- * copy in the reference's
- * layout part_iuv_pred [N,21,HW] (iuv_estimator.py:208-211). */
-int danet_iuv_clean_parts(int32_t N, int32_t HW, int32_t Cx, int32_t Cy, const float* x, const danet_act* y,
-                          float* raw_nchw, danet_stream_t stream);
-/* iuv_estimator.py:137-140,176-184,262-301: soft-argmax centres of 10*hm, part visibility,
- * affine thetas.  hm [B,HW,Chm] (24 heatmap channels first), index_argmax [B,HW] ->
- * centers [B,24,2] (x,y in [-1,1]), theta [B,24,3] = (scale, cx, cy).
- * smpl2dp/parents/children tables are the reference's (utils/smpl_utlis.py) and compiled in.
- * align_corners: 0 = torch>=1.3 default semantics, 1 = torch 1.1 semantics. */
-int danet_stn_params(int32_t B, int32_t S, int32_t Chm, const float* hm, const uint8_t* index_argmax,
-                     const float* learned_ratio, const float* learned_offset, float vis_thresh,
-                     int32_t align_corners, float* centers, float* theta, danet_stream_t stream);
-/* iuv_estimator.py:193-204: 24x affine_grid + grid_sample (bilinear, zeros) of xd [B,S,S,C]
- * -> crops [B*24,S,S,C] (image index b*24+part) */
-int danet_stn_sample(int32_t B, int32_t S, int32_t C, const danet_act* xd, const float* theta,
-                     int32_t align_corners, const danet_act* crops, danet_stream_t stream);
-
-/* smpl_regressor.py:858-895 + GCN.py:29-92 + geometry.py:47-61: r2p_gcn -> refine_gcn(+res) ->
- * p2r_gcn -> grouped 1x1 pose head + mean_pose -> rot6d_to_rotmat; also concatenates
- * global_para (cam,shape) -> para [B,229].  All matrices are device pointers prepared once:
- *   adj [3][24*24]   (r2p_A, normalised refine adjacency, p2r_A)
- *   per GCN layer l (5 layers: r2p, refine0..2, p2r): W_l [in,out], b_l [out], bn scale/shift [24]
- *   head_w [24][6][128], head_b [24*6], mean_pose [144]. */
-typedef struct {
-    const float* adj;
-    const float* W[5]; const float* b[5]; const float* bn_scale[5]; const float* bn_shift[5];
-    int32_t dim_in[5]; int32_t dim_out[5];
-    const float* head_w; const float* head_b; const float* mean_pose;
-} danet_gcn_params;
-int danet_gcn_pose_head(int32_t B, const danet_gcn_params* p, const float* rot_feats /*[B,24,128]*/,
-                        const float* global_para /*[B,13]*/, float* para /*[B,229]*/,
-                        danet_stream_t stream);
-
 /* ------------------------------------------------------------------------------------------
- * Regressor head, training path (csrc/gcn_train.cu): the same head as danet_gcn_pose_head, with raw (unfolded)
+ * Regressor head, training path (csrc/gcn_train.cu): the same head as the network program's, with raw (unfolded)
  * parameters, BatchNorm1d(24) on batch statistics (training = 1) or on the running statistics (training = 0), the
  * intermediate supervision heads of training mode and the backward.  fp32 throughout; no float atomics, every
  * reduction in a fixed order (bit-repeatable), no host synchronisation (capturable in a CUDA graph).
@@ -506,8 +442,8 @@ int danet_gcn_head_losses(int32_t B, const float* pose0, const float* coord0, co
 /* ------------------------------------------------------------------------------------------
  * Whole-network entry (csrc/net.cu).  Replaces the network half of DaNet.infer_net
  * (models/danet/danet.py:78-98: img2iuv -> iuvmap_clean -> iuv2smpl, up to `para`) for hosts without Python.
- * A "network program" is what danet_b200.plan.Plan.export() writes for ONE batch size: the launch steps (each one of
- * the entries above, with its arguments), the activation buffer table and the BN-folded, packed weights.  Loading
+ * A "network program" is what danet_b200.plan.Plan.export() writes for ONE batch size: the launch steps (each one
+ * kernel launch, with its arguments), the activation buffer table and the BN-folded, packed weights.  Loading
  * allocates everything on the CURRENT device; infer replays the steps (optionally as one CUDA graph, captured on the
  * first call).  danet_net_run_step runs one step record directly; the Python plan launches every kernel through it, so
  * it and a loaded program decode the same records with the same code.  A danet_net_t owns its buffers: one infer at a

@@ -1,5 +1,5 @@
 """GPU unit parity of the network-half kernels (csrc/conv_simt.cu, conv_tc.cu, glue.cu) against a
-plain torch fp32 reference of the same op (tests/emul_ops.py restates each op with torch)."""
+plain torch fp32 reference of the same op (oracle/net_ops.py restates each op with torch)."""
 import numpy as np
 import pytest
 import torch

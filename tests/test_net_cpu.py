@@ -1,6 +1,6 @@
 """CPU tests of the host logic of the network half (graph wiring, BatchNorm folding, weight packing,
 buffer planning, state_dict surface) using the torch test double of the kernel-level ops
-(tests/emul_ops.py) against golden vectors produced by the reference's own modules."""
+(oracle/net_ops.py) against golden vectors produced by the reference's own modules."""
 import os
 
 import numpy as np
@@ -220,3 +220,53 @@ def test_exported_steps_have_the_arity_the_loader_requires(algo):
         else:
             assert (len(ints), nf, nr) == _FIXED_ARITY[op], s
     assert seen == set(range(1, 13)) - {3 if algo == "tc" else 2}
+
+
+class _PlaneOps(TorchEmulOps):
+    """The test double with CudaOps' fp16 planes, so tensor-core plans carry the views they carry on the GPU."""
+
+    def planes(self, precision):
+        return 2 if precision == "exact" else 1
+
+
+def _step_conditions(name, ints, ptrs):
+    """Conditions of the launchers in csrc/glue.cu and csrc/conv_simt.cu beyond the loader's arity check, for one step
+    record; returns the names of those it breaks."""
+    bad = []
+    if name in ("fuse_sum", "maxpool", "stn_sample"):
+        C = ints[2] if name == "stn_sample" else ints[3]
+        if C % 8:
+            bad.append("C % 8 == 0")                       # the 8-channel kernels are the only ones
+    if name == "clean_global":
+        Chead, Cbody, heads = ints[2], ints[7], ptrs[0]
+        if Chead % 4 or Cbody % 4:
+            bad.append("Chead, Cbody % 4 == 0")
+        if 64 * (Chead + 1 + Cbody + 1) * 4 > 48 * 1024:
+            bad.append("64 staged pixels fit in 48 KB")
+        if heads.data_ptr() % 16:
+            bad.append("heads 16-byte aligned")
+    if name == "clean_parts" and (min(ints[2], ints[3]) < 24 or ints[2] % 4 or ints[3] % 4):
+        bad.append("Cx, Cy >= 24 and % 4 == 0")
+    if name == "conv2d" and ints[10] != 0:
+        bad.append("flags == 0")
+    return bad
+
+
+@pytest.mark.parametrize("width", [32, 48])
+@pytest.mark.parametrize("algo,precision", [("simt", "exact"), ("tc", "exact"), ("tc", "fast")])
+def test_plan_steps_meet_the_launchers_conditions(width, algo, precision):
+    """Every step record a plan emits (B = 2 and 64) meets the conditions the executor's launchers check, so no plan
+    step is refused: the fuse, pool and STN-sampler records carry C % 8 == 0, the global iuvmap_clean record fits the
+    staged kernel and the part iuvmap_clean record has 24-channel rows.  The simt plan does not depend on precision."""
+    from danet_b200.plan import wire
+    net = build(width, conv_algo=algo, precision=precision)
+    ops = _PlaneOps()
+    for B in (2, 64):
+        plan = net.plan_for(B, "cpu", ops=ops)
+        assert plan.P == (0 if algo == "simt" else ops.planes(precision))
+        names = set()
+        for s in plan.steps:
+            _op, ints, _floats, ptrs = wire(s.name, s.args)
+            assert not _step_conditions(s.name, ints, ptrs), (B, s.name, ints, _step_conditions(s.name, ints, ptrs))
+            names.add(s.name)
+        assert {"fuse_sum", "maxpool", "stn_sample", "clean_global", "clean_parts"} <= names
