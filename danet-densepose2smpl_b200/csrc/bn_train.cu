@@ -4,16 +4,18 @@
 // bit for bit and the calls can be captured in a CUDA graph.
 //
 // BatchNorm (x [N][C][HW], n = N * HW values per channel):
-//   Statistics.  Training mode sums x and x * x per channel in double (chan_sums_partial: (channel, image chunk)
-//       partials with a fixed thread assignment and tree); k_bn2d_stats_finish adds the chunks in order and writes
-//       mean, invstd = 1 / sqrt(biased var + eps) and the new running statistics (momentum, unbiased variance
-//       n / (n - 1)).  Eval mode uses the running statistics.  save [2][C] (double) keeps mean and invstd for the
-//       backward.
-//   Apply.  y = ((x - m_hi) - m_lo) * (w * invstd) + b (+ r), then ReLU: the mean as an fp32 pair (hi + lo) is
-//       subtracted before scaling, so |mean| >> std does not cancel away the deviation.
-//   Backward.  dz = dy masked by y > 0 with ReLU (threshold_backward on the output).  One reduction gives sum dz and
-//       sum dz * (x - mean) in double; dbias = sum dz, dweight = invstd * sum dz (x - mean).  One apply pass writes
-//       dx = w invstd (dz - sum dz / n - xhat * sum dz xhat / n) (training) or w invstd dz (eval), and dresidual = dz.
+//   Statistics.  Training mode sums x - K and (x - K)^2 per channel in double, K = x[0][c][0] (chan_sums_partial:
+//       (channel, image chunk) partials with a fixed thread assignment and tree); k_bn2d_stats_finish adds the chunks
+//       in order and writes mean = K + sum (x - K) / n, var = sum (x - K)^2 / n - (mean - K)^2, invstd =
+//       1 / sqrt(var + eps) and the new running statistics (momentum, unbiased variance n / (n - 1)).  K is a data
+//       element, so (mean - K)^2 / var <= n - 1 whatever |mean| / std is: the subtraction loses at most log2(n) bits of
+//       the double sums, where unshifted sums lose 2 log2(|mean| / std).  Eval mode uses the running statistics.  save
+//       [2][C] (double) keeps mean and invstd for the backward.
+//   Apply.  y = ((x - m_hi) - m_lo) * (w * invstd) + b (+ r), then ReLU (NaN stays NaN): the mean as an fp32 pair
+//       (hi + lo) is subtracted before scaling, so |mean| >> std does not cancel away the deviation.
+//   Backward.  dz = dy with ReLU zeroed where y <= 0 (torch's threshold_backward on the output: a NaN y passes dy).
+//       One reduction gives sum dz and sum dz * (x - mean) in double; dbias = sum dz, dweight = invstd * sum dz
+//       (x - mean).  One apply pass writes dx = w invstd (dz - sum dz / n - xhat * sum dz xhat / n) (training) or w invstd dz (eval), and dresidual = dz.
 //   The apply passes run over the flat tensor in float4 groups; a group that straddles two (n, c) planes (planes of
 //       49 or 2 elements) looks up each element's channel.
 //
@@ -23,7 +25,8 @@
 //
 // HRNet fuse: the forward adds the nearest-upsampled terms in list order, so it is bit-identical to the reference's
 // F.interpolate + add + relu chain.  The backward of a term upsampled by f is a gather: one thread per term element
-// sums dy * [y > 0] over its f x f block in row-major order (fp32: within (f^2 - 1) 2^-24 sum |dy| of the exact sum).
+// sums dy * [not y <= 0] over its f x f block in row-major order (fp32: within (f^2 - 1) 2^-24 sum |dy| of the exact
+// sum).  The ReLU keeps NaN forward and passes dy at a NaN output backward, as BatchNorm's does.
 //
 // Branch tails (their forwards are danet_global_avgpool and danet_linear of glue.cu): the average pool's backward
 // spreads dy / HW over the plane; the linear layer's backward sums dx = dy W, dW = dy^T x and db = sum dy in double, in
@@ -47,9 +50,11 @@ __device__ __forceinline__ void split_f(double v, float* hi, float* lo) {
     *lo = (float)(v - (double)*hi);
 }
 
-// Training: chunks of sum x and sum x^2 in order -> save (mean, invstd), the forward coefficients
-// {m_hi, m_lo, w * invstd, b} and new_running [2][C] (mean, unbiased variance).  Eval: the running statistics.
+// Training: chunks of sum (x - K) and sum (x - K)^2 in order, K = x[0][c][0] -> save (mean, invstd), the forward
+// coefficients {m_hi, m_lo, w * invstd, b} and new_running [2][C] (mean, unbiased variance).  Eval: the running
+// statistics.
 __global__ void k_bn2d_stats_finish(const double* __restrict__ part, int nchunk, int C, long long n, int training,
+                                    const float* __restrict__ x, int HW,
                                     const float* __restrict__ w, const float* __restrict__ b, const float* __restrict__ rm,
                                     const float* __restrict__ rv, float momentum, float eps, double* __restrict__ save,
                                     float* __restrict__ coef, float* __restrict__ new_running) {
@@ -60,8 +65,10 @@ __global__ void k_bn2d_stats_finish(const double* __restrict__ part, int nchunk,
         double s1 = 0.0, s2 = 0.0;
         for (int j = 0; j < nchunk; ++j) s1 += part[(size_t)j * C + c];
         for (int j = 0; j < nchunk; ++j) s2 += part[((size_t)nchunk + j) * C + c];
-        mean = s1 / (double)n;
-        const double var = fmax(s2 / (double)n - mean * mean, 0.0);
+        const double d = s1 / (double)n;             // mean - K
+        mean = (double)x[(size_t)c * HW] + d;
+        const double v0 = s2 / (double)n - d * d;
+        const double var = v0 < 0.0 ? 0.0 : v0;       // rounding below 0 is clamped; NaN stays (fmax would drop it)
         invstd = 1.0 / sqrt(var + (double)eps);
         if (new_running) {
             const double m = (double)momentum;
@@ -109,6 +116,11 @@ __global__ void k_bn2d_eval_coef(int C, const float* __restrict__ w, const doubl
     k[4] = (float)((double)w[c] * save[C + c]);
 }
 
+// ReLU as torch's: NaN stays NaN.  Its backward passes dy except where y <= 0, so a NaN output passes dy as torch's
+// threshold_backward does (and a diverging step shows in every gradient it reaches).
+__device__ __forceinline__ float relu_fwd(float v) { return (v > 0.f || v != v) ? v : 0.f; }
+__device__ __forceinline__ float relu_mask(float y, float g) { return y <= 0.f ? 0.f : g; }
+
 // channel of flat element e of [N][C][HW]
 __device__ __forceinline__ int chan_of(long long e, int HW, int C) { return (int)((e / HW) % C); }
 
@@ -118,7 +130,7 @@ __device__ __forceinline__ float bn_fwd1(const FwdArgs& a, float x, float r, int
     const float4 k = __ldg(reinterpret_cast<const float4*>(a.coef + (size_t)c * kCoef));
     float v = ((x - k.x) - k.y) * k.z + k.w;
     if (a.r) v += r;
-    if (a.relu) v = fmaxf(v, 0.0f);
+    if (a.relu) v = relu_fwd(v);
     return v;
 }
 
@@ -153,7 +165,7 @@ struct BwdArgs {
 
 // dz, and dx when a.dx is set
 __device__ __forceinline__ float bn_bwd1(const BwdArgs& a, float dy, float y, float x, int c, float* dx) {
-    const float dz = (a.y && !(y > 0.0f)) ? 0.0f : dy;
+    const float dz = a.y ? relu_mask(y, dy) : dy;
     if (a.dx) {
         const float* k = a.coef + (size_t)c * kCoef;
         const float kk = __ldg(k + 4);
@@ -288,8 +300,6 @@ k_linear_bwd(int N, int In, int Out, long long ndx, long long ndw, long long ndb
 // ------------------------------------------------------------------------------------------------
 struct FuseArgs { const float* t[4]; int sh[4]; int n; };     // sh = log2 of the upsample factor
 
-__device__ __forceinline__ float relu_fwd(float v) { return (v > 0.f || v != v) ? v : 0.f; }     // torch: NaN stays
-
 // Forward: a thread writes V consecutive outputs of one row (V = 4: 16-byte stores, and 16-/8-byte loads of the
 // terms at factor 1 / 2).  The terms are added in list order, each sum rounded on its own, as the reference's
 // y = y + term chain.
@@ -332,10 +342,10 @@ k_hr_fuse_fwd(long long items, int H, int W, const FuseArgs a, int relu, float* 
     else o[0] = acc[0];
 }
 
-// dy masked by the ReLU: torch's rule on the output, no gradient where y <= 0 (an exact 0 sum included)
-__device__ __forceinline__ float relu_bwd(float g, const float* y, size_t e) { return (y && !(__ldg(y + e) > 0.f)) ? 0.f : g; }
+// dy masked by the ReLU on the output: no gradient where y <= 0 (an exact 0 sum included), dy where y > 0 or NaN
+__device__ __forceinline__ float relu_bwd(float g, const float* y, size_t e) { return y ? relu_mask(__ldg(y + e), g) : g; }
 
-// Backward of one term upsampled by F: a thread owns one element of dterm and sums dy * [y > 0] over its F x F block in
+// Backward of one term upsampled by F: a thread owns one element of dterm and sums relu_mask(y, dy) over its F x F block in
 // row-major order (fp32).  VEC: the block's rows are read as 8- (F = 2) or 16-byte (F = 4, 8) vectors.
 template <int F, bool VEC>
 __global__ void __launch_bounds__(kThreads)
@@ -352,20 +362,20 @@ k_hr_fuse_bwd(long long items, int Hj, int Wj, const float* __restrict__ dy, con
         const size_t e = (size_t)((nc * Hj + hj) * F + r) * W + (size_t)wj * F;
         if (VEC && F == 2) {
             const float2 g = __ldg(reinterpret_cast<const float2*>(dy + e));
-            float2 m = make_float2(1.f, 1.f);
-            if (y) { const float2 t = __ldg(reinterpret_cast<const float2*>(y + e)); m = make_float2(t.x > 0.f, t.y > 0.f); }
-            acc += m.x != 0.f ? g.x : 0.f;
-            acc += m.y != 0.f ? g.y : 0.f;
+            float2 t = make_float2(1.f, 1.f);
+            if (y) t = __ldg(reinterpret_cast<const float2*>(y + e));
+            acc += relu_mask(t.x, g.x);
+            acc += relu_mask(t.y, g.y);
         } else if (VEC && F >= 4) {
 #pragma unroll
             for (int q = 0; q < F; q += 4) {
                 const float4 g = __ldg(reinterpret_cast<const float4*>(dy + e + q));
                 float4 t = make_float4(1.f, 1.f, 1.f, 1.f);
                 if (y) t = __ldg(reinterpret_cast<const float4*>(y + e + q));
-                acc += t.x > 0.f ? g.x : 0.f;
-                acc += t.y > 0.f ? g.y : 0.f;
-                acc += t.z > 0.f ? g.z : 0.f;
-                acc += t.w > 0.f ? g.w : 0.f;
+                acc += relu_mask(t.x, g.x);
+                acc += relu_mask(t.y, g.y);
+                acc += relu_mask(t.z, g.z);
+                acc += relu_mask(t.w, g.w);
             }
         } else {
 #pragma unroll
@@ -375,7 +385,7 @@ k_hr_fuse_bwd(long long items, int Hj, int Wj, const float* __restrict__ dy, con
     dt[i] = acc;
 }
 
-// Backward of a term at factor 1: dterm = dy * [y > 0], 16-byte vectors when aligned
+// Backward of a term at factor 1: dterm = relu_mask(y, dy), 16-byte vectors when aligned
 __global__ void __launch_bounds__(kThreads)
 k_hr_fuse_bwd1(long long total, int vec, const float* __restrict__ dy, const float* __restrict__ y, float* __restrict__ dt) {
     const long long e = 4 * ((long long)blockIdx.x * kThreads + threadIdx.x);
@@ -385,7 +395,7 @@ k_hr_fuse_bwd1(long long total, int vec, const float* __restrict__ dy, const flo
         float4 o = g;
         if (y) {
             const float4 t = __ldg(reinterpret_cast<const float4*>(y + e));
-            o = make_float4(t.x > 0.f ? g.x : 0.f, t.y > 0.f ? g.y : 0.f, t.z > 0.f ? g.z : 0.f, t.w > 0.f ? g.w : 0.f);
+            o = make_float4(relu_mask(t.x, g.x), relu_mask(t.y, g.y), relu_mask(t.z, g.z), relu_mask(t.w, g.w));
         }
         *reinterpret_cast<float4*>(dt + e) = o;
         return;
@@ -423,11 +433,11 @@ extern "C" int danet_bn2d_forward(int32_t N, int32_t C, int32_t HW, const float*
     double* part = (double*)workspace;
     float* coef = (float*)((char*)workspace + bn::part_bytes(N, C, HW));
     if (training) {
-        const ChanSums s = {x, nullptr, x, nullptr};
+        const ChanSums s = {x, nullptr, x, nullptr, x};
         if (chan_sums_partial(s, true, N, C, HW, part, st) != 0) return -3;
     }
     bn::k_bn2d_stats_finish<<<cdiv(C, 128), 128, 0, st>>>(part, chan_sums_chunks(N, HW), C, (long long)N * HW, training,
-                                                          weight, bias, running_mean, running_var, momentum, eps, save, coef,
+                                                          x, HW, weight, bias, running_mean, running_var, momentum, eps, save, coef,
                                                           training ? new_running : nullptr);
     bn::FwdArgs a;
     a.x = x; a.r = residual; a.coef = coef; a.y = y; a.total = (long long)N * C * HW; a.HW = HW; a.C = C; a.relu = relu != 0;
@@ -451,7 +461,7 @@ extern "C" int danet_bn2d_backward(int32_t N, int32_t C, int32_t HW, const float
     const float* mask = relu ? y : nullptr;
     const bool sums = dweight || dbias || (dx && training);
     if (sums) {
-        const ChanSums s = {dy, mask, x, save};
+        const ChanSums s = {dy, mask, x, save, nullptr};
         if (chan_sums_partial(s, true, N, C, HW, part, st) != 0) return -3;
         bn::k_bn2d_grad_finish<<<cdiv(C, 128), 128, 0, st>>>(part, chan_sums_chunks(N, HW), C, (long long)N * HW, training,
                                                              weight, save, dweight, dbias, coef);

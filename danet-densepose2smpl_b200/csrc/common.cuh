@@ -160,10 +160,13 @@ static inline bool act_any(const danet_act* a) { return a && (a->f32 || a->hi); 
 // zeroed afterwards (words <= 256).  The packed conv weights' header and the dy scale of conv_wgrad.cu use it.
 int pow2_scale(const float* x, long long n, float* hdr, int words, cudaStream_t st);
 
-// Fixed-order per-channel sums of an fp32 NCHW tensor [N][C][HW] in double (conv_wgrad.cu, k_db_partial): sum 0 =
-// sum of a (counted only where mask > 0 when mask is given); with `two`, sum 1 = sum of a * (b - b_shift[c]) (b_shift
-// may be NULL).  part receives [two ? 2 : 1][chan_sums_chunks(N, HW)][C] chunk partials, to be added in chunk order.
-struct ChanSums { const float* a; const float* mask; const float* b; const double* b_shift; };
+// Fixed-order per-channel sums of an fp32 NCHW tensor [N][C][HW] in double (conv_wgrad.cu, k_db_partial): with u = a
+// (0 where mask <= 0 when mask is given; a NaN mask keeps a) minus K, sum 0 = sum of u; with `two`, sum 1 = sum of
+// u * (b - b_shift[c]).  K = k_src[c * HW] (element 0 of channel c, the first image's) when k_src is given, else 0;
+// with k_src and no b_shift, b is shifted by K too, so sum 1 = sum (a - K)^2 for b = a: the shift keeps the variance
+// sum from cancelling when |mean| >> std.  b_shift and k_src may be NULL.  part receives
+// [two ? 2 : 1][chan_sums_chunks(N, HW)][C] chunk partials, to be added in chunk order.
+struct ChanSums { const float* a; const float* mask; const float* b; const double* b_shift; const float* k_src; };
 int chan_sums_chunks(int N, int HW);
 int chan_sums_partial(const ChanSums& s, bool two, int N, int C, int HW, double* part, cudaStream_t st);
 

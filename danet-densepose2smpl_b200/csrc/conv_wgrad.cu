@@ -235,8 +235,10 @@ __global__ void k_wgrad_finish(const float* __restrict__ part, int nchunk, int w
 
 // Per-channel sums of an fp32 NCHW tensor [N][C][HW] (db here, BatchNorm's statistics and gradient sums in
 // bn_train.cu): block (channel c, image chunk j) sums its images' planes with a fixed thread assignment and a fixed
-// tree, in double; the finishing kernels add the chunks in order.  u = a (0 where mask <= 0 when a mask is given);
-// sum 0 = sum u, and with kTwo sum 1 = sum u * (b - b_shift[c]).  Sum k of chunk j lands at part[(k * nchunk + j) * C + c].
+// tree, in double; the finishing kernels add the chunks in order.  u = a (0 where mask <= 0 when a mask is given) - K;
+// sum 0 = sum u, and with kTwo sum 1 = sum u * (b - shift), shift = b_shift[c] or K (common.cuh, ChanSums).  Without
+// k_src, K = 0 and each term is the double of the fp32 value, so db's bits do not depend on the shift.  Sum k of
+// chunk j lands at part[(k * nchunk + j) * C + c].
 constexpr int kDbThreads = 256;
 constexpr int kDbElems = 16384;                  // elements of one channel per db partial (at least one image)
 static int db_images_per_chunk(int HW) { return HW >= kDbElems ? 1 : kDbElems / HW; }
@@ -246,15 +248,17 @@ k_db_partial(ChanSums s, int N, int C, int HW, int ipc, double* __restrict__ par
     __shared__ double red[kTwo ? 2 : 1][kDbThreads];
     const int c = blockIdx.x, j = blockIdx.y;
     const int n0 = j * ipc, n1 = min(N, n0 + ipc);
-    const double shift = kTwo && s.b_shift ? s.b_shift[c] : 0.0;
+    const double k = s.k_src ? (double)__ldg(s.k_src + (size_t)c * HW) : 0.0;
+    const double shift = kTwo && s.b_shift ? s.b_shift[c] : k;
     double acc = 0.0, acc2 = 0.0;
     for (int n = n0; n < n1; ++n) {
         const size_t off = ((size_t)n * C + c) * HW;
         for (int q = threadIdx.x; q < HW; q += kDbThreads) {
             float v = __ldg(s.a + off + q);
-            if (s.mask && !(__ldg(s.mask + off + q) > 0.0f)) v = 0.0f;
-            acc += (double)v;
-            if (kTwo) acc2 += (double)v * ((double)__ldg(s.b + off + q) - shift);
+            if (s.mask && __ldg(s.mask + off + q) <= 0.0f) v = 0.0f;
+            const double u = (double)v - k;
+            acc += u;
+            if (kTwo) acc2 += u * ((double)__ldg(s.b + off + q) - shift);
         }
     }
     red[0][threadIdx.x] = acc;
@@ -503,7 +507,7 @@ extern "C" int danet_conv_bias_grad(int32_t N, int32_t C, int32_t HW, const floa
     const int nchunk = chan_sums_chunks(N, HW);
     DANET_CHECK(nchunk < 65536, "danet_conv_bias_grad: too many images");
     cudaStream_t st = (cudaStream_t)stream;
-    const ChanSums s = {dy, nullptr, nullptr, nullptr};
+    const ChanSums s = {dy, nullptr, nullptr, nullptr, nullptr};
     if (chan_sums_partial(s, false, N, C, HW, (double*)workspace, st) != 0) return -3;
     wg::k_db_finish<<<cdiv(C, 128), 128, 0, st>>>((const double*)workspace, nchunk, C, db);
     DANET_LAUNCH_CHECK();

@@ -344,9 +344,10 @@ __global__ void k_global_avgpool(int N, int HW, int C, ActV x, float* __restrict
 
 __global__ void k_linear(int N, int In, int Out, const float* __restrict__ x, const float* __restrict__ w,
                          const float* __restrict__ b, const float* __restrict__ add, float* __restrict__ y) {
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= N * Out) return;
-    const int n = gw / Out, o = gw % Out;
+    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // one warp per output: 64-bit
+    const int lane = threadIdx.x & 31;
+    if (gw >= (long long)N * Out) return;
+    const int n = (int)(gw / Out), o = (int)(gw % Out);
     float s = 0.f;
     for (int i = lane; i < In; i += 32) s = fmaf(x[(size_t)n * In + i], w[(size_t)o * In + i], s);
     s = warp_sum(s);
@@ -666,7 +667,9 @@ extern "C" int danet_linear(int32_t N, int32_t In, int32_t Out, const float* x, 
     DANET_CHECK(N >= 0 && In > 0 && Out > 0, "danet_linear: bad sizes");
     if (N == 0) return 0;
     DANET_CHECK(x && w && y, "danet_linear: null pointer");
-    k_linear<<<cdiv(N * Out * 32, 256), 256, 0, (cudaStream_t)s>>>(N, In, Out, x, w, b, add, y);
+    const long long blocks = ((long long)N * Out + 7) / 8;            // 8 warps (outputs) per block
+    DANET_CHECK(blocks < (1LL << 31), "danet_linear: N=%d x Out=%d outputs are too many for one grid", N, Out);
+    k_linear<<<(unsigned)blocks, 256, 0, (cudaStream_t)s>>>(N, In, Out, x, w, b, add, y);
     DANET_LAUNCH_CHECK();
     return 0;
 }

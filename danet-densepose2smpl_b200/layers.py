@@ -14,7 +14,9 @@ biased batch variance over (N, H, W) and updates running_mean / running_var in p
 variance (the kernel writes the new statistics to a scratch tensor, copied in under no_grad, so the buffers' _version
 moves and DaNet.plan_for refolds).  num_batches_tracked belongs to the module and is left alone, as F.batch_norm does.
 Eval mode normalises with the running statistics and is still differentiable.  The keyword-only options fuse the
-ResNet forms: bn + relu (bn1, the stems), bn + residual + relu (bn2), bn alone (the downsample).
+ResNet forms: bn + relu (bn1, the stems), bn + residual + relu (bn2), bn alone (the downsample).  The batch statistics
+are sums of x - x[0, c, 0] in double, so the variance keeps its precision at any |mean| / std.  The ReLU is torch's:
+NaN stays NaN, and its backward passes dy except where the output is <= 0, so a NaN output passes dy.
 
 `max_pool2d` takes only kernel 3, stride 2, padding 1 (the SmplResNet stem pool).  Ties and NaN pick the window slot
 torch picks, and the backward is a gather, so results match torch's CUDA max_pool2d bit for bit.
@@ -306,7 +308,7 @@ def hr_fuse(terms, factors, relu=True):
     terms: 1 to 4 fp32 contiguous NCHW CUDA tensors [N, C, H / f, W / f] with t.H * f == H and t.W * f == W for one
     (H, W).  The terms are added in list order, the reference's `y = y + ...` order, so the forward is bit-identical
     to the fp32 sequence F.interpolate(t, scale_factor=f, mode='nearest') + ... + relu.  The backward of a term is
-    the sum of dy * [y > 0] over each f x f block in row-major order (torch's ReLU rule: an exact 0 gets no gradient),
+    the sum of dy over each f x f block, except where y <= 0 (an exact 0 gets no gradient, a NaN passes dy), in row-major order,
     in fp32: within (f^2 - 1) 2^-24 sum |dy| of the exact block sum."""
     where = "danet_b200.layers.hr_fuse"
     if not isinstance(terms, (list, tuple)) or not 1 <= len(terms) <= 4:

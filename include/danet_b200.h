@@ -359,8 +359,8 @@ int danet_linear_backward(int32_t N, int32_t In, int32_t Out, const float* x, co
 /* HRNet fuse (models/module/hr_module.py:161-179) in training: fp32 NCHW
  * y [N,C,H,W] = relu?(up(t_0) + up(t_1) + ...), term j [N,C,H/f_j,W/f_j] upsampled nearest by f_j in {1,2,4,8},
  * added in list order (bit-identical to the F.interpolate + add + relu chain).  terms / factors: host arrays of
- * nterms (1..4) entries.  The backward writes one term's gradient: dterm = the f x f block sums of dy * [y > 0]
- * (y NULL: no ReLU), row-major. */
+ * nterms (1..4) entries; the ReLU keeps NaN.  The backward writes one term's gradient: dterm = the f x f block sums
+ * of dy, 0 where y <= 0 (a NaN y passes dy; y NULL: no ReLU), row-major. */
 int danet_hr_fuse_forward(int32_t N, int32_t C, int32_t H, int32_t W, int32_t nterms, const float* const* terms,
                           const int32_t* factors, int32_t relu, float* y, danet_stream_t stream);
 int danet_hr_fuse_backward(int32_t N, int32_t C, int32_t H, int32_t W, int32_t factor, const float* dy, const float* y,
