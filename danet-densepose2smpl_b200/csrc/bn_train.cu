@@ -404,7 +404,6 @@ k_hr_fuse_bwd1(long long total, int vec, const float* __restrict__ dy, const flo
 }
 
 static unsigned grid_of(long long work) { return (unsigned)((work + kThreads - 1) / kThreads); }
-static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 }  // namespace bn
 }  // namespace danet
@@ -427,7 +426,7 @@ extern "C" int danet_bn2d_forward(int32_t N, int32_t C, int32_t HW, const float*
     DANET_CHECK(bn_shape_ok(N, C, HW), "danet_bn2d_forward: bad sizes N=%d C=%d HW=%d", N, C, HW);
     DANET_CHECK(x && y && weight && bias && running_mean && running_var && save,
                 "danet_bn2d_forward: x, y, weight, bias, running statistics and save must be non-null");
-    DANET_CHECK(workspace && ((uintptr_t)workspace & 15) == 0, "danet_bn2d_forward: workspace must be non-null and 16-byte aligned");
+    DANET_CHECK(workspace && aligned16(workspace), "danet_bn2d_forward: workspace must be non-null and 16-byte aligned");
     DANET_CHECK(!training || (long long)N * HW > 1, "danet_bn2d_forward: training needs more than one value per channel");
     cudaStream_t st = (cudaStream_t)stream;
     double* part = (double*)workspace;
@@ -441,7 +440,7 @@ extern "C" int danet_bn2d_forward(int32_t N, int32_t C, int32_t HW, const float*
                                                           training ? new_running : nullptr);
     bn::FwdArgs a;
     a.x = x; a.r = residual; a.coef = coef; a.y = y; a.total = (long long)N * C * HW; a.HW = HW; a.C = C; a.relu = relu != 0;
-    a.vec = bn::aligned16(x) && bn::aligned16(y) && (!residual || bn::aligned16(residual));
+    a.vec = aligned16(x) && aligned16(y) && (!residual || aligned16(residual));
     bn::k_bn2d_apply<<<bn::grid_of((a.total + 3) / 4), bn::kThreads, 0, st>>>(a);
     DANET_LAUNCH_CHECK();
     return 0;
@@ -453,7 +452,7 @@ extern "C" int danet_bn2d_backward(int32_t N, int32_t C, int32_t HW, const float
     DANET_CHECK(bn_shape_ok(N, C, HW), "danet_bn2d_backward: bad sizes N=%d C=%d HW=%d", N, C, HW);
     DANET_CHECK(x && dy && weight && save, "danet_bn2d_backward: x, dy, weight and save must be non-null");
     DANET_CHECK(!relu || y, "danet_bn2d_backward: relu needs the forward's output y");
-    DANET_CHECK(workspace && ((uintptr_t)workspace & 15) == 0, "danet_bn2d_backward: workspace must be non-null and 16-byte aligned");
+    DANET_CHECK(workspace && aligned16(workspace), "danet_bn2d_backward: workspace must be non-null and 16-byte aligned");
     DANET_CHECK(!training || (long long)N * HW > 1, "danet_bn2d_backward: training needs more than one value per channel");
     cudaStream_t st = (cudaStream_t)stream;
     double* part = (double*)workspace;
@@ -472,8 +471,8 @@ extern "C" int danet_bn2d_backward(int32_t N, int32_t C, int32_t HW, const float
         bn::BwdArgs a;
         a.dy = dy; a.y = mask; a.x = x; a.coef = coef; a.dx = dx; a.dres = dresidual;
         a.total = (long long)N * C * HW; a.HW = HW; a.C = C; a.training = training != 0;
-        a.vec = bn::aligned16(dy) && bn::aligned16(x) && (!mask || bn::aligned16(mask)) && (!dx || bn::aligned16(dx)) &&
-                (!dresidual || bn::aligned16(dresidual));
+        a.vec = aligned16(dy) && aligned16(x) && (!mask || aligned16(mask)) && (!dx || aligned16(dx)) &&
+                (!dresidual || aligned16(dresidual));
         bn::k_bn2d_bwd_apply<<<bn::grid_of((a.total + 3) / 4), bn::kThreads, 0, st>>>(a);
     }
     DANET_LAUNCH_CHECK();
@@ -519,7 +518,7 @@ extern "C" int danet_hr_fuse_forward(int32_t N, int32_t C, int32_t H, int32_t W,
     DANET_CHECK(terms && factors && y, "danet_hr_fuse_forward: terms, factors and y must be non-null");
     bn::FuseArgs a;
     a.n = nterms;
-    bool vec = (W % 4) == 0 && bn::aligned16(y);
+    bool vec = (W % 4) == 0 && aligned16(y);
     for (int j = 0; j < 4; ++j) {
         a.t[j] = nullptr; a.sh[j] = 0;
         if (j >= nterms) continue;
@@ -527,7 +526,7 @@ extern "C" int danet_hr_fuse_forward(int32_t N, int32_t C, int32_t H, int32_t W,
         DANET_CHECK(fuse_factor_ok(factors[j], H, W), "danet_hr_fuse_forward: factor %d of term %d must be 1, 2, 4 or 8 and "
                     "divide H=%d and W=%d", factors[j], j, H, W);
         a.t[j] = terms[j]; a.sh[j] = fuse_shift(factors[j]);
-        vec = vec && (a.sh[j] == 0 ? bn::aligned16(terms[j]) : a.sh[j] == 1 ? ((uintptr_t)terms[j] & 7) == 0 : true);
+        vec = vec && (a.sh[j] == 0 ? aligned16(terms[j]) : a.sh[j] == 1 ? ((uintptr_t)terms[j] & 7) == 0 : true);
     }
     const long long total = (long long)N * C * H * W;
     if (vec) bn::k_hr_fuse_fwd<4><<<bn::grid_of(total / 4), bn::kThreads, 0, (cudaStream_t)stream>>>(total / 4, H, W, a, relu, y);
@@ -545,9 +544,9 @@ extern "C" int danet_hr_fuse_backward(int32_t N, int32_t C, int32_t H, int32_t W
     cudaStream_t st = (cudaStream_t)stream;
     const int Hj = H / factor, Wj = W / factor;
     const long long items = (long long)N * C * Hj * Wj;
-    const bool vec = bn::aligned16(dy) && (!y || bn::aligned16(y));
+    const bool vec = aligned16(dy) && (!y || aligned16(y));
     switch (factor) {
-        case 1: bn::k_hr_fuse_bwd1<<<bn::grid_of((items + 3) / 4), bn::kThreads, 0, st>>>(items, vec && bn::aligned16(dterm), dy, y, dterm); break;
+        case 1: bn::k_hr_fuse_bwd1<<<bn::grid_of((items + 3) / 4), bn::kThreads, 0, st>>>(items, vec && aligned16(dterm), dy, y, dterm); break;
         case 2: if (vec) bn::k_hr_fuse_bwd<2, true><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
                 else bn::k_hr_fuse_bwd<2, false><<<bn::grid_of(items), bn::kThreads, 0, st>>>(items, Hj, Wj, dy, y, dterm);
                 break;

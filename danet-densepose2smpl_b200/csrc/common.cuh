@@ -33,6 +33,19 @@ void set_error(const char* fmt, ...);
 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t align_up(int64_t a, int64_t b) { return (a + b - 1) / b * b; }
+static inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// Hands out the regions of a caller's workspace in order, each 256-byte aligned.  On a null base it only counts, so one
+// layout serves an entry's *_workspace_bytes query and the entry itself, and the two cannot disagree.
+struct WsCarve {
+    char* base;
+    int64_t bytes = 0;
+    template <typename T> T* take(int64_t count) {
+        T* p = base ? (T*)(base + bytes) : nullptr;
+        bytes = align_up(bytes + count * (int64_t)sizeof(T), 256);
+        return p;
+    }
+};
 
 template <typename T>
 int upload(T** dptr, const T* host, size_t count) {
@@ -50,6 +63,35 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
+}
+
+struct V3 { float x, y, z; };
+__device__ __forceinline__ V3 v3(float x, float y, float z) { V3 r; r.x = x; r.y = y; r.z = z; return r; }
+__device__ __forceinline__ float dot3(V3 a, V3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+__device__ __forceinline__ V3 cross3(V3 a, V3 b) { return v3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x); }
+
+// rot6d_to_rotmat (utils/geometry.py:47-61): x viewed [3,2], a1 = x[:,0], a2 = x[:,1]; b1 = a1 / max(|a1|, 1e-12),
+// u = a2 - (b1 . a2) b1, b2 = u / max(|u|, 1e-12), b3 = b1 x b2; R has the columns (b1, b2, b3).  The SMPL front-end,
+// the inference pose head and the training head all run this one definition, so they agree to the last bit.  The state
+// keeps what the training head's backward needs: the raw norms n1r, n2r, the clamped n1, n2 and dd = b1 . a2.
+struct Rot6dState { V3 a1, a2, b1, u, b2; float n1r, n1, dd, n2r, n2; };
+__device__ __forceinline__ Rot6dState rot6d_state(const float* x) {
+    Rot6dState s;
+    s.a1 = v3(x[0], x[2], x[4]); s.a2 = v3(x[1], x[3], x[5]);
+    s.n1r = sqrtf(dot3(s.a1, s.a1)); s.n1 = fmaxf(s.n1r, 1e-12f);
+    s.b1 = v3(s.a1.x / s.n1, s.a1.y / s.n1, s.a1.z / s.n1);
+    s.dd = dot3(s.b1, s.a2);
+    s.u = v3(s.a2.x - s.dd * s.b1.x, s.a2.y - s.dd * s.b1.y, s.a2.z - s.dd * s.b1.z);
+    s.n2r = sqrtf(dot3(s.u, s.u)); s.n2 = fmaxf(s.n2r, 1e-12f);
+    s.b2 = v3(s.u.x / s.n2, s.u.y / s.n2, s.u.z / s.n2);
+    return s;
+}
+__device__ __forceinline__ void rot6d(const float* x, float* R) {
+    const Rot6dState s = rot6d_state(x);
+    const V3 b3 = cross3(s.b1, s.b2);
+    R[0] = s.b1.x; R[1] = s.b2.x; R[2] = b3.x;
+    R[3] = s.b1.y; R[4] = s.b2.y; R[5] = b3.y;
+    R[6] = s.b1.z; R[7] = s.b2.z; R[8] = b3.z;
 }
 
 // cudaFuncSetAttribute is per device: true the first time the calling thread's current device is seen by this

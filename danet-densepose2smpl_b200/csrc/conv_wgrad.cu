@@ -457,7 +457,7 @@ extern "C" int danet_conv_wgrad(const danet_conv_desc* d, int32_t cout_r, int32_
     DANET_CHECK(d && wg::make_geo(d, &g), "danet_conv_wgrad: shape not supported (k in {1,3,7}, pad k/2, stride 1|2, "
                                           "channels %% 8, N %% wsets == 0)");
     DANET_CHECK(cout_r >= 1 && cout_r <= d->Cout && cin_r >= 1 && cin_r <= d->Cin, "danet_conv_wgrad: bad real channel counts");
-    DANET_CHECK(workspace && ((uintptr_t)workspace & 15) == 0, "danet_conv_wgrad: workspace must be non-null and 16-byte aligned");
+    DANET_CHECK(workspace && aligned16(workspace), "danet_conv_wgrad: workspace must be non-null and 16-byte aligned");
     DANET_CHECK(dW && x && dy && x->hi && x->lo && dy->hi && dy->lo, "danet_conv_wgrad: needs dW and the hi and lo planes of x and dy");
     cudaStream_t st = (cudaStream_t)stream;
     int dev = 0;

@@ -1,6 +1,7 @@
 // Regressor head, training path: r2p_gcn -> refine_gcn (+ residual) -> p2r_gcn -> pose head + rot6d, with BatchNorm1d(24)
 // on batch statistics, the intermediate heads of training mode and the backward of all of it
-// (smpl_regressor.py:844-895, GCN.py:29-92, graph.py:232-261, geometry.py rot6d_to_rotmat).
+// (smpl_regressor.py:844-895, GCN.py:29-92, graph.py:232-261, geometry.py rot6d_to_rotmat).  rot6d and the state its
+// backward reads (Rot6dState) are common.cuh's, shared with the inference pose head and the SMPL front-end.
 //
 // One launch per stage over the whole batch: a GraphConv layer is A.X (k_adj_mul), (A.X).W + b (k_gemm), the per-node
 // batch statistics (k_bn_stats, one CTA per node: BatchNorm1d(24) normalises each node over B x F_out values, so no
@@ -287,25 +288,9 @@ __global__ void k_head_bwd_w(int B, int K, const float* __restrict__ X, const fl
     if (f == 0) db[jk] = sb;
 }
 
-struct V3 { float x, y, z; };
-__device__ __forceinline__ V3 v3(float x, float y, float z) { V3 r; r.x = x; r.y = y; r.z = z; return r; }
-__device__ __forceinline__ float dot3(V3 a, V3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-__device__ __forceinline__ V3 cross3(V3 a, V3 b) { return v3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x); }
 __device__ __forceinline__ V3 axpy3(float s, V3 a, V3 b) { return v3(fmaf(s, a.x, b.x), fmaf(s, a.y, b.y), fmaf(s, a.z, b.z)); }
 __device__ __forceinline__ V3 scale3(V3 a, float s) { return v3(a.x * s, a.y * s, a.z * s); }
 
-struct Rot6dState { V3 a1, a2, b1, u, b2; float n1r, n1, dd, n2r, n2; };
-__device__ __forceinline__ Rot6dState rot6d_state(const float* x) {
-    Rot6dState s;
-    s.a1 = v3(x[0], x[2], x[4]); s.a2 = v3(x[1], x[3], x[5]);
-    s.n1r = sqrtf(dot3(s.a1, s.a1)); s.n1 = fmaxf(s.n1r, 1e-12f);
-    s.b1 = v3(s.a1.x / s.n1, s.a1.y / s.n1, s.a1.z / s.n1);
-    s.dd = dot3(s.b1, s.a2);
-    s.u = v3(s.a2.x - s.dd * s.b1.x, s.a2.y - s.dd * s.b1.y, s.a2.z - s.dd * s.b1.z);
-    s.n2r = sqrtf(dot3(s.u, s.u)); s.n2 = fmaxf(s.n2r, 1e-12f);
-    s.b2 = v3(s.u.x / s.n2, s.u.y / s.n2, s.u.z / s.n2);
-    return s;
-}
 // F.normalize backward: v / max(|v|, 1e-12); the clamp's side passes g / eps
 __device__ __forceinline__ V3 normalize_bwd(float nraw, float n, V3 b, V3 g) {
     if (nraw > 1e-12f) return scale3(axpy3(-dot3(b, g), b, g), 1.f / n);
@@ -318,12 +303,11 @@ __global__ void k_rot6d_fwd(int B, const float* __restrict__ p6, float* __restri
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= B * 24) return;
     const int b = idx / 24, j = idx % 24;
-    const Rot6dState s = rot6d_state(p6 + (size_t)idx * 6);
-    const V3 b3 = cross3(s.b1, s.b2);
+    float R[9];
+    rot6d(p6 + (size_t)idx * 6, R);
     float* o = out + (size_t)b * stride + off + j * 9;
-    o[0] = s.b1.x; o[1] = s.b2.x; o[2] = b3.x;
-    o[3] = s.b1.y; o[4] = s.b2.y; o[5] = b3.y;
-    o[6] = s.b1.z; o[7] = s.b2.z; o[8] = b3.z;
+#pragma unroll
+    for (int e = 0; e < 9; ++e) o[e] = R[e];
     if (gpara && j < 13) out[(size_t)b * stride + j] = gpara[b * 13 + j];
 }
 
@@ -470,7 +454,7 @@ extern "C" int danet_gcn_head_train_forward(int32_t B, const danet_gcn_train_par
     GT_TRY(check_params(p, training, false));
     DANET_CHECK(rot_feats && global_para && para && workspace, "danet_gcn_head_train_forward: null pointer");
     DANET_CHECK(!training || (pose0 && coord0 && coord1), "danet_gcn_head_train_forward: training mode needs pose0 / coord0 / coord1");
-    DANET_CHECK(((uintptr_t)workspace & 15) == 0, "danet_gcn_head_train_forward: workspace must be 16-byte aligned");
+    DANET_CHECK(aligned16(workspace), "danet_gcn_head_train_forward: workspace must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     const Layout L = layout(B);
     float* w = (float*)workspace;
@@ -516,7 +500,7 @@ extern "C" int danet_gcn_head_train_backward(int32_t B, const danet_gcn_train_pa
     DANET_CHECK(rot_feats && g_para && g_rot_feats && g_global_para && workspace, "danet_gcn_head_train_backward: null pointer");
     DANET_CHECK(!training || (g_pose0 && g_coord0 && g_coord1),
                 "danet_gcn_head_train_backward: training mode needs g_pose0 / g_coord0 / g_coord1");
-    DANET_CHECK(((uintptr_t)workspace & 15) == 0, "danet_gcn_head_train_backward: workspace must be 16-byte aligned");
+    DANET_CHECK(aligned16(workspace), "danet_gcn_head_train_backward: workspace must be 16-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     const Layout L = layout(B);
     float* w = (float*)workspace;

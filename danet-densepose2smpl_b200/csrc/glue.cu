@@ -356,24 +356,11 @@ __global__ void k_linear(int N, int In, int Out, const float* __restrict__ x, co
 
 // ------------------------------------------------------------------------------------------
 // GCN refinement + pose head + rot6d (smpl_regressor.py:858-895,924; GCN.py:29-92)
-// One CTA (256 threads) per sample; thread o owns output column o of each GraphConv.
+// One CTA (256 threads) per sample; thread o owns output column o of each GraphConv.  rot6d is common.cuh's.
 // ------------------------------------------------------------------------------------------
 constexpr int kGcnThreads = 256;
 constexpr int kGcnMaxF = 256;
 constexpr int kGcnTF = 32;                 // input features per streamed weight tile
-
-__device__ __forceinline__ void rot6d_cols(const float* x, float* R) {
-    const float a1x = x[0], a1y = x[2], a1z = x[4], a2x = x[1], a2y = x[3], a2z = x[5];
-    const float n1 = fmaxf(sqrtf(a1x * a1x + a1y * a1y + a1z * a1z), 1e-12f);
-    const float b1x = a1x / n1, b1y = a1y / n1, b1z = a1z / n1;
-    const float d = b1x * a2x + b1y * a2y + b1z * a2z;
-    const float ux = a2x - d * b1x, uy = a2y - d * b1y, uz = a2z - d * b1z;
-    const float n2 = fmaxf(sqrtf(ux * ux + uy * uy + uz * uz), 1e-12f);
-    const float b2x = ux / n2, b2y = uy / n2, b2z = uz / n2;
-    R[0] = b1x; R[1] = b2x; R[2] = b1y * b2z - b1z * b2y;
-    R[3] = b1y; R[4] = b2y; R[5] = b1z * b2x - b1x * b2z;
-    R[6] = b1z; R[7] = b2z; R[8] = b1x * b2y - b1y * b2x;
-}
 
 __global__ void __launch_bounds__(kGcnThreads)
 k_gcn_pose_head(int B, GcnArgs g, const float* __restrict__ rot_feats, const float* __restrict__ global_para,
@@ -466,7 +453,7 @@ k_gcn_pose_head(int B, GcnArgs g, const float* __restrict__ rot_feats, const flo
     if (tid < 13) out[tid] = global_para[(size_t)b * 13 + tid];
     if (tid < 24) {
         float R[9];
-        rot6d_cols(s_p6 + tid * 6, R);
+        rot6d(s_p6 + tid * 6, R);
 #pragma unroll
         for (int e = 0; e < 9; ++e) out[13 + tid * 9 + e] = R[e];
     }
@@ -574,7 +561,7 @@ int danet::iuv_clean_global(int B, int HW, int Chead, int off_u, int off_v, int 
                 Chead, Cbody);
     if (B == 0) return 0;
     DANET_CHECK(heads && index_argmax, "danet_iuv_clean_global: null pointer");
-    DANET_CHECK(((uintptr_t)heads & 15) == 0, "danet_iuv_clean_global: heads must be 16-byte aligned");
+    DANET_CHECK(aligned16(heads), "danet_iuv_clean_global: heads must be 16-byte aligned");
     if (check_act(body_iuv, "danet_iuv_clean_global", 4) != 0) return -1;
     k_iuv_clean_global_staged<kPx><<<cdiv(B * HW, kPx), 128, smem, s>>>(
         B * HW, HW, Chead, off_u, off_v, off_i, off_a, Cbody, heads, actv(body_iuv), index_argmax, u_nchw, v_nchw, i_nchw, ann_nchw);
@@ -683,7 +670,7 @@ int danet::gcn_pose_head(int B, const GcnArgs& g, const float* rot_feats, const 
     for (int l = 0; l < 5; ++l) {
         DANET_CHECK(g.W[l] && g.b[l] && g.bn_s[l] && g.bn_t[l], "danet_gcn_pose_head: layer %d has null params", l);
         DANET_CHECK(g.din[l] > 0 && g.din[l] <= kGcnMaxF && g.dout[l] > 0 && g.dout[l] <= kGcnMaxF &&
-                    g.din[l] % 4 == 0 && g.dout[l] % 4 == 0 && ((uintptr_t)g.W[l] & 15) == 0,
+                    g.din[l] % 4 == 0 && g.dout[l] % 4 == 0 && aligned16(g.W[l]),
                     "danet_gcn_pose_head: layer %d dims %d->%d must be <= %d, multiples of 4, W 16-byte aligned", l, g.din[l], g.dout[l], kGcnMaxF);
     }
     DANET_CHECK(g.din[0] == 128 && g.dout[0] == 128 && g.dout[3] == 128 && g.din[4] == 128 && g.dout[4] == 128,

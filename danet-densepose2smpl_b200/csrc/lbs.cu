@@ -3,7 +3,7 @@
 // and the vertex-regressed joints (extra 9, H36M 17, 21 picked vertices) -> 49-joint output.
 //
 // Replaces models/smpl.py:15-46 + smplx.lbs (third-party, see oracle/lbs.py) and
-// utils/geometry.py:9-91.  Two routes:
+// utils/geometry.py:9-91; rot6d is common.cuh's, the one both pose heads use.  Two routes:
 //  * small batches (B < kGemmMinB): everything fp32 SIMT in one fused kernel (below);
 //  * large batches: the blend-shape + pose-corrective contraction  v_posed[B, 20670] = template +
 //    [pose_feature | betas][B, 224] x [posedirs ; shapedirs][224, 20670]  is a genuine GEMM (4.5 MMAC per body,
@@ -102,24 +102,6 @@ __device__ __forceinline__ void rodrigues_quat(const float* v, float* R) {
     R[0] = w2 + x2 - y2 - z2; R[1] = 2 * xy - 2 * wz;   R[2] = 2 * wy + 2 * xz;
     R[3] = 2 * wz + 2 * xy;   R[4] = w2 - x2 + y2 - z2; R[5] = 2 * yz - 2 * wx;
     R[6] = 2 * xz - 2 * wy;   R[7] = 2 * wx + 2 * yz;   R[8] = w2 - x2 - y2 + z2;
-}
-
-__device__ __forceinline__ void rot6d(const float* x, float* R) {
-    // utils/geometry.py:47-61: x viewed [3,2]; a1 = x[:,0], a2 = x[:,1]; columns (b1,b2,b3)
-    const float a1x = x[0], a1y = x[2], a1z = x[4];
-    const float a2x = x[1], a2y = x[3], a2z = x[5];
-    const float n1 = fmaxf(sqrtf(a1x * a1x + a1y * a1y + a1z * a1z), 1e-12f);
-    const float b1x = a1x / n1, b1y = a1y / n1, b1z = a1z / n1;
-    const float d = b1x * a2x + b1y * a2y + b1z * a2z;
-    const float ux = a2x - d * b1x, uy = a2y - d * b1y, uz = a2z - d * b1z;
-    const float n2 = fmaxf(sqrtf(ux * ux + uy * uy + uz * uz), 1e-12f);
-    const float b2x = ux / n2, b2y = uy / n2, b2z = uz / n2;
-    const float b3x = b1y * b2z - b1z * b2y;
-    const float b3y = b1z * b2x - b1x * b2z;
-    const float b3z = b1x * b2y - b1y * b2x;
-    R[0] = b1x; R[1] = b2x; R[2] = b3x;
-    R[3] = b1y; R[4] = b2y; R[5] = b3y;
-    R[6] = b1z; R[7] = b2z; R[8] = b3z;
 }
 
 __global__ void k_rot6d(int n, const float* __restrict__ x, float* __restrict__ R) {
@@ -812,6 +794,49 @@ static int up(danet_smpl* h, const T** dst, const std::vector<T>& src) {
     return 0;
 }
 
+// The forward's route and workspace (a null base only sizes it): skinning transforms, pose feature, posed joints,
+// regressor partials and, on the GEMM route, the split-fp16 feature planes and the fp32 v_posed of one chunk.
+struct SmplFwdWs {
+    bool gemm;
+    float *A, *pf, *posed, *partials, *vposed = nullptr;
+    __half *feat_hi = nullptr, *feat_lo = nullptr;
+    int64_t bytes;
+    SmplFwdWs(const danet_smpl* h, int B, int bodies_per_cta, void* base)
+        : gemm(B >= kGemmMinB && h->gemm_cout > 0 && bodies_per_cta >= 0) {
+        WsCarve c{(char*)base};
+        A = c.take<float>((int64_t)B * kJ * 12);
+        pf = c.take<float>((int64_t)B * kPF);
+        posed = c.take<float>((int64_t)B * kJ * 3);
+        partials = c.take<float>((int64_t)B * (h->v.npairs > 0 ? h->v.npairs : 1) * 3);
+        if (gemm) {
+            const int64_t Bp = align_up(B, 8);
+            feat_hi = c.take<__half>(Bp * kGF);
+            feat_lo = c.take<__half>(Bp * kGF);
+            vposed = c.take<float>((B < kGemmChunk ? Bp : kGemmChunk) * h->gemm_cout);
+        }
+        bytes = c.bytes;
+    }
+};
+
+// The backward's workspace (a null base only sizes it): world and skinning transforms, pose feature, posed joints,
+// dL/dv_posed, dL/dA, dL/dpose_feature and the per-tile partials of dL/dA.
+struct SmplBwdWs {
+    float *G, *A, *pf, *posed, *dvp, *dA, *dpf, *dA_tiles;
+    int64_t bytes;
+    SmplBwdWs(const danet_smpl* h, int B, void* base) {
+        WsCarve c{(char*)base};
+        G = c.take<float>((int64_t)B * kJ * 12);
+        A = c.take<float>((int64_t)B * kJ * 12);
+        pf = c.take<float>((int64_t)B * kPF);
+        posed = c.take<float>((int64_t)B * kJ * 3);
+        dvp = c.take<float>((int64_t)B * h->v.npad);
+        dA = c.take<float>((int64_t)B * kJ * 12);
+        dpf = c.take<float>((int64_t)B * kPF);
+        dA_tiles = c.take<float>((int64_t)B * h->v.ntiles * kJ * 12);
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace danet
 
 using namespace danet;
@@ -962,23 +987,9 @@ extern "C" int danet_smpl_destroy(danet_smpl_t h) {
     return 0;
 }
 
-static inline int64_t ws_off(int64_t& cur, int64_t bytes) { int64_t o = cur; cur = align_up(cur + bytes, 256); return o; }
-
 extern "C" int64_t danet_smpl_workspace_bytes(danet_smpl_t h, int32_t B) {
     if (!h || B <= 0) return 0;
-    int64_t cur = 0;
-    ws_off(cur, (int64_t)B * kJ * 12 * 4);          // G
-    ws_off(cur, (int64_t)B * kJ * 12 * 4);          // A
-    ws_off(cur, (int64_t)B * kPF * 4);              // pose feature
-    ws_off(cur, (int64_t)B * kJ * 3 * 4);           // posed joints
-    ws_off(cur, (int64_t)B * (h->v.npairs > 0 ? h->v.npairs : 1) * 3 * 4);  // regressor partials
-    if (B >= kGemmMinB && h->gemm_cout > 0) {
-        const int64_t Bp = align_up(B, 8);
-        ws_off(cur, Bp * kGF * 2);                  // feature plane hi
-        ws_off(cur, Bp * kGF * 2);                  // feature plane lo
-        ws_off(cur, (int64_t)(B < kGemmChunk ? Bp : kGemmChunk) * h->gemm_cout * 4);   // fp32 v_posed of one chunk
-    }
-    return cur;
+    return SmplFwdWs(h, B, 0, nullptr).bytes;
 }
 
 extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas, const float* pose,
@@ -993,24 +1004,8 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
                 "danet_smpl_forward: joint outputs need the verts buffer (picked vertices are read from it)");
     cudaStream_t stream = (cudaStream_t)stream_;
     const SmplView& m = h->v;
-    char* ws = (char*)workspace;
-    int64_t cur = 0;
-    float* G = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 12 * 4));
-    float* A = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 12 * 4));
-    float* pf = (float*)(ws + ws_off(cur, (int64_t)B * kPF * 4));
-    float* posed = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 3 * 4));
-    float* partials = (float*)(ws + ws_off(cur, (int64_t)B * (m.npairs > 0 ? m.npairs : 1) * 3 * 4));
-
-    const bool gemm = B >= kGemmMinB && h->gemm_cout > 0 && bodies_per_cta >= 0;
-    __half* feat_hi = nullptr; __half* feat_lo = nullptr; float* vposed = nullptr;
-    if (gemm) {
-        const int64_t Bp = align_up(B, 8);
-        feat_hi = (__half*)(ws + ws_off(cur, Bp * kGF * 2));
-        feat_lo = (__half*)(ws + ws_off(cur, Bp * kGF * 2));
-        vposed = (float*)(ws + ws_off(cur, (int64_t)(B < kGemmChunk ? Bp : kGemmChunk) * h->gemm_cout * 4));
-    }
-    k_smpl_pose<<<cdiv(B, kPoseWarps), kPoseWarps * 32, 0, stream>>>(B, pose_kind, betas, pose, m, rotmats, nullptr, A, pf, posed, feat_hi, feat_lo);
-    (void)G;
+    const SmplFwdWs ws(h, B, bodies_per_cta, workspace);
+    k_smpl_pose<<<cdiv(B, kPoseWarps), kPoseWarps * 32, 0, stream>>>(B, pose_kind, betas, pose, m, rotmats, nullptr, ws.A, ws.pf, ws.posed, ws.feat_hi, ws.feat_lo);
     DANET_LAUNCH_CHECK();
     int nb = bodies_per_cta;
     if (nb <= 0) nb = B >= 32 ? 8 : (B >= 4 ? 4 : (B >= 2 ? 2 : 1));      // tools/lbs_sweep.py sweeps it
@@ -1023,11 +1018,11 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
                                             (int)((size_t)NBV * (kPF + kJ * 12 + kTileC + kMaxBetas) * sizeof(float)))); \
         }                                                                                           \
         dim3 grid(m.ntiles, cdiv(Bc, NBV));                                                         \
-        k_smpl_verts<NBV><<<grid, kTileV, smem, stream>>>(Bc, betas + (size_t)(off) * m.nbetas, pf + (size_t)(off) * kPF, \
-            A + (size_t)(off) * kJ * 12, m, verts ? verts + (size_t)(off) * m.nv * 3 : nullptr,   \
-            partials + (size_t)(off) * (m.npairs > 0 ? m.npairs : 1) * 3, VP, h->gemm_cout);       \
+        k_smpl_verts<NBV><<<grid, kTileV, smem, stream>>>(Bc, betas + (size_t)(off) * m.nbetas, ws.pf + (size_t)(off) * kPF, \
+            ws.A + (size_t)(off) * kJ * 12, m, verts ? verts + (size_t)(off) * m.nv * 3 : nullptr, \
+            ws.partials + (size_t)(off) * (m.npairs > 0 ? m.npairs : 1) * 3, VP, h->gemm_cout);       \
     } while (0)
-    if (gemm) {
+    if (ws.gemm) {
         // tensor-core route: per chunk, one 1x1 "convolution" over the bodies (exact mode) + the skinning phases
         for (int off = 0; off < B; off += kGemmChunk) {
             const int Bc = B - off < kGemmChunk ? B - off : kGemmChunk;
@@ -1035,18 +1030,18 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
             memset(&pr, 0, sizeof(pr));
             pr.d.N = 1; pr.d.H = cdiv(Bc, 8); pr.d.W = 8; pr.d.Cin = kGF; pr.d.Cout = h->gemm_cout; pr.d.ksize = 1; pr.d.stride = 1;
             pr.d.pad = 0; pr.d.wsets = 1; pr.d.relu = 0; pr.d.flags = DANET_CONV_EXACT;
-            pr.x.hi = feat_hi + (size_t)off * kGF; pr.x.lo = feat_lo + (size_t)off * kGF;
-            pr.y.f32 = vposed; pr.w_packed = h->gemm_w; pr.bias = h->gemm_bias;
+            pr.x.hi = ws.feat_hi + (size_t)off * kGF; pr.x.lo = ws.feat_lo + (size_t)off * kGF;
+            pr.y.f32 = ws.vposed; pr.w_packed = h->gemm_w; pr.bias = h->gemm_bias;
             if (conv_tc_group_launch(1, &pr, stream) != 0) return -1;
             constexpr int kSkinTL = 3;                                  // vertex tiles per CTA of the skinning pass
             if (m.skin_packed && m.ntiles % kSkinTL == 0) {
                 dim3 grid(m.ntiles / kSkinTL, cdiv(Bc, 8));
                 const size_t sm = (size_t)8 * (kJ * 12 + 2 * kTileC) * sizeof(float);
-                k_smpl_skin<8, kSkinTL><<<grid, kTileV, sm, stream>>>(Bc, A + (size_t)off * kJ * 12, m,
-                    verts ? verts + (size_t)off * m.nv * 3 : nullptr, partials + (size_t)off * (m.npairs > 0 ? m.npairs : 1) * 3,
-                    vposed, h->gemm_cout);
+                k_smpl_skin<8, kSkinTL><<<grid, kTileV, sm, stream>>>(Bc, ws.A + (size_t)off * kJ * 12, m,
+                    verts ? verts + (size_t)off * m.nv * 3 : nullptr, ws.partials + (size_t)off * (m.npairs > 0 ? m.npairs : 1) * 3,
+                    ws.vposed, h->gemm_cout);
             } else {
-                DANET_LBS_LAUNCH(8, Bc, off, vposed);
+                DANET_LBS_LAUNCH(8, Bc, off, ws.vposed);
             }
             DANET_LAUNCH_CHECK();
         }
@@ -1064,7 +1059,7 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
 #undef DANET_LBS_LAUNCH
     if (joints || smpl_joints || joints_h36m) {
         const int ncat = kJ + m.nsel + m.nrows;
-        k_smpl_joints<<<B, 192, ncat * 3 * sizeof(float), stream>>>(B, m, posed, verts, partials, joints,
+        k_smpl_joints<<<B, 192, ncat * 3 * sizeof(float), stream>>>(B, m, ws.posed, verts, ws.partials, joints,
                                                                     smpl_joints, joints_h36m);
         DANET_LAUNCH_CHECK();
     }
@@ -1073,16 +1068,7 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
 
 extern "C" int64_t danet_smpl_backward_workspace_bytes(danet_smpl_t h, int32_t B) {
     if (!h || B <= 0) return 0;
-    int64_t cur = 0;
-    ws_off(cur, (int64_t)B * kJ * 12 * 4);          // G
-    ws_off(cur, (int64_t)B * kJ * 12 * 4);          // A
-    ws_off(cur, (int64_t)B * kPF * 4);              // pose feature
-    ws_off(cur, (int64_t)B * kJ * 3 * 4);           // posed joints
-    ws_off(cur, (int64_t)B * h->v.npad * 4);        // dL/dv_posed
-    ws_off(cur, (int64_t)B * kJ * 12 * 4);          // dL/dA
-    ws_off(cur, (int64_t)B * kPF * 4);              // dL/dpose_feature
-    ws_off(cur, (int64_t)B * h->v.ntiles * kJ * 12 * 4);   // per-tile partials of dL/dA
-    return cur;
+    return SmplBwdWs(h, B, nullptr).bytes;
 }
 
 extern "C" int danet_smpl_backward(danet_smpl_t h, int32_t B, const float* betas, const float* rotmats,
@@ -1093,26 +1079,17 @@ extern "C" int danet_smpl_backward(danet_smpl_t h, int32_t B, const float* betas
     DANET_CHECK(betas && rotmats && grad_verts && grad_betas && grad_rotmats && workspace, "danet_smpl_backward: null pointer");
     cudaStream_t stream = (cudaStream_t)stream_;
     const SmplView& m = h->v;
-    char* ws = (char*)workspace;
-    int64_t cur = 0;
-    float* G = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 12 * 4));
-    float* A = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 12 * 4));
-    float* pf = (float*)(ws + ws_off(cur, (int64_t)B * kPF * 4));
-    float* posed = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 3 * 4));
-    float* dvp = (float*)(ws + ws_off(cur, (int64_t)B * m.npad * 4));
-    float* dA = (float*)(ws + ws_off(cur, (int64_t)B * kJ * 12 * 4));
-    float* dpf = (float*)(ws + ws_off(cur, (int64_t)B * kPF * 4));
-    float* dA_tiles = (float*)(ws + ws_off(cur, (int64_t)B * m.ntiles * kJ * 12 * 4));
-    k_smpl_pose<<<cdiv(B, kPoseWarps), kPoseWarps * 32, 0, stream>>>(B, DANET_POSE_ROTMAT, betas, rotmats, m, nullptr, G, A, pf, posed, nullptr, nullptr);
+    const SmplBwdWs ws(h, B, workspace);
+    k_smpl_pose<<<cdiv(B, kPoseWarps), kPoseWarps * 32, 0, stream>>>(B, DANET_POSE_ROTMAT, betas, rotmats, m, nullptr, ws.G, ws.A, ws.pf, ws.posed, nullptr, nullptr);
     DANET_LAUNCH_CHECK();
-    k_lbs_bwd_verts<<<dim3(m.ntiles, B), kTileV, 0, stream>>>(B, betas, pf, A, m, grad_verts, dvp, dA_tiles);
+    k_lbs_bwd_verts<<<dim3(m.ntiles, B), kTileV, 0, stream>>>(B, betas, ws.pf, ws.A, m, grad_verts, ws.dvp, ws.dA_tiles);
     DANET_LAUNCH_CHECK();
-    k_lbs_bwd_dA<<<cdiv(B * kJ * 12, 256), 256, 0, stream>>>(B, m.ntiles, dA_tiles, dA);
+    k_lbs_bwd_dA<<<cdiv(B * kJ * 12, 256), 256, 0, stream>>>(B, m.ntiles, ws.dA_tiles, ws.dA);
     DANET_LAUNCH_CHECK();
     const int nrow = 207 + m.nbetas;
-    k_lbs_bwd_blend<<<cdiv((int64_t)B * nrow * 32, 256), 256, 0, stream>>>(B, m, dvp, dpf, grad_betas);
+    k_lbs_bwd_blend<<<cdiv((int64_t)B * nrow * 32, 256), 256, 0, stream>>>(B, m, ws.dvp, ws.dpf, grad_betas);
     DANET_LAUNCH_CHECK();
-    k_lbs_bwd_chain<<<cdiv(B, 32), 32, 0, stream>>>(B, m, betas, rotmats, G, dA, dpf, grad_smpl_joints, grad_betas, grad_rotmats);
+    k_lbs_bwd_chain<<<cdiv(B, 32), 32, 0, stream>>>(B, m, betas, rotmats, ws.G, ws.dA, ws.dpf, grad_smpl_joints, grad_betas, grad_rotmats);
     DANET_LAUNCH_CHECK();
     return 0;
 }

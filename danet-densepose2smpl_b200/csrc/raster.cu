@@ -187,6 +187,17 @@ __global__ void k_img2map(int B, int HW, const float* __restrict__ img, float* m
               img[((size_t)b * 3 + 2) * HW + pix], b, pix, HW, mu, mv, mi, ma);
 }
 
+// the rasteriser's workspace: projected mesh vertices, then the z-buffer keys; a null base only sizes it
+struct RasterWs {
+    float* pv; unsigned long long* zbuf; int64_t bytes;
+    RasterWs(const danet_raster* h, int B, void* base) {
+        WsCarve c{(char*)base};
+        pv = c.take<float>((int64_t)B * h->nmv * 3);
+        zbuf = c.take<unsigned long long>((int64_t)B * h->S * h->S);
+        bytes = c.bytes;
+    }
+};
+
 }  // namespace danet
 
 using namespace danet;
@@ -223,7 +234,7 @@ extern "C" int danet_raster_destroy(danet_raster_t h) {
 
 extern "C" int64_t danet_raster_workspace_bytes(danet_raster_t h, int32_t B) {
     if (!h || B <= 0) return 0;
-    return align_up((int64_t)B * h->nmv * 3 * 4, 256) + align_up((int64_t)B * h->S * h->S * 8, 256);
+    return RasterWs(h, B, nullptr).bytes;
 }
 
 extern "C" int danet_raster_iuv(danet_raster_t h, int32_t B, const float* verts, const float* cam, float* img,
@@ -233,14 +244,13 @@ extern "C" int danet_raster_iuv(danet_raster_t h, int32_t B, const float* verts,
     DANET_CHECK(B > 0, "danet_raster_iuv: empty batch (B=%d)", B);
     DANET_CHECK(verts && cam && workspace, "danet_raster_iuv: null input/workspace pointer");
     cudaStream_t stream = (cudaStream_t)stream_;
-    float* pv = (float*)workspace;
-    unsigned long long* zbuf = (unsigned long long*)((char*)workspace + align_up((int64_t)B * h->nmv * 3 * 4, 256));
-    DANET_CUDA(cudaMemsetAsync(zbuf, 0xff, (size_t)B * h->S * h->S * 8, stream));
-    k_project<<<cdiv(B * h->nmv, 256), 256, 0, stream>>>(B, h->nv, h->nmv, verts, cam, h->vmap, h->focal, h->orig, pv);
+    const RasterWs ws(h, B, workspace);
+    DANET_CUDA(cudaMemsetAsync(ws.zbuf, 0xff, (size_t)B * h->S * h->S * 8, stream));
+    k_project<<<cdiv(B * h->nmv, 256), 256, 0, stream>>>(B, h->nv, h->nmv, verts, cam, h->vmap, h->focal, h->orig, ws.pv);
     DANET_LAUNCH_CHECK();
-    k_faces<<<cdiv(B * h->nf, 128), 128, 0, stream>>>(B, h->nmv, h->nf, h->S, h->near_, h->far_, pv, h->faces, zbuf);
+    k_faces<<<cdiv(B * h->nf, 128), 128, 0, stream>>>(B, h->nmv, h->nf, h->S, h->near_, h->far_, ws.pv, h->faces, ws.zbuf);
     DANET_LAUNCH_CHECK();
-    k_resolve<<<cdiv(B * h->S * h->S, 256), 256, 0, stream>>>(B, h->S, h->nf, h->tex_mode, zbuf, h->tex, img, face_idx,
+    k_resolve<<<cdiv(B * h->S * h->S, 256), 256, 0, stream>>>(B, h->S, h->nf, h->tex_mode, ws.zbuf, h->tex, img, face_idx,
                                                             maps_u, maps_v, maps_i, maps_ann);
     DANET_LAUNCH_CHECK();
     return 0;

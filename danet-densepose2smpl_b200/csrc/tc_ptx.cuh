@@ -129,7 +129,7 @@ static int encode_nhwc_f16(CUtensorMap* tm, const void* base, int N, int H, int 
                            CUtensorMapSwizzle sw, int stride) {
     PFN_encodeTiled fn = encode_fn();
     DANET_CHECK(fn, "cuTensorMapEncodeTiled is not available from this driver");
-    DANET_CHECK(base && ((uintptr_t)base & 15) == 0, "tensor map: activation planes must be non-null and 16-byte aligned");
+    DANET_CHECK(base && aligned16(base), "tensor map: activation planes must be non-null and 16-byte aligned");
     cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
     cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)(stride * (box_w - 1) + 1), (cuuint32_t)(stride * (box_h - 1) + 1), 1u};
