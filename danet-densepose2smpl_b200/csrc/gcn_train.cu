@@ -36,12 +36,17 @@ __device__ __forceinline__ float bn_z(float y, float mean, float invstd, float g
     return (y - mean) * invstd * g + b;
 }
 
+// The ReLU keeps NaN (fmaxf would return 0 for it), and its backward passes dy except where the input is <= 0, so a NaN
+// passes dy: torch's relu and threshold_backward, and bn_train.cu's policy.
+__device__ __forceinline__ float relu_keep_nan(float v) { return v <= 0.f ? 0.f : v; }
+__device__ __forceinline__ bool relu_passes(float v) { return !(v <= 0.f); }
+
 // ---- normalize_undigraph(I_n + A_mask * relu(E)) (graph.py:232-261): one CTA of 576 threads -----------------------
 __global__ void k_adj_fwd(const float* __restrict__ I_n, const float* __restrict__ A_mask, const float* __restrict__ E,
                           float* __restrict__ Mout, float* __restrict__ Ahat, float* __restrict__ dout) {
     __shared__ float sM[576], sd[24];
     const int t = threadIdx.x;
-    sM[t] = I_n[t] + A_mask[t] * fmaxf(E[t], 0.f);
+    sM[t] = I_n[t] + A_mask[t] * relu_keep_nan(E[t]);
     __syncthreads();
     if (t < 24) {
         float s = 0.f;
@@ -70,12 +75,12 @@ __global__ void k_adj_bwd(const float* __restrict__ dApart, const float* __restr
     __syncthreads();
     const int i = t / 24, j = t % 24;
     const float dM = sG[t] * d[i] * d[j] + sgs[j];
-    gE[t] = E[t] > 0.f ? dM * A_mask[t] : 0.f;
+    gE[t] = relu_passes(E[t]) ? dM * A_mask[t] : 0.f;
 }
 
-// Y[b,n,f] (+)= sum_k A'[n,k] X[b,k,f], A' = A or A^T
+// Y[b,n,f] = (add[b,n,f] +) sum_k A'[n,k] X[b,k,f], A' = A or A^T; add may be Y itself
 __global__ void k_adj_mul(int B, int F, const float* __restrict__ A, int transpose, const float* __restrict__ X,
-                          float* __restrict__ Y, int accumulate) {
+                          const float* add, float* Y) {
     __shared__ float sA[576];
     for (int i = threadIdx.x; i < 576; i += blockDim.x) sA[i] = transpose ? A[(i % 24) * 24 + i / 24] : A[i];
     __syncthreads();
@@ -86,7 +91,7 @@ __global__ void k_adj_mul(int B, int F, const float* __restrict__ A, int transpo
     float s = 0.f;
 #pragma unroll
     for (int k = 0; k < 24; ++k) s = fmaf(sA[n * 24 + k], x[k * F], s);
-    Y[idx] = accumulate ? Y[idx] + s : s;
+    Y[idx] = add ? add[idx] + s : s;
 }
 
 // C[M,N] = sum_k A(m,k) B(k,n) (+ bias[n]); A(m,k) = A[m*sam + k*sak], B(k,n) = B[k*sbk + n*sbn].  64 x 64 tiles,
@@ -141,8 +146,11 @@ __global__ void __launch_bounds__(kT) k_gemm(int M, int N, int K, const float* _
     }
 }
 
-// per-node statistics of Y [B,24,F] (one CTA per node): training -> batch mean / biased variance (two passes) and the
-// updated running statistics; eval -> the running statistics
+// per-node statistics of Y [B,24,F] (one CTA per node): training -> batch mean / biased variance and the updated running
+// statistics; eval -> the running statistics.  Both passes sum y - K with K = Y[0,n,0], a data element (as bn_train.cu
+// does): the shifted mean dm = sum (y - K) / N is then off by a few units of the spread, not of |mean|, and the
+// variance sum ((y - K) - dm)^2 / N keeps its digits when |mean| >> std.  An infinite first element would make every
+// y - K NaN, so K is 0 then: the mean is infinite, as torch's is, and the running mean shows it.
 __global__ void __launch_bounds__(kT) k_bn_stats(int B, int F, const float* __restrict__ Y, int training,
                                                  const float* __restrict__ rm, const float* __restrict__ rv,
                                                  float* __restrict__ mean_out, float* __restrict__ invstd_out,
@@ -153,12 +161,15 @@ __global__ void __launch_bounds__(kT) k_bn_stats(int B, int F, const float* __re
         if (threadIdx.x == 0) { mean_out[n] = rm[n]; invstd_out[n] = 1.f / sqrtf(rv[n] + kBnEps); }
         return;
     }
+    const float y0 = Y[(size_t)n * F];
+    const float K = isfinite(y0) ? y0 : 0.f;
     float s = 0.f;
-    for (int i = threadIdx.x; i < N; i += kT) s += Y[((size_t)(i / F) * 24 + n) * F + i % F];
-    const float mean = block_sum(s, red) / (float)N;
+    for (int i = threadIdx.x; i < N; i += kT) s += Y[((size_t)(i / F) * 24 + n) * F + i % F] - K;
+    const float dm = block_sum(s, red) / (float)N;
+    const float mean = K + dm;
     float q = 0.f;
     for (int i = threadIdx.x; i < N; i += kT) {
-        const float d = Y[((size_t)(i / F) * 24 + n) * F + i % F] - mean;
+        const float d = (Y[((size_t)(i / F) * 24 + n) * F + i % F] - K) - dm;
         q = fmaf(d, d, q);
     }
     const float var = block_sum(q, red) / (float)N;
@@ -178,7 +189,7 @@ __global__ void k_bn_act(int B, int F, const float* __restrict__ Y, const float*
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= B * 24 * F) return;
     const int n = (idx / F) % 24;
-    float v = fmaxf(bn_z(Y[idx], mean[n], invstd[n], g[n], beta[n]), 0.f);
+    float v = relu_keep_nan(bn_z(Y[idx], mean[n], invstd[n], g[n], beta[n]));
     if (res) v += res[idx];                                    // l_pos_feat = pos_feats_init + refine (smpl_regressor.py:873)
     H[idx] = v;
 }
@@ -197,7 +208,7 @@ __global__ void __launch_bounds__(kT) k_bn_bwd_reduce(int B, int F, const float*
     for (int i = threadIdx.x; i < N; i += kT) {
         const size_t e = ((size_t)(i / F) * 24 + n) * F + i % F;
         const float y = Y[e];
-        const float dz = bn_z(y, mu, is, ga, be) > 0.f ? dH[e] : 0.f;
+        const float dz = relu_passes(bn_z(y, mu, is, ga, be)) ? dH[e] : 0.f;
         s1 += dz;
         s2 = fmaf(dz, (y - mu) * is, s2);
     }
@@ -216,7 +227,7 @@ __global__ void k_bn_bwd_dy(int B, int F, int training, const float* __restrict_
     if (idx >= B * 24 * F) return;
     const int n = (idx / F) % 24;
     const float y = Y[idx], mu = mean[n], is = invstd[n];
-    const float dxh = bn_z(y, mu, is, g[n], beta[n]) > 0.f ? dH[idx] * g[n] : 0.f;
+    const float dxh = relu_passes(bn_z(y, mu, is, g[n], beta[n])) ? dH[idx] * g[n] : 0.f;
     if (training) {
         const float Nf = (float)(B * F);
         dY[idx] = is / Nf * (Nf * dxh - sums[2 * n] - (y - mu) * is * sums[2 * n + 1]);
@@ -261,15 +272,15 @@ __global__ void k_group_head(int B, int K, const float* __restrict__ X, const fl
     out[idx] = s + bias[jk] + (add ? add[jk] : 0.f);
 }
 
-// head backward, input half: dX[b,j,f] (+)= sum_k W[j*K+k, f] dp[b, j*K+k]
+// head backward, input half: dX[b,j,f] = (add[b,j,f] +) sum_k W[j*K+k, f] dp[b, j*K+k]; add may be dX itself
 __global__ void k_head_bwd_x(int B, int K, const float* __restrict__ W, const float* __restrict__ dp,
-                             float* __restrict__ dX, int accumulate) {
+                             const float* add, float* dX) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= B * 24 * 128) return;
     const int f = idx % 128, j = (idx / 128) % 24, b = idx / (24 * 128);
     float s = 0.f;
     for (int k = 0; k < K; ++k) s = fmaf(W[(size_t)(j * K + k) * 128 + f], dp[(size_t)b * 24 * K + j * K + k], s);
-    dX[idx] = accumulate ? dX[idx] + s : s;
+    dX[idx] = add ? add[idx] + s : s;
 }
 
 // head backward, parameter half: dW[jk, f] = sum_b dp[b,jk] X[b,j,f]; db[jk] = sum_b dp[b,jk]
@@ -369,8 +380,11 @@ __global__ void __launch_bounds__(kT) k_head_losses(int B, const float* __restri
 }
 
 // ---- workspace layout (floats, every region 256-byte aligned) -----------------------------------------------------
+// The forward's saved activations, then one region per backward intermediate: gH[l] the full gradient of H[l] (the
+// residual's and the coord heads' shares included), dY[l] the gradient of the GraphConv output, dAX[l] that of A X.
+// tests/gcn_head_sweep_common.py mirrors this layout and reads every region.
 struct Layout {
-    size_t M, Ahat, d, AX[5], Y[5], H[5], mean[5], invstd[5], p6[2], dp6[2], P[3], dY, dAX, dA, sums, total;
+    size_t M, Ahat, d, AX[5], Y[5], H[5], mean[5], invstd[5], p6[2], dp6[2], gH[5], dY[5], dAX[5], dA, sums, total;
 };
 Layout layout(int B) {
     Layout L;
@@ -383,8 +397,8 @@ Layout layout(int B) {
         L.mean[l] = take(24); L.invstd[l] = take(24);
     }
     for (int k = 0; k < 2; ++k) { L.p6[k] = take((size_t)B * 144); L.dp6[k] = take((size_t)B * 144); }
-    for (int k = 0; k < 3; ++k) L.P[k] = take(R * 256);
-    L.dY = take(R * 256); L.dAX = take(R * 256); L.dA = take(3 * 576); L.sums = take(48);
+    for (int l = 0; l < 5; ++l) { L.gH[l] = take(R * kDO[l]); L.dY[l] = take(R * kDO[l]); L.dAX[l] = take(R * kDI[l]); }
+    L.dA = take(3 * 576); L.sums = take(48);
     L.total = o;
     return L;
 }
@@ -396,8 +410,8 @@ int gemm(cudaStream_t st, int M, int N, int K, const float* A, int sam, int sak,
     return 0;
 }
 
-int adj_mul(cudaStream_t st, int B, int F, const float* A, int transpose, const float* X, float* Y, int acc) {
-    k_adj_mul<<<cdiv(B * 24 * F, kT), kT, 0, st>>>(B, F, A, transpose, X, Y, acc);
+int adj_mul(cudaStream_t st, int B, int F, const float* A, int transpose, const float* X, const float* add, float* Y) {
+    k_adj_mul<<<cdiv(B * 24 * F, kT), kT, 0, st>>>(B, F, A, transpose, X, add, Y);
     DANET_LAUNCH_CHECK();
     return 0;
 }
@@ -409,13 +423,18 @@ int head_fwd(cudaStream_t st, int B, int K, const float* X, const float* W, cons
 }
 
 int head_bwd(cudaStream_t st, int B, int K, const float* X, const float* W, const float* dp, float* dW, float* db,
-             float* dX, int acc) {
+             const float* add, float* dX) {
     k_head_bwd_w<<<cdiv(24 * K * 128, kT), kT, 0, st>>>(B, K, X, dp, dW, db);
     DANET_LAUNCH_CHECK();
-    k_head_bwd_x<<<cdiv(B * 24 * 128, kT), kT, 0, st>>>(B, K, W, dp, dX, acc);
+    k_head_bwd_x<<<cdiv(B * 24 * 128, kT), kT, 0, st>>>(B, K, W, dp, add, dX);
     DANET_LAUNCH_CHECK();
     return 0;
 }
+
+// The largest batch: the R-row gemms' grid.y, cdiv(24 B, 64), must stay within 65535, and every B * 24 * F element
+// count (F <= 256) within int.  Both entries refuse a larger B before any launch.
+constexpr int kMaxBatch = 65535 * kGT / 24;
+static_assert((int64_t)kMaxBatch * 24 * 256 < ((int64_t)1 << 31), "element counts must fit in int");
 
 int check_params(const danet_gcn_train_params* p, int training, bool grads) {
     DANET_CHECK(p, "gcn_head_train: null parameter struct");
@@ -442,7 +461,7 @@ int check_params(const danet_gcn_train_params* p, int training, bool grads) {
 using namespace danet;
 
 extern "C" int64_t danet_gcn_head_train_workspace_bytes(int32_t B) {
-    if (B < 1) return 0;
+    if (B < 1 || B > kMaxBatch) return 0;
     return (int64_t)layout(B).total * (int64_t)sizeof(float);
 }
 
@@ -450,7 +469,7 @@ extern "C" int danet_gcn_head_train_forward(int32_t B, const danet_gcn_train_par
                                             const float* rot_feats, const float* global_para, float* para, float* pose0,
                                             float* coord0, float* coord1, float* new_stats, void* workspace,
                                             danet_stream_t stream) {
-    DANET_CHECK(B >= 1 && B <= (1 << 20), "danet_gcn_head_train_forward: bad batch size %d", B);
+    DANET_CHECK(B >= 1 && B <= kMaxBatch, "danet_gcn_head_train_forward: batch size %d outside 1..%d", B, kMaxBatch);
     GT_TRY(check_params(p, training, false));
     DANET_CHECK(rot_feats && global_para && para && workspace, "danet_gcn_head_train_forward: null pointer");
     DANET_CHECK(!training || (pose0 && coord0 && coord1), "danet_gcn_head_train_forward: training mode needs pose0 / coord0 / coord1");
@@ -470,7 +489,7 @@ extern "C" int danet_gcn_head_train_forward(int32_t B, const danet_gcn_train_par
     const int R = 24 * B;
     for (int l = 0; l < 5; ++l) {
         const int Fi = kDI[l], Fo = kDO[l];
-        GT_TRY(adj_mul(st, B, Fi, adj[l], 0, X, w + L.AX[l], 0));
+        GT_TRY(adj_mul(st, B, Fi, adj[l], 0, X, nullptr, w + L.AX[l]));
         GT_TRY(gemm(st, R, Fo, Fi, w + L.AX[l], Fi, 1, p->W[l], Fo, 1, p->b[l], w + L.Y[l]));
         const bool upd = training && new_stats;
         k_bn_stats<<<24, kT, 0, st>>>(B, Fo, w + L.Y[l], training, p->running_mean[l], p->running_var[l], w + L.mean[l],
@@ -495,7 +514,7 @@ extern "C" int danet_gcn_head_train_backward(int32_t B, const danet_gcn_train_pa
                                              const float* rot_feats, const float* g_para, const float* g_pose0,
                                              const float* g_coord0, const float* g_coord1, float* g_rot_feats,
                                              float* g_global_para, void* workspace, danet_stream_t stream) {
-    DANET_CHECK(B >= 1 && B <= (1 << 20), "danet_gcn_head_train_backward: bad batch size %d", B);
+    DANET_CHECK(B >= 1 && B <= kMaxBatch, "danet_gcn_head_train_backward: batch size %d outside 1..%d", B, kMaxBatch);
     GT_TRY(check_params(p, training, true));
     DANET_CHECK(rot_feats && g_para && g_rot_feats && g_global_para && workspace, "danet_gcn_head_train_backward: null pointer");
     DANET_CHECK(!training || (g_pose0 && g_coord0 && g_coord1),
@@ -506,12 +525,11 @@ extern "C" int danet_gcn_head_train_backward(int32_t B, const danet_gcn_train_pa
     float* w = (float*)workspace;
     const int R = 24 * B;
     const float* adj[5] = {p->r2p_A, w + L.Ahat, w + L.Ahat, w + L.Ahat, p->p2r_A};
-    float* P0 = w + L.P[0]; float* P1 = w + L.P[1]; float* P2 = w + L.P[2];
-    float* dY = w + L.dY; float* dAX = w + L.dAX;
-    // one GraphConv + BN + ReLU layer: dH -> gradients of its parameters, dX (+)= A^T (dY W^T)
-    auto layer = [&](int l, const float* dH, float* dX, int acc) -> int {
+    // one GraphConv + BN + ReLU layer: dH -> gradients of its parameters, dY[l], dAX[l] and dX = (add +) A^T dAX[l]
+    auto layer = [&](int l, const float* dH, const float* add, float* dX) -> int {
         const int Fi = kDI[l], Fo = kDO[l];
         const float* Xin = l == 0 ? rot_feats : w + L.H[l - 1];
+        float* dY = w + L.dY[l]; float* dAX = w + L.dAX[l];
         k_bn_bwd_reduce<<<24, kT, 0, st>>>(B, Fo, w + L.Y[l], w + L.mean[l], w + L.invstd[l], p->bn_weight[l], p->bn_bias[l],
                                            dH, p->g_bn_weight[l], p->g_bn_bias[l], w + L.sums);
         DANET_LAUNCH_CHECK();
@@ -526,23 +544,26 @@ extern "C" int danet_gcn_head_train_backward(int32_t B, const danet_gcn_train_pa
             k_dadj<<<576, kT, 0, st>>>(B, Fi, dAX, Xin, w + L.dA + (l - 1) * 576);
             DANET_LAUNCH_CHECK();
         }
-        return adj_mul(st, B, Fi, adj[l], 1, dAX, dX, acc);
+        return adj_mul(st, B, Fi, adj[l], 1, dAX, add, dX);
     };
+    float* gH[5];
+    for (int l = 0; l < 5; ++l) gH[l] = w + L.gH[l];
     // pose_regressors[1] + rot6d; global_para's gradient is para's first 13 columns
     k_rot6d_bwd<<<cdiv(B * 24, kT), kT, 0, st>>>(B, w + L.p6[1], g_para, 229, 13, w + L.dp6[1], g_global_para);
     DANET_LAUNCH_CHECK();
-    GT_TRY(head_bwd(st, B, 6, w + L.H[4], p->pose_w[1], w + L.dp6[1], p->g_pose_w[1], p->g_pose_b[1], P0, 0));
-    GT_TRY(layer(4, P0, P1, 0));                                        // P1 = d l_pos_feat
-    if (training) GT_TRY(head_bwd(st, B, 3, w + L.H[3], p->coord_w[1], g_coord1, p->g_coord_w[1], p->g_coord_b[1], P1, 1));
-    GT_TRY(layer(3, P1, P2, 0));
-    GT_TRY(layer(2, P2, P0, 0));
-    GT_TRY(layer(1, P0, P1, 1));                                        // + the residual's share already in P1
-    if (training) GT_TRY(head_bwd(st, B, 3, w + L.H[0], p->coord_w[0], g_coord0, p->g_coord_w[0], p->g_coord_b[0], P1, 1));
-    GT_TRY(layer(0, P1, g_rot_feats, 0));
+    GT_TRY(head_bwd(st, B, 6, w + L.H[4], p->pose_w[1], w + L.dp6[1], p->g_pose_w[1], p->g_pose_b[1], nullptr, gH[4]));
+    GT_TRY(layer(4, gH[4], nullptr, gH[3]));                           // gH[3] = d l_pos_feat
+    if (training) GT_TRY(head_bwd(st, B, 3, w + L.H[3], p->coord_w[1], g_coord1, p->g_coord_w[1], p->g_coord_b[1], gH[3], gH[3]));
+    GT_TRY(layer(3, gH[3], nullptr, gH[2]));
+    GT_TRY(layer(2, gH[2], nullptr, gH[1]));
+    GT_TRY(layer(1, gH[1], gH[3], gH[0]));                             // + the residual's share, gH[3]
+    if (training) GT_TRY(head_bwd(st, B, 3, w + L.H[0], p->coord_w[0], g_coord0, p->g_coord_w[0], p->g_coord_b[0], gH[0], gH[0]));
+    GT_TRY(layer(0, gH[0], nullptr, g_rot_feats));
     if (training) {
         k_rot6d_bwd<<<cdiv(B * 24, kT), kT, 0, st>>>(B, w + L.p6[0], g_pose0, 216, 0, w + L.dp6[0], nullptr);
         DANET_LAUNCH_CHECK();
-        GT_TRY(head_bwd(st, B, 6, rot_feats, p->pose_w[0], w + L.dp6[0], p->g_pose_w[0], p->g_pose_b[0], g_rot_feats, 1));
+        GT_TRY(head_bwd(st, B, 6, rot_feats, p->pose_w[0], w + L.dp6[0], p->g_pose_w[0], p->g_pose_b[0], g_rot_feats,
+                        g_rot_feats));
     }
     k_adj_bwd<<<1, 576, 0, st>>>(w + L.dA, w + L.M, w + L.d, p->A_mask, p->edge_importance, p->g_edge_importance);
     DANET_LAUNCH_CHECK();

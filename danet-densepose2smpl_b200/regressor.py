@@ -99,10 +99,10 @@ class _GcnHead(torch.autograd.Function):
     forward keeps its saved activations in a workspace the backward reads."""
 
     @staticmethod
-    def forward(ctx, training, bufs, new_stats, rot_feats, global_para, *params):
+    def forward(ctx, training, bufs, new_stats, ws_bytes, rot_feats, global_para, *params):
         dev, B = rot_feats.device, rot_feats.shape[0]
         with torch.cuda.device(dev):
-            ws = _lib.workspace(_lib.load().danet_gcn_head_train_workspace_bytes(B), dev)
+            ws = _lib.workspace(ws_bytes, dev)
             para = _empty(B, 229, dev=dev)
             pose0, c0, c1 = (_empty(B, 216, dev=dev), _empty(B, 24, 3, dev=dev), _empty(B, 24, 3, dev=dev)) if training \
                 else (None, None, None)
@@ -131,7 +131,7 @@ class _GcnHead(torch.autograd.Function):
             _lib.call("gcn_head_train_backward", B, ctypes.byref(p), int(training), _lib.ptr(rot_feats), _lib.ptr(g_para),
                       _lib.ptr(g_pose0), _lib.ptr(g_c0), _lib.ptr(g_c1), _lib.ptr(g_rot), _lib.ptr(g_gp), _lib.ptr(ctx.ws),
                       device=dev)
-        return (None, None, None, g_rot, g_gp, *grads)
+        return (None, None, None, None, g_rot, g_gp, *grads)
 
 
 def head_module(model):
@@ -157,6 +157,9 @@ def gcn_head(model, rot_feats, global_para):
     B = rot_feats.shape[0]
     if tuple(global_para.shape) != (B, 13):
         raise ValueError("%s: global_para must be [B,13] = [%d,13], got %s" % (where, B, tuple(global_para.shape)))
+    ws_bytes = _lib.load().danet_gcn_head_train_workspace_bytes(B)
+    if ws_bytes <= 0:                                   # refused before anything is allocated or launched
+        raise ValueError("%s: batch size %d is larger than the head's kernels take" % (where, B))
     _args.cuda(where, (("rot_feats", rot_feats), ("global_para", global_para)), dev)
     for (name, i), (di, do) in zip(LAYERS, DIMS):
         if tuple(_attr(mod, "%s.gc.%d.weight" % (name, i)).shape) != (di, do):
@@ -168,8 +171,8 @@ def gcn_head(model, rot_feats, global_para):
     if any(t.dtype != torch.float32 or not t.is_contiguous() for t in params + bufs):
         raise ValueError("%s: the head's parameters and buffers must be contiguous fp32" % where)
     new_stats = torch.empty(2, 5, 24, device=dev) if training else None
-    out = _GcnHead.apply(training, bufs, new_stats, rot_feats.float().contiguous(), global_para.float().contiguous(),
-                         *params)
+    out = _GcnHead.apply(training, bufs, new_stats, ws_bytes, rot_feats.float().contiguous(),
+                         global_para.float().contiguous(), *params)
     if not training:
         return {"para": out, "joint_rotation": [], "joint_position": []}
     with torch.no_grad():                     # in-place: the tensors' versions move, so plans refold their BatchNorm

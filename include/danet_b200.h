@@ -417,7 +417,8 @@ typedef struct {
     float* g_edge_importance;
     float* g_pose_w[2]; float* g_pose_b[2]; float* g_coord_w[2]; float* g_coord_b[2];
 } danet_gcn_train_params;
-/* Bytes of the workspace one forward + backward pair shares (saved activations and backward scratch). */
+/* Bytes of the workspace one forward + backward pair shares (saved activations and backward intermediates); 0 outside
+ * 1 <= B <= 174760, the batch sizes the entries accept (cdiv(24 B, 64) gemm row blocks fit a grid's y dimension). */
 int64_t danet_gcn_head_train_workspace_bytes(int32_t B);
 /* smpl_regressor.py:849-895 + GCN.py:29-92 + graph.py:232-261 (normalize_undigraph of I_n + A_mask * relu(E), on the
  * device) + geometry.py rot6d_to_rotmat: rot_feats [B,24,128], global_para [B,13] -> para [B,229]; in training mode

@@ -1,9 +1,13 @@
-"""Times one training step of the regressor head -- gcn_head forward + the three head losses + backward to every head
-parameter, rot_feats and global_para (danet_b200.regressor, csrc/gcn_train.cu) -- at B = 16 (the reference's training
-batch) and B = 64, with CUDA events after warm-up.  For scale, the same step through the oracle's torch restatement
-(oracle/gcn_head.py torch_head, fp32 autograd over eager torch ops) on the same device.  Prints one JSON object with
-the device name and power limit read in the same run and the number of kernel launches per step (torch.profiler).
-Dev tool: `python tools/gcn_head_bench.py [--out FILE]`."""
+"""Times one training step of the regressor head (danet_b200.regressor, csrc/gcn_train.cu) at B = 16 (the reference's
+training batch) and B = 64, with CUDA events after warm-up: the whole step, and separately its forward (gcn_head + the
+three head losses) and its backward (autograd to every head parameter, rot_feats and global_para), each the mean
+device time between events recorded around that half of every step.  For scale, the same step through the oracle's
+torch restatement (oracle/gcn_head.py torch_head, fp32 autograd over eager torch ops) on the same device.
+
+--compare PATH loads another build of libdanet_b200.so into the same process and times the two builds in alternating
+rounds (in-tree, other, in-tree, ...), so that both see the same device, clocks and neighbours.  Prints one JSON
+object with the device name and power limit read in the same run and the number of kernel launches per step
+(torch.profiler).  Dev tool: `python tools/gcn_head_bench.py [--out FILE] [--compare PATH] [--rounds N]`."""
 import json
 import os
 import subprocess
@@ -12,6 +16,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.nn.functional as F
+from danet_b200 import _lib
 from danet_b200 import build_synthetic_danet
 from danet_b200.regressor import BN_NAMES, PARAM_NAMES, gcn_head, gcn_head_losses
 from oracle import gcn_head as og
@@ -37,6 +42,22 @@ def timed(f, n=50, warm=5):
     return e0.elapsed_time(e1) / n
 
 
+def split(fwd, bwd, n=50, warm=5):
+    """(forward ms, backward ms) per step: events before, between and after the two halves of every step"""
+    for _ in range(warm):
+        bwd(fwd())
+    torch.cuda.synchronize()
+    ev = [[torch.cuda.Event(enable_timing=True) for _ in range(3)] for _ in range(n)]
+    for e in ev:
+        e[0].record()
+        o = fwd()
+        e[1].record()
+        bwd(o)
+        e[2].record()
+    torch.cuda.synchronize()
+    return sum(e[0].elapsed_time(e[1]) for e in ev) / n, sum(e[1].elapsed_time(e[2]) for e in ev) / n
+
+
 def launches(f):
     from torch.profiler import ProfilerActivity, profile
     f()
@@ -48,7 +69,22 @@ def launches(f):
                and not e.key.startswith(("Memcpy", "Memset")))
 
 
-res = {}
+def arg(name, default):
+    return sys.argv[sys.argv.index(name) + 1] if name in sys.argv else default
+
+
+builds = {"in_tree": _lib.load()}
+if "--compare" in sys.argv:                               # a second handle: the module-level one is swapped per round
+    tree_path, _lib._lib = _lib.LIB_PATH, None
+    _lib.LIB_PATH = os.path.abspath(arg("--compare", None))
+    builds["compare"] = _lib.load()
+    res_paths = {"in_tree": tree_path, "compare": _lib.LIB_PATH}
+    _lib.LIB_PATH, _lib._lib = tree_path, builds["in_tree"]
+else:
+    res_paths = {"in_tree": _lib.LIB_PATH}
+rounds = int(arg("--rounds", 3))
+
+res = {"builds": res_paths}
 for B in (16, 64):
     g = torch.Generator(device=dev).manual_seed(B)
     rot = torch.rand(B, 24, 128, device=dev, generator=g).requires_grad_()
@@ -58,11 +94,16 @@ for B in (16, 64):
     has = (torch.rand(B, device=dev, generator=g) < 0.7).to(torch.uint8)
     G = torch.randn(B, 229, device=dev, generator=g)
 
-    def ours():
+    def fwd():
         out = gcn_head(net, rot, gp)
         L = gcn_head_losses(out, target, gt, has)
-        tot = L["joint_rotation0"] + L["joint_position0"] + L["joint_position1"] + (out["para"] * G).sum()
+        return L["joint_rotation0"] + L["joint_position0"] + L["joint_position1"] + (out["para"] * G).sum()
+
+    def bwd(tot):
         torch.autograd.grad(tot, leaves + [rot, gp])
+
+    def ours():
+        bwd(fwd())
 
     bn = {n: (mod.get_submodule(n).running_mean.clone(), mod.get_submodule(n).running_var.clone()) for n in BN_NAMES}
     sel = (has == 1).float()
@@ -74,8 +115,18 @@ for B in (16, 64):
         lp = sum(F.l1_loss(c * sel[:, None, None], gt * sel[:, None, None], reduction="sum") / n for c in (c0, c1))
         torch.autograd.grad(lr + lp + (para * G).sum(), leaves + [rot, gp])
 
-    res["B%d" % B] = {"ms": timed(ours), "launches": launches(ours),
-                      "torch_restatement_fp32_autograd_ms": timed(torch_ref), "torch_launches": launches(torch_ref)}
+    r = {name: {"step_ms": [], "forward_ms": [], "backward_ms": []} for name in builds}
+    for _ in range(rounds):
+        for name, h in builds.items():
+            _lib._lib = h
+            r[name]["step_ms"].append(timed(ours))
+            f_ms, b_ms = split(fwd, bwd)
+            r[name]["forward_ms"].append(f_ms)
+            r[name]["backward_ms"].append(b_ms)
+    _lib._lib = builds["in_tree"]
+    r["launches"] = launches(ours)
+    r["torch_restatement_fp32_autograd_ms"], r["torch_launches"] = timed(torch_ref), launches(torch_ref)
+    res["B%d" % B] = r
 try:
     res["device"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                                    capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
