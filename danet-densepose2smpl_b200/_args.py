@@ -48,3 +48,15 @@ def int_pair(where, name, v):
     if isinstance(v, bool) or not isinstance(v, int):
         raise ValueError("%s: %s must be an int (got %r)" % (where, name, v))
     return v
+
+
+def mask(where, name, t, shape):
+    """t is a bool or uint8 tensor of shape `shape` (a per-image flag; nonzero = true), contiguous."""
+    if not isinstance(t, torch.Tensor):
+        raise ValueError("%s: %s must be a tensor (got %s)" % (where, name, type(t).__name__))
+    if t.dtype not in (torch.bool, torch.uint8):
+        raise ValueError("%s: %s must be bool or uint8 (got %s)" % (where, name, t.dtype))
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError("%s: %s must have shape %s (got %s)" % (where, name, tuple(shape), tuple(t.shape)))
+    if not t.is_contiguous():
+        raise ValueError("%s: %s must be contiguous" % (where, name))

@@ -87,7 +87,11 @@ SIGNATURES = {
     "danet_raster_destroy": (c_int, [c_p]),
     "danet_raster_workspace_bytes": (c_i64, [c_p, c_int]),
     "danet_raster_iuv": (c_int, [c_p, c_int, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
+    "danet_raster_iuv_select": (c_int, [c_p, c_int] + [c_p] * 11),
     "danet_iuv_img2map": (c_int, [c_int, c_int, c_p, c_p, c_p, c_p, c_p, c_p]),
+    "danet_estimate_translation": (c_int, [c_int, c_p, c_p, ctypes.c_double, ctypes.c_double, c_p, c_p]),
+    "danet_fit_merge": (c_int, [c_int] + [c_p] * 12),
+    "danet_train_targets": (c_int, [c_int] + [c_p] * 8 + [ctypes.c_double, c_int] + [c_p] * 5),
     "danet_conv_tc_packed_bytes": (c_i64, [ctypes.POINTER(ConvDesc)]),
     "danet_conv_tc_pack": (c_int, [ctypes.POINTER(ConvDesc), c_p, c_p, c_p]),
     "danet_conv_tc_supported": (c_int, [ctypes.POINTER(ConvDesc)]),

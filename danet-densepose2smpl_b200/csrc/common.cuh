@@ -94,6 +94,36 @@ __device__ __forceinline__ void rot6d(const float* x, float* R) {
     R[6] = s.b1.z; R[7] = s.b2.z; R[8] = b3.z;
 }
 
+// batch_rodrigues (utils/geometry.py:9-45, the quaternion route): axis-angle v -> row-major R.  danet_batch_rodrigues and
+// the training targets' 229-wide `target` (csrc/targets.cu) run this one definition.
+__device__ __forceinline__ void rodrigues_quat(const float* v, float* R) {
+    const float ax = v[0] + 1e-8f, ay = v[1] + 1e-8f, az = v[2] + 1e-8f;
+    const float l = sqrtf(ax * ax + ay * ay + az * az);
+    const float nx = v[0] / l, ny = v[1] / l, nz = v[2] / l;
+    const float h = l * 0.5f;
+    const float sn = sinf(h);
+    float w = cosf(h), x = sn * nx, y = sn * ny, z = sn * nz;
+    const float qn = sqrtf(w * w + x * x + y * y + z * z);
+    w /= qn; x /= qn; y /= qn; z /= qn;
+    const float w2 = w * w, x2 = x * x, y2 = y * y, z2 = z * z;
+    const float wx = w * x, wy = w * y, wz = w * z, xy = x * y, xz = x * z, yz = y * z;
+    R[0] = w2 + x2 - y2 - z2; R[1] = 2 * xy - 2 * wz;   R[2] = 2 * wy + 2 * xz;
+    R[3] = 2 * wz + 2 * xy;   R[4] = w2 - x2 + y2 - z2; R[5] = 2 * yz - 2 * wx;
+    R[6] = 2 * xz - 2 * wy;   R[7] = 2 * wx + 2 * yz;   R[8] = w2 - x2 - y2 + z2;
+}
+
+// perspective_projection (utils/geometry.py:63-91) of one point p: rotation R (row-major), translation t, focal f,
+// centre c -> out[2].  danet_perspective_projection and the training targets' key points run this one definition.
+__device__ __forceinline__ void persp_point(const float* R, const float* t, float f, const float* c, float px, float py,
+                                            float pz, float* out) {
+    const float x = R[0] * px + R[1] * py + R[2] * pz + t[0];
+    const float y = R[3] * px + R[4] * py + R[5] * pz + t[1];
+    const float z = R[6] * px + R[7] * py + R[8] * pz + t[2];
+    const float xn = x / z, yn = y / z, zn = z / z;
+    out[0] = f * xn + c[0] * zn;
+    out[1] = f * yn + c[1] * zn;
+}
+
 // cudaFuncSetAttribute is per device: true the first time the calling thread's current device is seen by this
 // call site (`mask` is the site's static bit set, one bit per device ordinal; -1 on error)
 inline std::mutex& first_use_mutex() { static std::mutex m; return m; }

@@ -87,22 +87,7 @@ __device__ __forceinline__ void rodrigues_smplx(const float* v, float* R) {
     R[6] = s * (-y) + c1 * (x * z);        R[7] = s * x + c1 * (y * z);          R[8] = 1.0f + c1 * (-(y * y) - x * x);
 }
 
-__device__ __forceinline__ void rodrigues_quat(const float* v, float* R) {
-    // utils/geometry.py:9-45
-    const float ax = v[0] + 1e-8f, ay = v[1] + 1e-8f, az = v[2] + 1e-8f;
-    const float l = sqrtf(ax * ax + ay * ay + az * az);
-    const float nx = v[0] / l, ny = v[1] / l, nz = v[2] / l;
-    const float h = l * 0.5f;
-    const float sn = sinf(h);
-    float w = cosf(h), x = sn * nx, y = sn * ny, z = sn * nz;
-    const float qn = sqrtf(w * w + x * x + y * y + z * z);
-    w /= qn; x /= qn; y /= qn; z /= qn;
-    const float w2 = w * w, x2 = x * x, y2 = y * y, z2 = z * z;
-    const float wx = w * x, wy = w * y, wz = w * z, xy = x * y, xz = x * z, yz = y * z;
-    R[0] = w2 + x2 - y2 - z2; R[1] = 2 * xy - 2 * wz;   R[2] = 2 * wy + 2 * xz;
-    R[3] = 2 * wz + 2 * xy;   R[4] = w2 - x2 + y2 - z2; R[5] = 2 * yz - 2 * wx;
-    R[6] = 2 * xz - 2 * wy;   R[7] = 2 * wx + 2 * yz;   R[8] = w2 - x2 - y2 + z2;
-}
+// rodrigues_quat (utils/geometry.py:9-45) is common.cuh's, shared with the training targets (csrc/targets.cu)
 
 __global__ void k_rot6d(int n, const float* __restrict__ x, float* __restrict__ R) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -130,14 +115,8 @@ __global__ void k_persp(int B, int N, const float* __restrict__ pts, const float
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= B * N) return;
     const int b = i / N;
-    const float* R = rot + (size_t)b * 9;
-    const float px = pts[(size_t)i * 3], py = pts[(size_t)i * 3 + 1], pz = pts[(size_t)i * 3 + 2];
-    const float x = R[0] * px + R[1] * py + R[2] * pz + tr[b * 3 + 0];
-    const float y = R[3] * px + R[4] * py + R[5] * pz + tr[b * 3 + 1];
-    const float z = R[6] * px + R[7] * py + R[8] * pz + tr[b * 3 + 2];
-    const float xn = x / z, yn = y / z, zn = z / z;
-    out[(size_t)i * 2 + 0] = focal[b] * xn + center[b * 2 + 0] * zn;
-    out[(size_t)i * 2 + 1] = focal[b] * yn + center[b * 2 + 1] * zn;
+    persp_point(rot + (size_t)b * 9, tr + b * 3, focal[b], center + b * 2, pts[(size_t)i * 3], pts[(size_t)i * 3 + 1],
+                pts[(size_t)i * 3 + 2], out + (size_t)i * 2);
 }
 
 __global__ void k_mpjpe(int B, const float* __restrict__ j17, const float* __restrict__ gt14,

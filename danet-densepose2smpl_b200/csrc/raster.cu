@@ -14,6 +14,8 @@
 //               25/25/25/15-channel maps
 // All geometry uses __f*_rn intrinsics (no FMA contraction) in the order oracle/raster.c uses,
 // so the integer winner (face id -> part id) is bit-exact against the CPU restatement.
+// danet_raster_iuv_select renders a per-image subset (danet.py:163-165): k_project and k_faces skip the other images,
+// whose z-buffer stays cleared, so k_resolve writes them as the zero image and its maps.
 #include "common.cuh"
 
 struct danet_raster {
@@ -31,10 +33,11 @@ __device__ __forceinline__ float fd(float a, float b) { return __fdiv_rn(a, b); 
 
 __global__ void k_project(int B, int nv, int nmv, const float* __restrict__ verts,
                           const float* __restrict__ cam, const int* __restrict__ vmap, float focal,
-                          int orig, float* __restrict__ pv) {
+                          int orig, const uint8_t* __restrict__ select, float* __restrict__ pv) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= B * nmv) return;
     const int b = i / nmv, k = i % nmv;
+    if (select && !select[b]) return;                 // unselected image: k_faces never reads its vertices
     const float* v = verts + ((size_t)b * nv + vmap[k]) * 3;
     const float* c = cam + (size_t)b * 3;
     const float o = (float)orig;
@@ -57,10 +60,11 @@ __global__ void k_project(int B, int nv, int nmv, const float* __restrict__ vert
 
 __global__ void k_faces(int B, int nmv, int nf, int S, float near_, float far_,
                         const float* __restrict__ pv, const int* __restrict__ faces,
-                        unsigned long long* __restrict__ zbuf) {
+                        const uint8_t* __restrict__ select, unsigned long long* __restrict__ zbuf) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= B * nf) return;
     const int b = i / nf, f = i % nf;
+    if (select && !select[b]) return;                 // its z-buffer stays cleared: k_resolve writes background
     float face[9];
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -237,23 +241,30 @@ extern "C" int64_t danet_raster_workspace_bytes(danet_raster_t h, int32_t B) {
     return RasterWs(h, B, nullptr).bytes;
 }
 
-extern "C" int danet_raster_iuv(danet_raster_t h, int32_t B, const float* verts, const float* cam, float* img,
-                                int32_t* face_idx, float* maps_u, float* maps_v, float* maps_i, float* maps_ann,
-                                void* workspace, danet_stream_t stream_) {
+extern "C" int danet_raster_iuv_select(danet_raster_t h, int32_t B, const float* verts, const float* cam,
+                                       const uint8_t* select, float* img, int32_t* face_idx, float* maps_u, float* maps_v,
+                                       float* maps_i, float* maps_ann, void* workspace, danet_stream_t stream_) {
     DANET_CHECK(h, "danet_raster_iuv: null handle");
     DANET_CHECK(B > 0, "danet_raster_iuv: empty batch (B=%d)", B);
     DANET_CHECK(verts && cam && workspace, "danet_raster_iuv: null input/workspace pointer");
     cudaStream_t stream = (cudaStream_t)stream_;
     const RasterWs ws(h, B, workspace);
     DANET_CUDA(cudaMemsetAsync(ws.zbuf, 0xff, (size_t)B * h->S * h->S * 8, stream));
-    k_project<<<cdiv(B * h->nmv, 256), 256, 0, stream>>>(B, h->nv, h->nmv, verts, cam, h->vmap, h->focal, h->orig, ws.pv);
+    k_project<<<cdiv(B * h->nmv, 256), 256, 0, stream>>>(B, h->nv, h->nmv, verts, cam, h->vmap, h->focal, h->orig, select, ws.pv);
     DANET_LAUNCH_CHECK();
-    k_faces<<<cdiv(B * h->nf, 128), 128, 0, stream>>>(B, h->nmv, h->nf, h->S, h->near_, h->far_, ws.pv, h->faces, ws.zbuf);
+    k_faces<<<cdiv(B * h->nf, 128), 128, 0, stream>>>(B, h->nmv, h->nf, h->S, h->near_, h->far_, ws.pv, h->faces, select, ws.zbuf);
     DANET_LAUNCH_CHECK();
     k_resolve<<<cdiv(B * h->S * h->S, 256), 256, 0, stream>>>(B, h->S, h->nf, h->tex_mode, ws.zbuf, h->tex, img, face_idx,
                                                             maps_u, maps_v, maps_i, maps_ann);
     DANET_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int danet_raster_iuv(danet_raster_t h, int32_t B, const float* verts, const float* cam, float* img,
+                                int32_t* face_idx, float* maps_u, float* maps_v, float* maps_i, float* maps_ann,
+                                void* workspace, danet_stream_t stream) {
+    return danet_raster_iuv_select(h, B, verts, cam, nullptr, img, face_idx, maps_u, maps_v, maps_i, maps_ann, workspace,
+                                   stream);
 }
 
 extern "C" int danet_iuv_img2map(int32_t B, int32_t S, const float* img, float* maps_u, float* maps_v,

@@ -87,7 +87,9 @@ class IUV_Renderer(object):
             pass
 
     @torch.no_grad()
-    def _render(self, verts, cam, want_maps=False, want_face_idx=False):
+    def _render(self, verts, cam, want_maps=False, want_face_idx=False, select=None):
+        """select: optional uint8 [B] on the device; images with select == 0 are not rasterised and come out as
+        background (the zero image and its maps), as danet.py:163-165 renders only the has_iuv images."""
         _lib.require_cuda(verts, "verts")
         dev = verts.device
         B = verts.size(0)
@@ -109,8 +111,12 @@ class IUV_Renderer(object):
             img = torch.empty(B, 3, S, S, device=dev)
             fidx = torch.empty(B, S, S, dtype=torch.int32, device=dev) if want_face_idx else None
             maps = [torch.empty(B, c, S, S, device=dev) for c in (25, 25, 25, 15)] if want_maps else [None] * 4
-            _lib.call("raster_iuv", h, B, _lib.ptr(verts_c), _lib.ptr(cam_c), _lib.ptr(img), _lib.ptr(fidx),
-                      *map(_lib.ptr, maps), _lib.ptr(ws))
+            if select is None:
+                _lib.call("raster_iuv", h, B, _lib.ptr(verts_c), _lib.ptr(cam_c), _lib.ptr(img), _lib.ptr(fidx),
+                          *map(_lib.ptr, maps), _lib.ptr(ws))
+            else:
+                _lib.call("raster_iuv_select", h, B, _lib.ptr(verts_c), _lib.ptr(cam_c), _lib.ptr(select), _lib.ptr(img),
+                          _lib.ptr(fidx), *map(_lib.ptr, maps), _lib.ptr(ws))
         return img, fidx, maps
 
     def verts2uvimg(self, verts, cam):

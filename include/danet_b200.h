@@ -98,6 +98,36 @@ int danet_mpjpe_h36m(int32_t B, const float* pred_j17, const float* gt_j14, floa
                      danet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Training targets (csrc/targets.cu).  No entry synchronises with the host, so a step's target
+ * preparation can be captured in one CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+/* utils/geometry.py:94-157 estimate_translation (with estimate_translation_np): S [B,49,3] joints and joints_2d
+ * [B,49,3] key points (x, y in pixels, confidence), of which joints 25..48 are used -> trans [B,3].  Weights are the
+ * fp32 sqrt of the confidences; the normal equations are formed and solved (LU with partial pivoting) in fp64 and
+ * rounded once to fp32.  Where numpy raises LinAlgError (an exactly zero pivot: every confidence 0), the row is NaN. */
+int danet_estimate_translation(int32_t B, const float* S, const float* joints_2d, double focal_length, double img_size,
+                               float* trans, danet_stream_t stream);
+/* train/trainer.py:157-161 and :177-191: fit_pose [B,72] / fit_betas [B,10] (the SPIN fits) with a row's betas zeroed
+ * when any |beta| > 3, then replaced by gt_pose / gt_betas where has_smpl -> opt_pose, opt_betas; valid_fit [B] =
+ * has_smpl | fit_valid (fit_valid NULL = has_smpl alone); has_iuv [B] = iuv_annotated & valid_fit.  Flags are uint8,
+ * nonzero = true; the outputs are 0 / 1. */
+int danet_fit_merge(int32_t B, const float* fit_pose, const float* fit_betas, const float* gt_pose, const float* gt_betas,
+                    const uint8_t* has_smpl, const uint8_t* fit_valid, const uint8_t* iuv_annotated, float* opt_pose,
+                    float* opt_betas, uint8_t* valid_fit, uint8_t* has_iuv, danet_stream_t stream);
+/* train/trainer.py:163-212 after the SMPL forward of the merged fits, and models/danet/danet.py:159-162.
+ * opt_joints [B,49,3] and smpl_joints [B,24,3] of that forward, keypoints [B,49,3] (x, y in [-1,1], confidence),
+ * opt_pose [B,72], opt_betas [B,10], has_iuv / has_dp [B] uint8, smpl_2dkps [B,24,3] ->
+ *   opt_cam_t [B,3]        danet_estimate_translation of opt_joints on the de-normalised key points (:168-175)
+ *   target_cam [B,3]       [2 f / img_res / t_z, t_x, t_y] (:208-212)
+ *   target_smpl_kps [B,24,3]  smpl_joints projected with R = I, t = opt_cam_t, centre img_res / 2, normalised to
+ *                          [-1,1], confidence (has_iuv == 1); the row is smpl_2dkps where has_dp == 1 (:194-204)
+ *   target [B,229]         cat(target_cam, opt_betas, batch_rodrigues(opt_pose)), quaternion route (danet.py:159-162) */
+int danet_train_targets(int32_t B, const float* opt_joints, const float* smpl_joints, const float* keypoints,
+                        const float* opt_pose, const float* opt_betas, const uint8_t* has_iuv, const uint8_t* has_dp,
+                        const float* smpl_2dkps, double focal_length, int32_t img_res, float* opt_cam_t, float* target_cam,
+                        float* target_smpl_kps, float* target, danet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Dense IUV losses of the training step (SURVEY section 8f-2), forward and backward in one pass.
  * Replaces models/danet/iuv_estimator.py:304-341 (IUV_Estimator.body_uv_losses) and the autograd
  * graph torch records for it.  Predictions u/v/index [N,C,HW] and targets U/V/I [N,C,HW] (fp32,
@@ -182,6 +212,13 @@ int64_t danet_raster_workspace_bytes(danet_raster_t h, int32_t B);
 int danet_raster_iuv(danet_raster_t h, int32_t B, const float* verts, const float* cam, float* img,
                      int32_t* face_idx, float* maps_u, float* maps_v, float* maps_i, float* maps_ann,
                      void* workspace, danet_stream_t stream);
+/* danet_raster_iuv for the images b with select[b] != 0 (select [B] uint8; NULL = every image), as
+ * models/danet/danet.py:163-165 renders verts2uvimg(target_verts[has_iuv], target_cam[has_iuv]) into a zero image:
+ * the other images cost no rasterisation and come out as background (the zero image, face -1, its maps), whatever
+ * their vertices and camera hold.  danet_raster_iuv is this entry with select = NULL. */
+int danet_raster_iuv_select(danet_raster_t h, int32_t B, const float* verts, const float* cam, const uint8_t* select,
+                            float* img, int32_t* face_idx, float* maps_u, float* maps_v, float* maps_i, float* maps_ann,
+                            void* workspace, danet_stream_t stream);
 /* utils/iuvmap.py:103-151 on an arbitrary IUV image [B,3,S,S] */
 int danet_iuv_img2map(int32_t B, int32_t S, const float* img, float* maps_u, float* maps_v,
                       float* maps_i, float* maps_ann, danet_stream_t stream);
