@@ -230,7 +230,7 @@ class _DpUviaLosses(torch.autograd.Function):
 def dp_uvia_losses(U_estimated, V_estimated, Index_UV, Ann_Index, body_uv_X_points, body_uv_Y_points, body_uv_I_points,
                    body_uv_Ind_points, body_uv_U_points, body_uv_V_points, body_uv_point_weights, body_uv_ann_labels,
                    body_uv_ann_weights=None, has_dp=None, align_corners=False, point_weight=POINT_REGRESSION_WEIGHTS,
-                   part_weight=PART_WEIGHTS, index_weight=INDEX_WEIGHTS):
+                   part_weight=PART_WEIGHTS, index_weight=INDEX_WEIGHTS, check_labels=True):
     """models/danet/iuv_estimator.py:343-419 with the has_dp selection of :106-121, keyword names = the reference's
     blob names (datasets/base_dataset.py:228-232).  U/V_estimated, Index_UV [N,25,S,S]; Ann_Index [N,Cann,S,S];
     X / Y / I (/ Ind) points [N,P] (P = 196); U / V points and point weights [N,25*P] (patch-major); ann labels [N,S*S].
@@ -238,7 +238,9 @@ def dp_uvia_losses(U_estimated, V_estimated, Index_UV, Ann_Index, body_uv_X_poin
     what the reference's grid_sample call means on torch >= 1.3; True reproduces torch 1.1.
     Returns (loss_Udp, loss_Vdp, loss_IndexUVdp, loss_segAnndp), differentiable w.r.t. the four predictions.
     Deviation, stated: has_dp selects images on the device (no host synchronisation, no copies of the selected
-    predictions); with no image selected the losses are 0-dim zeros, not the reference's torch.zeros(1)."""
+    predictions); with no image selected the losses are 0-dim zeros, not the reference's torch.zeros(1).
+    check_labels=False skips the host-side label check (a host synchronisation), for callers that must stay off the
+    host; a label outside the classes then contributes nothing to the losses and gradients."""
     _lib.require_cuda(U_estimated, "U_estimated")
     u, v, idx, ann = U_estimated, V_estimated, Index_UV, Ann_Index
     if u.dim() != 4 or u.shape[1] != NUM_UV_CHANNELS or u.shape[2] != u.shape[3] or v.shape != u.shape or idx.shape != u.shape:
@@ -262,8 +264,9 @@ def dp_uvia_losses(U_estimated, V_estimated, Index_UV, Ann_Index, body_uv_X_poin
     if A.shape[1] != S * S:
         raise ValueError("dp_uvia_losses: body_uv_ann_labels must hold S*S labels per image")
     sel = None if has_dp is None else (has_dp.to(u.device) == 1)           # iuv_estimator.py:108
-    _check_labels(I.to(u.device), NUM_UV_CHANNELS, sel, "I_points")
-    _check_labels(A.to(u.device), ann.shape[1], sel, "ann")
+    if check_labels:
+        _check_labels(I.to(u.device), NUM_UV_CHANNELS, sel, "I_points")
+        _check_labels(A.to(u.device), ann.shape[1], sel, "ann")
     has = None if sel is None else sel.to(torch.uint8).contiguous()
     L = _DpUviaLosses.apply(u, v, idx, ann, (X, Y, I, Up, Vp, W, A), has, bool(align_corners), point_weight, part_weight,
                             index_weight)

@@ -246,9 +246,10 @@ _BN_KEYS = ("weight", "bias", "running_mean", "running_var", "num_batches_tracke
 _LOWERED = weakref.WeakKeyDictionary()
 
 
-def _lower_op(op):
+def _lower_op(op, where="lower_branches"):
     """One graph op -> training ops: dicts with the op name, input / output tensor names, their arguments and `keys`,
-    the state_dict keys the op consumes."""
+    the state_dict keys the op consumes.  `where` names the caller in refusals (danet_b200.estimator shares the conv
+    rule)."""
     kind, x, y = op["op"], op["x"].name, op["y"].name
     if kind == "conv":
         (wkey, _, has_bias), = op["parts"]
@@ -258,7 +259,7 @@ def _lower_op(op):
         conv["keys"] = tuple(k for k in (conv["weight"], conv["bias"]) if k)
         if not op["bn"]:
             if op["relu"] or op["res"] is not None:
-                raise ValueError("lower_branches: a residual or ReLU without BatchNorm (%s) has no training lowering" % wkey)
+                raise ValueError("%s: a residual or ReLU without BatchNorm (%s) has no training lowering" % (where, wkey))
             return [conv]
         conv["y"] = y + ":conv"
         bn = dict(op="batch_norm", x=conv["y"], y=y, bn=op["bn"], res=op["res"].name if op["res"] is not None else None,
@@ -272,7 +273,7 @@ def _lower_op(op):
         w, b, add = RP + "body_net.3.final_layer.weight", RP + "body_net.3.final_layer.bias", RP + "mean_cam_shape"
         return [dict(op="adaptive_avg_pool2d", x=x, y=y + ":pool", keys=()),
                 dict(op="linear", x=y + ":pool", y=y, weight=w, bias=b, add=add, keys=(w, b, add))]
-    raise ValueError("lower_branches: graph op %r has no training lowering" % kind)
+    raise ValueError("%s: graph op %r has no training lowering" % (where, kind))
 
 
 def _walk(graph, src, dst):
