@@ -10,6 +10,7 @@
 // so that the DANET_LOSSES_HOST_CHECK build walks it on the CPU against the reference-generated golden.
 #include "common.cuh"
 #include "stn_common.cuh"
+#include "loss_common.cuh"
 
 namespace danet {
 
@@ -26,7 +27,6 @@ namespace danet {
 #endif
 
 __host__ __device__ inline float sl1(float d) { const float a = fabsf(d); return a < 1.f ? 0.5f * d * d : a - 0.5f; }
-__host__ __device__ inline float sl1_grad(float d) { return fminf(fmaxf(d, -1.f), 1.f); }
 
 // bilinear footprint of one sample point: north-west corner and the four weights (nw, ne, sw, se).  Points whose
 // corners are all outside the map (or NaN coordinates) get x0 = y0 = -2: nothing is read or written for them.
@@ -111,7 +111,7 @@ __host__ __device__ inline float dp_point_map(const DpArgs& a, int n, int p, int
         const float x = foot_sample(pred + c * HW, a.S, f);
         coef[c] = x;
         if (c == lab) xt = x;
-        if (x > mx) { s = s * expf(mx - x) + 1.f; mx = x; } else s += expf(x - mx);
+        lse_step(x, mx, s);
     }
     if (lab < 0) {                           // rejected by the Python layer; the kernel just contributes nothing
         for (int c = 0; c < kDpC; ++c) coef[c] = 0.f;
@@ -154,7 +154,7 @@ __host__ __device__ inline float dp_pixel_ann(const DpArgs& a, int n, int pix, f
         for (int c = 0; c < a.Cann; ++c) {
             const float xv = DANET_LDG(x + c * HW);
             if (c == lab) xt = xv;
-            if (xv > mx) { s = s * expf(mx - xv) + 1.f; mx = xv; } else s += expf(xv - mx);
+            lse_step(xv, mx, s);
         }
     if (a.gann) {
         float* g = a.gann + (size_t)n * a.Cann * HW + pix;

@@ -10,6 +10,7 @@
 // gradients.  Loss sums: fp32 per thread and block, block partials to the workspace, one finishing block adds them in
 // double in a fixed order -- the result does not depend on the launch schedule.
 #include "common.cuh"
+#include "loss_common.cuh"
 
 namespace danet {
 
@@ -41,7 +42,9 @@ __global__ void k_loss_count(const uint8_t* has, int N, int* nsel) {
 #define DANET_LDG(p) (*(p))
 #endif
 
-// cross-entropy of one pixel: loss = lse(x) - x[target]; d/dx = (softmax - onehot) * scale.
+// cross-entropy of one pixel: loss = lse(x) - x[target]; d/dx = (softmax - onehot) * scale.  The target is
+// torch.argmax of the target map: the first maximum, NaN counting as maximal, channel 0 when every entry is -inf; the
+// loss and the gradient use that one channel.
 // The channel loops are unrolled by 4 over restrict-qualified pointers so that a thread has 8 / 4 independent loads in
 // flight (the first version, one load pair per iteration, was latency-bound: 18 long-scoreboard stalls per issue, ncu).
 __host__ __device__ inline float pixel_ce(const float* __restrict__ x, const float* __restrict__ t, float* __restrict__ g,
@@ -52,8 +55,8 @@ __host__ __device__ inline float pixel_ce(const float* __restrict__ x, const flo
 #pragma unroll 4
         for (int c = 0; c < C; ++c) {
             const float tv = DANET_LDG(t + (size_t)c * HW), xv = DANET_LDG(x + (size_t)c * HW);
-            if (tv > tmax) { tmax = tv; arg = c; xt = xv; }
-            if (xv > m) { s = s * expf(m - xv) + 1.f; m = xv; } else s += expf(xv - m);
+            if (c == 0 || tv > tmax || (tv != tv && tmax == tmax)) { tmax = tv; arg = c; xt = xv; }
+            lse_step(xv, m, s);
         }
     }
     const float lse = on ? m + logf(s) : 0.f;
@@ -91,8 +94,8 @@ __host__ __device__ inline float4 pixel_body_uv(const LossArgs& a, int n, int p,
             const float au = fabsf(du), av = fabsf(dv);
             lu += au < 1.f ? 0.5f * du * du : au - 0.5f;
             lv += av < 1.f ? 0.5f * dv * dv : av - 0.5f;
-            gu = fminf(fmaxf(du, -1.f), 1.f) * sc;
-            gv = fminf(fmaxf(dv, -1.f), 1.f) * sc;
+            gu = sl1_grad(du) * sc;
+            gv = sl1_grad(dv) * sc;
         }
         if (gup) gup[e] = gu;
         if (gvp) gvp[e] = gv;
