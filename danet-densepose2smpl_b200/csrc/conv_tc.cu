@@ -309,8 +309,9 @@ constexpr uint32_t kOffSchedRing = kOffSchedFull + 16 * kSchedDepth, kOffCursor 
 
 // Exact mode's copy cursor.  Warp 0 walks the copy sequence of its CTA's tile pairs (each pair: per channel chunk and
 // parity plane, the hi and lo halos of both tiles, then the plane's weight blocks) and runs it ahead of consumption by
-// the ring depths.  Its state is a row of ints in shared memory, so that it costs no registers where warp 0 runs it,
-// between wgmmas with every accumulator live.  Every lane of warp 0 reads and writes the same values.
+// the ring depths.  Its state is a row of ints in shared memory between runs, so that it costs no registers while the
+// tile body runs with every accumulator live; produce() holds the row in registers only while warp 0's own loop state
+// is parked (exact_tile).  Every lane of warp 0 reads and writes the same values.
 enum CursorField {
     kCurSeq, kCurPub, kCurPubEnd,        // pair being loaded, next scheduler ring entry to publish, the last one is out
     kCurPi,                              // problem of the pair being loaded (-1: take the next pair)
@@ -322,7 +323,8 @@ enum CursorField {
     kCurAs, kCurBs, kCurAph, kCurBph,    // next A / B slot and the empty-barrier phases
     kCurFields
 };
-static_assert(kOffCursor + 4 * kCurFields <= kOffPark && kOffPark + 4 * 32 <= 1024, "barrier region layout");
+constexpr int kCurWords = (kCurFields + 3) / 4 * 4;   // the row padded to whole 16-byte vectors (cur_load)
+static_assert(kOffCursor % 16 == 0 && kOffCursor + 4 * kCurWords <= kOffPark && kOffPark + 4 * 32 <= 1024, "barrier region layout");
 
 // consumer side of the scheduler ring: one lane waits for entry `seq`, reads the work unit and frees the entry
 __device__ __forceinline__ int sched_next(const Smem& S, int seq) {
@@ -356,31 +358,44 @@ __device__ __forceinline__ void cur_set(uint32_t cur, int f, int v) {
     asm volatile("st.shared.s32 [%0], %1;" ::"r"(cur + 4 * f), "r"(v) : "memory");
 }
 
-// Exact mode, warp 0 only, every lane (uniform control flow; the elected lane issues): warpgroup 0 has just released dA A
-// and dB B ring uses.  Issue the copies whose slots warpgroup 0 no longer holds, in consumption order, waiting for the
-// other warpgroups to free each slot.  Those never wait on a copy at or after the one waited for: a warpgroup frees a
-// weight block once the next block's MMAs are issued, and a halo slot at the end of its parity plane (drained), so only
-// earlier copies are needed.  Stops at the first copy whose slot warpgroup 0 still holds.
-__device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, int dB) {
-    const uint32_t cur = S.bar_a_full + kOffCursor;
-    cur_set(cur, kCurRa, cur_get(cur, kCurRa) + dA);
-    cur_set(cur, kCurRb, cur_get(cur, kCurRb) + dB);
+// The cursor's row as 16-byte vectors: produce() reads it once into registers and writes it back once, so its steps do
+// not wait on a shared-memory load each.
+__device__ __forceinline__ void cur_load(uint32_t cur, int* f) {
+#pragma unroll
+    for (int k = 0; k < kCurWords; k += 4)
+        asm volatile("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(f[k]), "=r"(f[k + 1]), "=r"(f[k + 2]), "=r"(f[k + 3])
+                     : "r"(cur + 4 * k) : "memory");
+}
+__device__ __forceinline__ void cur_store(uint32_t cur, const int* f) {
+#pragma unroll
+    for (int k = 0; k < kCurWords; k += 4)
+        asm volatile("st.shared.v4.s32 [%0], {%1, %2, %3, %4};" ::"r"(cur + 4 * k), "r"(f[k]), "r"(f[k + 1]), "r"(f[k + 2]),
+                     "r"(f[k + 3]) : "memory");
+}
+
+// Exact mode, warp 0 only, every lane (uniform control flow; the elected lane issues): the copy cursor's steps on its row f
+// (cur_load).  Issue the copies whose slots warpgroup 0 no longer holds (ring fills below the releases f[kCurRa],
+// f[kCurRb] plus the ring depths), in consumption order, waiting for the other warpgroups to free each slot.  Those never
+// wait on a copy at or after the one waited for: a warpgroup frees a weight block once the next block's MMAs are issued,
+// and a halo slot at the end of its parity plane (drained), so only earlier copies are needed.  Stops at the first copy
+// whose slot warpgroup 0 still holds.
+__device__ __forceinline__ void cursor_steps(const ArgsN& a, const Smem& S, int* f) {
 #pragma unroll 1
     for (;;) {
-        if (cur_get(cur, kCurPi) < 0) {
+        if (f[kCurPi] < 0) {
             // publish scheduler entries up to kSchedAhead pairs past the one loaded next, then take that one
 #pragma unroll 1
-            while (cur_get(cur, kCurPub) <= cur_get(cur, kCurSeq) + kSchedAhead && !cur_get(cur, kCurPubEnd)) {
-                const int pub = cur_get(cur, kCurPub), rs = pub & (kSchedDepth - 1);
+            while (f[kCurPub] <= f[kCurSeq] + kSchedAhead && !f[kCurPubEnd]) {
+                const int pub = f[kCurPub], rs = pub & (kSchedDepth - 1);
                 mbar_wait_inl(S.bar_a_full + kOffSchedEmpty + 8 * rs, ((pub / kSchedDepth) & 1) ^ 1);
                 const int t = sched_unit(a, pub, [&] { return __shfl_sync(0xffffffffu, atom_inc_elect(a.sched), 0); });
-                if (t == a.total_units) cur_set(cur, kCurPubEnd, 1);
+                if (t == a.total_units) f[kCurPubEnd] = 1;
                 st_arrive_elect(S.bar_a_full + kOffSchedRing + 4 * rs, t, S.bar_a_full + kOffSchedFull + 8 * rs);
-                cur_set(cur, kCurPub, pub + 1);
+                f[kCurPub] = pub + 1;
             }
             int pair;
             asm volatile("ld.shared.s32 %0, [%1];" : "=r"(pair)
-                         : "r"(S.bar_a_full + kOffSchedRing + 4 * (cur_get(cur, kCurSeq) & (kSchedDepth - 1))) : "memory");
+                         : "r"(S.bar_a_full + kOffSchedRing + 4 * (f[kCurSeq] & (kSchedDepth - 1))) : "memory");
             pair = __shfl_sync(0xffffffffu, pair, 0);            // the elected lane 0 wrote it
             if (pair >= a.total_units) return;
             const int pi = unit_prob(a, pair);
@@ -388,71 +403,75 @@ __device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, i
             const int pp = pair - a.unit_base[pi];
             {
                 const TileCoord tc = pair_coord(P, pp, 0);
-                cur_set(cur, kCurH0, tc.th * kTileH * P.stride - P.pad);
-                cur_set(cur, kCurW0, tc.tw * kTileW * P.stride - P.pad);
-                cur_set(cur, kCurImg0, tc.img0);
-                cur_set(cur, kCurBlk, tc.ws * (int)P.blocks_per_set + tc.nt * P.nblk);
+                f[kCurH0] = tc.th * kTileH * P.stride - P.pad;
+                f[kCurW0] = tc.tw * kTileW * P.stride - P.pad;
+                f[kCurImg0] = tc.img0;
+                f[kCurBlk] = tc.ws * (int)P.blocks_per_set + tc.nt * P.nblk;
             }
             {
                 const TileCoord tc = pair_coord(P, pp, 1);
-                cur_set(cur, kCurH1, tc.th * kTileH * P.stride - P.pad);
-                cur_set(cur, kCurImg1, tc.img0);
+                f[kCurH1] = tc.th * kTileH * P.stride - P.pad;
+                f[kCurImg1] = tc.img0;
             }
-            cur_set(cur, kCurC, 0); cur_set(cur, kCurSlot, 0); cur_set(cur, kCurStep, 0);
-            cur_set(cur, kCurPi, pi);
+            f[kCurC] = 0; f[kCurSlot] = 0; f[kCurStep] = 0;
+            f[kCurPi] = pi;
         }
-        const Prob& P = a.p[cur_get(cur, kCurPi)];
-        const int step = cur_get(cur, kCurStep);
+        const Prob& P = a.p[f[kCurPi]];
+        const int step = f[kCurStep], slot = f[kCurSlot];
         if (step < 2) {
             // the hi (step 0) or lo (step 1) halo plane of both tiles, into one A slot
-            if (cur_get(cur, kCurFa) >= cur_get(cur, kCurRa) + a.na_stages) return;
-            {
-                const int as = cur_get(cur, kCurAs);
-                mbar_wait_inl(S.bar_a_empty + 8 * as, ((cur_get(cur, kCurAph) >> as) & 1) ^ 1);
-                mbar_expect_tx_elect(S.bar_a_full + 8 * as, 2u * P.nstack * P.box_h * P.sbo_a);
-            }
+            if (f[kCurFa] >= f[kCurRa] + a.na_stages) return;
+            const int as = f[kCurAs];
+            mbar_wait_inl(S.bar_a_empty + 8 * as, ((f[kCurAph] >> as) & 1) ^ 1);
+            mbar_expect_tx_elect(S.bar_a_full + 8 * as, 2u * P.nstack * P.box_h * P.sbo_a);
             // box k: the first tile's nstack images, then the second tile's (rows or images beyond the map are out of
-            // bounds: zero fill).  Operands are read from the cursor right at the copy.
+            // bounds: zero fill)
 #pragma unroll 1
             for (int k = 0; k < 2 * P.nstack; ++k) {
-                const int h = k >= P.nstack ? 1 : 0, n = k - h * P.nstack, slot = cur_get(cur, kCurSlot), as = cur_get(cur, kCurAs);
+                const int h = k >= P.nstack ? 1 : 0, n = k - h * P.nstack;
                 tma_load_4d_elect(S.sA + as * a.a_slot_bytes + h * (a.a_slot_bytes >> 1) + n * P.hs * P.sbo_a,
-                                  &P.tm[step], cur_get(cur, kCurC) * P.KCH, cur_get(cur, kCurW0) + P.par_px[slot],
-                                  cur_get(cur, kCurH0 + h) + P.par_py[slot], cur_get(cur, kCurImg0 + h) + n * P.wsets,
+                                  &P.tm[step], f[kCurC] * P.KCH, f[kCurW0] + P.par_px[slot],
+                                  (h ? f[kCurH1] : f[kCurH0]) + P.par_py[slot], (h ? f[kCurImg1] : f[kCurImg0]) + n * P.wsets,
                                   S.bar_a_full + 8 * as);
             }
-            const int as = cur_get(cur, kCurAs);
-            cur_set(cur, kCurAph, cur_get(cur, kCurAph) ^ (1 << as));
-            cur_set(cur, kCurAs, as + 1 == a.na_stages ? 0 : as + 1);
-            cur_set(cur, kCurFa, cur_get(cur, kCurFa) + 1);
-            cur_set(cur, kCurStep, step + 1);
+            f[kCurAph] ^= 1 << as;
+            f[kCurAs] = as + 1 == a.na_stages ? 0 : as + 1;
+            f[kCurFa] += 1;
+            f[kCurStep] = step + 1;
         } else {
-            if (cur_get(cur, kCurFb) >= cur_get(cur, kCurRb) + a.nb_stages) return;
-            {
-                const int bs = cur_get(cur, kCurBs);
-                mbar_wait_inl(S.bar_b_empty + 8 * bs, ((cur_get(cur, kCurBph) >> bs) & 1) ^ 1);
-                const uint32_t bar = S.bar_b_full + 8 * bs;
-                mbar_expect_tx_elect(bar, (uint32_t)P.b_block_bytes);
-                bulk_g2s_elect(S.sB + bs * a.b_slot_bytes, P.wpk + kPackHeader + (long long)cur_get(cur, kCurBlk) * P.b_block_bytes,
-                               (uint32_t)P.b_block_bytes, bar);
-                cur_set(cur, kCurBph, cur_get(cur, kCurBph) ^ (1 << bs));
-                cur_set(cur, kCurBs, bs + 1 == a.nb_stages ? 0 : bs + 1);
-            }
-            cur_set(cur, kCurFb, cur_get(cur, kCurFb) + 1);
-            cur_set(cur, kCurBlk, cur_get(cur, kCurBlk) + 1);
-            const int slot = cur_get(cur, kCurSlot);
-            if (step - 1 < P.ngrp[slot]) cur_set(cur, kCurStep, step + 1);
+            if (f[kCurFb] >= f[kCurRb] + a.nb_stages) return;
+            const int bs = f[kCurBs];
+            mbar_wait_inl(S.bar_b_empty + 8 * bs, ((f[kCurBph] >> bs) & 1) ^ 1);
+            const uint32_t bar = S.bar_b_full + 8 * bs;
+            mbar_expect_tx_elect(bar, (uint32_t)P.b_block_bytes);
+            bulk_g2s_elect(S.sB + bs * a.b_slot_bytes, P.wpk + kPackHeader + (long long)f[kCurBlk] * P.b_block_bytes,
+                           (uint32_t)P.b_block_bytes, bar);
+            f[kCurBph] ^= 1 << bs;
+            f[kCurBs] = bs + 1 == a.nb_stages ? 0 : bs + 1;
+            f[kCurFb] += 1;
+            f[kCurBlk] += 1;
+            if (step - 1 < P.ngrp[slot]) f[kCurStep] = step + 1;
             else {                                            // the parity plane is complete
-                cur_set(cur, kCurStep, 0);
-                if (slot + 1 < P.npa) cur_set(cur, kCurSlot, slot + 1);
+                f[kCurStep] = 0;
+                if (slot + 1 < P.npa) f[kCurSlot] = slot + 1;
                 else {
-                    cur_set(cur, kCurSlot, 0);
-                    if (cur_get(cur, kCurC) + 1 < P.nchunks) cur_set(cur, kCurC, cur_get(cur, kCurC) + 1);
-                    else { cur_set(cur, kCurPi, -1); cur_set(cur, kCurSeq, cur_get(cur, kCurSeq) + 1); }
+                    f[kCurSlot] = 0;
+                    if (f[kCurC] + 1 < P.nchunks) f[kCurC] += 1;
+                    else { f[kCurPi] = -1; f[kCurSeq] += 1; }
                 }
             }
         }
     }
+}
+
+// Exact mode, warp 0 only: warpgroup 0 has just released dA A and dB B ring uses; run the copy cursor.
+__device__ __forceinline__ void produce(const ArgsN& a, const Smem& S, int dA, int dB) {
+    const uint32_t cur = S.bar_a_full + kOffCursor;
+    int f[kCurWords];
+    cur_load(cur, f);
+    f[kCurRa] += dA; f[kCurRb] += dB;
+    cursor_steps(a, S, f);
+    cur_store(cur, f);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -747,8 +766,9 @@ __device__ __forceinline__ void exact_tile(const ArgsN& a, const Prob& P, const 
                     mbar_arrive_if(S.bar_b_empty + 8 * pend_b, leader && pend_b >= 0);
                     pend_b = bs;
                 }
-                if (prod) {
-                    // Warp 0 runs the copy cursor.  Its loop state waits in shared memory meanwhile: with every
+                if (prod && (dA | dB)) {
+                    // Warp 0 runs the copy cursor, unless the block released no slot: then the cursor would stop at
+                    // the copy it stopped at last time.  Its loop state waits in shared memory meanwhile: with every
                     // accumulator live, the cursor has no registers to spare otherwise.  The reloads go through a
                     // shuffle so that ptxas still sees warp-uniform values (a loop bound it cannot prove uniform
                     // would serialise the wgmmas).
@@ -823,7 +843,7 @@ k_conv_tc_exact(const __grid_constant__ ArgsN a) {
     const Smem S = carve_smem(a);
     const int warp = warp_index(), lane = threadIdx.x & 31;
     if (threadIdx.x == 0)                                   // the copy cursor: no pair taken yet
-        for (int f = 0; f < kCurFields; ++f) cur_set(S.bar_a_full + kOffCursor, f, f == kCurPi ? -1 : 0);
+        for (int f = 0; f < kCurWords; ++f) cur_set(S.bar_a_full + kOffCursor, f, f == kCurPi ? -1 : 0);
     start_cta(a, S, kConsExact, 0, 2, warp, lane);
     const int wg = warp >> 2, w4 = warp & 3;
     const bool leader = (threadIdx.x & 127) == 0;          // releases ring slots for its warpgroup
