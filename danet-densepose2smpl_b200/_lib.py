@@ -75,6 +75,7 @@ SIGNATURES = {
     "danet_batch_rodrigues": (c_int, [c_int, c_p, c_p, c_int, c_p]),
     "danet_perspective_projection": (c_int, [c_int, c_int, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
     "danet_mpjpe_h36m": (c_int, [c_int, c_p, c_p, c_p, c_p]),
+    "danet_seg_confusion": (c_int, [c_int, c_int, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_p, c_p, c_p]),
     "danet_body_uv_losses_workspace_bytes": (c_i64, [c_int, c_int]),
     "danet_body_uv_losses": (c_int, [c_int, c_int, c_int, c_int, c_i64, c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p,
                                      c_p, c_f, c_f, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),

@@ -255,3 +255,53 @@ def keyed_state_dict(template, seed=0):
         t = keyed_tensor(k, v.shape, seed, _bn_role(k, template))
         out[k] = v.clone() if t is None else t.to(v.dtype)
     return out
+
+
+# ---------------------------------------------------------------------------------------------
+# evaluation stand-ins: the gendered SMPL models of 3DPW, PartRenderer's colour / part tables, and small caches
+# ---------------------------------------------------------------------------------------------
+def make_gendered_smpl_models(seed=0):
+    """{'male', 'female'} stand-ins for SMPL_MALE.pkl / SMPL_FEMALE.pkl: synthetic models of their own seeds that carry
+    the neutral model's J_regressor_h36m (eval.py uses one H36M regressor for every model)."""
+    h36m = make_smpl_model(seed)["J_regressor_h36m"]
+    out = {}
+    for k, g in enumerate(("male", "female")):
+        m = make_smpl_model(seed + 101 + k)
+        m["J_regressor_h36m"] = h36m
+        out[g] = m
+    return out
+
+
+def make_part_assets(seed=0):
+    """PartRenderer's textures (VERTEX_TEXTURE_FILE: a colour per face, placed so that floor(100 * c) is unambiguous) and
+    cube_parts (CUBE_PARTS_FILE: 100^3 part ids 0..6)."""
+    rng = np.random.default_rng(seed + 3)
+    tex = (rng.integers(0, 100, (NF, 3)).astype(np.float32) + 0.5) / 100.0
+    return {"textures": tex, "cube_parts": rng.integers(0, 7, (100, 100, 100)).astype(np.float32)}
+
+
+def make_eval_cache(dataset, n, seed=0):
+    """A small cache in the format danet_b200.eval_h36m reads for `dataset` ('3dpw' or 'lsp'), with uint8 RGB crops."""
+    rng = np.random.default_rng(seed + 4)
+    yy, xx = np.mgrid[0:224, 0:224]
+    img = ((np.sin(xx / 17.0)[None, :, :, None] + np.cos(yy / 23.0)[None, :, :, None]) * 60 + 128
+           + rng.normal(0, 20, (n, 224, 224, 3))).clip(0, 255).astype(np.uint8)
+    if dataset == "3dpw":
+        return {"img": img, "pose": (rng.normal(0, 0.2, (n, 72))).astype(np.float32),
+                "betas": rng.normal(0, 1, (n, 10)).astype(np.float32), "gender": rng.integers(-1, 2, n).astype(np.int32)}
+    if dataset != "lsp":
+        raise ValueError("make_eval_cache: '3dpw' or 'lsp' (got %r)" % (dataset,))
+    shapes = np.stack([rng.integers(120, 400, n), rng.integers(120, 400, n)], 1).astype(np.int64)
+    center = np.stack([rng.uniform(0.2, 0.8, n) * shapes[:, 1], rng.uniform(0.2, 0.8, n) * shapes[:, 0]], 1)
+    scale = rng.uniform(0.4, 1.2, n) * shapes.min(1) / 200.0
+    masks, parts = [], []
+    for h, w in shapes:
+        y, x = np.mgrid[0:h, 0:w]
+        cy, cx, ry, rx = rng.uniform(0.3, 0.7) * h, rng.uniform(0.3, 0.7) * w, rng.uniform(0.2, 0.4) * h, rng.uniform(0.1, 0.3) * w
+        inside = ((y - cy) / ry) ** 2 + ((x - cx) / rx) ** 2 < 1
+        masks.append(np.where(inside, 255, 0).astype(np.uint8).ravel())
+        p = np.where(inside, 1 + (y * 6) // h, 0).astype(np.uint8)
+        p[rng.random((h, w)) < 0.02] = 255
+        parts.append(p.ravel())
+    return {"img": img, "center": center.astype(np.float32), "scale": scale.astype(np.float64), "orig_shape": shapes,
+            "mask_gt": np.concatenate(masks), "parts_gt": np.concatenate(parts)}

@@ -96,6 +96,21 @@ int danet_perspective_projection(int32_t B, int32_t N, const float* points, cons
  * pelvis-centred + H36M_TO_J14-selected) -> mpjpe [B] */
 int danet_mpjpe_h36m(int32_t B, const float* pred_j17, const float* gt_j14, float* mpjpe,
                      danet_stream_t stream);
+/* eval.py:219-266 with utils/imutils.py:89-113 (uncrop): LSP mask and part scoring of B rendered maps at their
+ * original image sizes (csrc/seg_eval.cu).  mask / parts [B,R,R] uint8 (the render: mask nonzero = covered -- the
+ * caller applies toimage's bytescale, which empties an all-covered float mask; parts 0..6); geom [B,8] int64 per image
+ * = { ul_x, ul_y, crop_h, crop_w, orig_h, orig_w, gt_offset, table_offset } where ul and crop = br - ul are uncrop's
+ * integers and the crop overlaps or touches the image; mask_gt / parts_gt: the ground-truth images, row-major
+ * [orig_h, orig_w] uint8 at gt_offset of one packed buffer each; tables: int32 workspace of sum(crop_h + crop_w)
+ * entries, image b's at table_offset; max_pixels: the largest orig_h * orig_w (it sizes the grid, <= INT32_MAX) ->
+ *   mask_conf [B,2,2] int64   pixel counts of (gt > 0, pred > 0)
+ *   part_conf [B,9,7] int64   pixel counts of (gt row, pred part): rows 0..6 the labels, 7 the label 255, 8 any other
+ *                             label; a predicted part past 6 is counted in no column
+ * The crop is resized like scipy.misc.imresize(interp='nearest') = Pillow's NEAREST (a sequential double recurrence
+ * per axis).  Integer counts: exact and repeatable. */
+int danet_seg_confusion(int32_t B, int32_t R, const uint8_t* mask, const uint8_t* parts, const int64_t* geom,
+                        const uint8_t* mask_gt, const uint8_t* parts_gt, int64_t max_pixels, int32_t* tables,
+                        int64_t* mask_conf, int64_t* part_conf, danet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Training targets (csrc/targets.cu).  No entry synchronises with the host, so a step's target
