@@ -84,6 +84,8 @@ SIGNATURES = {
     "danet_stn_kps_losses_workspace_bytes": (c_i64, [c_int, c_int]),
     "danet_stn_kps_losses": (c_int, [c_int, c_int, c_int, c_p, c_p, c_int, c_f, c_f, c_p, c_p, c_p, c_p, c_p]),
     "danet_part_iuv_targets": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_int, c_p, c_p]),
+    "danet_part_drop_clean_forward": (c_int, [c_int, c_int, c_int] + [c_p] * 16),
+    "danet_part_drop_clean_backward": (c_int, [c_int, c_int] + [c_p] * 11),
     "danet_raster_create": (c_int, [ctypes.POINTER(RasterDesc), ctypes.POINTER(c_p)]),
     "danet_raster_destroy": (c_int, [c_p]),
     "danet_raster_workspace_bytes": (c_i64, [c_p, c_int]),

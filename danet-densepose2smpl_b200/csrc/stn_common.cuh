@@ -30,6 +30,15 @@ __device__ __forceinline__ int argmax_first(const float* v, int n) {
     }
     return best;
 }
+// the same over n values `stride` floats apart
+__device__ __forceinline__ int argmax_first(const float* v, int n, size_t stride) {
+    int best = 0; float bv = v[0];
+    for (int c = 1; c < n; ++c) {
+        const float x = v[(size_t)c * stride];
+        if ((x > bv) || (x != x && bv == bv)) { bv = x; best = c; }
+    }
+    return best;
+}
 
 // fp32 product and sum rounded on their own: the device never contracts them into a fused multiply-add, so a host
 // restatement (which has no FMA either) sees the same values

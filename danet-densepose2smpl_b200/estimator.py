@@ -247,8 +247,25 @@ def iuv_estimator(model, image, iuv_image_gt=None, smpl_kps_gt=None, uvia_dp_gt=
                   center_noise=None, scale_noise=None, stn_hm_weight=None):
     """IUV_Estimator.forward (iuv_estimator.py:58-260) for INPUT_MODE='iuv', DECOMPOSED=True in model.training's mode.
     See the module docstring.  stn_hm_weight: cfg.DANET.STN_HM_WEIGHTS (default danet_b200.losses.STN_HM_WEIGHTS)."""
+    low, state, training, hm_w, noise = prepare_estimator("danet_b200.estimator.iuv_estimator", model, image,
+                                                          iuv_image_gt, smpl_kps_gt, uvia_dp_gt, has_iuv, has_dp,
+                                                          center_noise, scale_noise, stn_hm_weight)
+    ops = _cuda_ops()
+    pred = run_estimator(low, state, image.contiguous(), training, ops, noise)
+    ret = {"losses": {}, "uvia_pred": [pred[k] for k in HEADS], "part_iuv_pred": pred["part_pred"],
+           "stn_kps_pred": pred["centers"].detach(), "skps_hm_pred": pred["hm"].detach()}
+    if training:
+        ret["losses"], part_gt = estimator_losses(pred, ops, iuv_image_gt, smpl_kps_gt, uvia_dp_gt, has_iuv, has_dp,
+                                                  hm_w)
+        if part_gt is not None:
+            ret["part_iuv_gt"] = part_gt
+    return ret
+
+
+def prepare_estimator(where, model, image, iuv_image_gt, smpl_kps_gt, uvia_dp_gt, has_iuv, has_dp, center_noise,
+                      scale_noise, stn_hm_weight):
+    """iuv_estimator's argument checks and STN draws: (lowered ops, state, training, stn_hm_weight, noise)."""
     from . import losses
-    where = "danet_b200.estimator.iuv_estimator"
     graph = getattr(model, "graph", None)
     if graph is None:
         raise ValueError("%s: model must be a danet_b200.DaNet (it has no network graph)" % where)
@@ -301,13 +318,4 @@ def iuv_estimator(model, image, iuv_image_gt=None, smpl_kps_gt=None, uvia_dp_gt=
             scale_noise = sn.to(dev)
         elif center_noise is None and smpl_kps_gt is not None:
             center_noise = torch.rand(B, NUM_PARTS, 2).to(dev)
-    ops = _cuda_ops()
-    pred = run_estimator(low, state, image.contiguous(), training, ops, (center_noise, scale_noise))
-    ret = {"losses": {}, "uvia_pred": [pred[k] for k in HEADS], "part_iuv_pred": pred["part_pred"],
-           "stn_kps_pred": pred["centers"].detach(), "skps_hm_pred": pred["hm"].detach()}
-    if training:
-        ret["losses"], part_gt = estimator_losses(pred, ops, iuv_image_gt, smpl_kps_gt, uvia_dp_gt, has_iuv, has_dp,
-                                                  hm_w)
-        if part_gt is not None:
-            ret["part_iuv_gt"] = part_gt
-    return ret
+    return low, state, training, hm_w, (center_noise, scale_noise)

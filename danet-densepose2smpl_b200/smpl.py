@@ -381,13 +381,14 @@ class _SmplLbs(torch.autograd.Function):
 
 
 def smpl_losses(smpl, para, target, target_kps, target_kps3d, target_verts, has_kp3d, has_smpl, focal_length=5000.0,
-                img_size=224, openpose_weight=0.0, gt_weight=1.0, weights=None):
+                img_size=224, openpose_weight=0.0, gt_weight=1.0, weights=None, outputs=None):
     """The SMPL-branch losses of the reference's training step (models/danet/smpl_regressor.py:170-215 with the
     criteria of :224-330: keypoint 2D / 3D, per-vertex, pose / betas regression, camera) on top of the differentiable
     SMPL layer.  para / target [B,229] = cam 3 | betas 10 | 24 rotation matrices; target_kps [B,49,3] (x, y in [-1,1],
     confidence); target_kps3d [B,24,4]; target_verts [B,6890,3]; has_kp3d / has_smpl [B] masks.  Returns a dict of
     scalar losses (already multiplied by their weights); the loss arithmetic is plain torch on the GPU -- the SMPL
-    forward / backward underneath are the CUDA kernels."""
+    forward / backward underneath are the CUDA kernels.  A dict passed as `outputs` receives the predicted 'vertices'
+    [B,V,3] and 'cam_t' [B,3] (smpl_regressor.py:183-188), attached to the graph."""
     w = {"keypoints_2d": 300.0, "keypoints_3d": 300.0, "smpl_pose": 60.0, "smpl_betas": 0.06, "smpl_verts": 0.0}      # configs/danet_default.yaml:25-29
     if weights:
         w.update(weights)
@@ -396,6 +397,8 @@ def smpl_losses(smpl, para, target, target_kps, target_kps3d, target_verts, has_
     out = smpl(betas=betas, body_pose=rot[:, 1:], global_orient=rot[:, :1], pose2rot=False)
     verts, joints = out.vertices, out.joints
     cam_t = torch.stack([cam[:, 1], cam[:, 2], 2 * focal_length / (img_size * cam[:, 0] + 1e-9)], dim=-1)
+    if outputs is not None:
+        outputs.update(vertices=verts, cam_t=cam_t)
     pts = joints + cam_t.unsqueeze(1)                                       # rotation = identity, centre = 0
     kp2d = focal_length * pts[..., :2] / pts[..., 2:3] / (img_size / 2.0)
     conf = target_kps[:, :, -1:].clone()

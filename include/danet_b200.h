@@ -201,6 +201,31 @@ int danet_stn_kps_losses(int32_t B, int32_t J, int32_t S, const float* hm, const
 int danet_part_iuv_targets(int32_t B, int32_t S, int32_t C, const float* Umap, const float* Vmap, const float* Imap,
                            const float* theta, int32_t align_corners, float* out, danet_stream_t stream);
 
+/* Part dropout + iuvmap_clean of the estimator's outputs for training.  Replaces models/danet/danet.py:193-205 (drop
+ * the U / V / Index channels of the dropped DensePose parts), :247-283 (the same for the part crops' channels that
+ * dp2smpl_mapping maps to a dropped part, then iuvmap_clean per crop) and utils/iuvmap.py:6-38, with their autograd.
+ * u / v / index [B,25,S,S] and ann [B,Ca,S,S] contiguous; parts [B,24,3,7,S,S] read through part_strides[6]
+ * (elements); drop [B,24] uint8 (drop[b*24 + d-1] != 0: DensePose part d of image b is dropped) or NULL (no dropout
+ * stage); dp2smpl HOST [24,6] DensePose parts 1..24 of each crop's channels 1..6.  A dropped entry is multiplied by
+ * 0.0f (NaN and +-inf give NaN) and still takes part in the argmax (first maximum, NaN wins).  Outputs, contiguous:
+ * the cleaned u / v / index [B,25,S,S] and ann [B,Ca,S,S] and parts [B,24,3,7,S,S]: one-hot = 1 at the argmax, -0.0
+ * below it, +0.0 above it; U and V are products with it.  argmax_global [B,S*S] and argmax_parts [B,24,S*S] (one
+ * byte per pixel) are kept for the backward. */
+int danet_part_drop_clean_forward(int32_t B, int32_t S, int32_t Ca, const float* u, const float* v, const float* index,
+                                  const float* ann, const float* parts, const int64_t* part_strides, const uint8_t* drop,
+                                  const int8_t* dp2smpl, float* u_out, float* v_out, float* index_out, float* ann_out,
+                                  float* parts_out, uint8_t* argmax_global, uint8_t* argmax_parts,
+                                  danet_stream_t stream);
+/* Backward of danet_part_drop_clean_forward: bit for bit torch autograd of the reference's expressions.  grad_u /
+ * grad_v [B,25,S,S] = g * one-hot (times 0 where dropped; with a drop mask, +0.0 added, which turns -0.0 into +0.0, as
+ * the index_put_ of the dropout does); grad_parts [B,24,3,7,S,S] likewise for the U and V maps (+0.0 always added: the
+ * reference assembles it from per-crop slices) and +0.0 on the Index maps.  The one-hot of Index and Ann comes from an
+ * argmax: they get no gradient.  Same drop and dp2smpl as the forward; the gradients in and out are contiguous. */
+int danet_part_drop_clean_backward(int32_t B, int32_t S, const uint8_t* drop, const int8_t* dp2smpl,
+                                   const uint8_t* argmax_global, const uint8_t* argmax_parts, const float* grad_u_out,
+                                   const float* grad_v_out, const float* grad_parts_out, float* grad_u, float* grad_v,
+                                   float* grad_parts, danet_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * IUV rasteriser.  Replaces utils/renderer.py:207-298 (IUV_Renderer) and the third-party
  * neural_renderer forward pass it calls; optionally fuses utils/iuvmap.py:103-151 (iuv_img2map).
