@@ -9,7 +9,7 @@ from . import geometry, iuvmap  # noqa: F401
 from .danet import DaNet, build_synthetic_danet  # noqa: F401
 from . import synthetic  # noqa: F401
 from . import parallel, evaluate, losses, regressor, conv, layers, stn  # noqa: F401
-from . import targets, training  # noqa: F401
+from . import optim, targets, training  # noqa: F401
 from . import estimator  # noqa: F401
 from .estimator import iuv_estimator  # noqa: F401
 from .part_utils import PartRenderer  # noqa: F401

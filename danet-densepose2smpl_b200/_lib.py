@@ -86,6 +86,7 @@ SIGNATURES = {
     "danet_part_iuv_targets": (c_int, [c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_int, c_p, c_p]),
     "danet_part_drop_clean_forward": (c_int, [c_int, c_int, c_int] + [c_p] * 16),
     "danet_part_drop_clean_backward": (c_int, [c_int, c_int] + [c_p] * 11),
+    "danet_adam_step": (c_int, [c_int] + [c_p] * 5 + [ctypes.c_double] * 6 + [c_p]),
     "danet_raster_create": (c_int, [ctypes.POINTER(RasterDesc), ctypes.POINTER(c_p)]),
     "danet_raster_destroy": (c_int, [c_p]),
     "danet_raster_workspace_bytes": (c_i64, [c_p, c_int]),

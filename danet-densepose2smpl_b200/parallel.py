@@ -92,3 +92,39 @@ def all_reduce_gradients(tensors, group=None, bucket_bytes=64 << 20, average=Tru
             g.copy_(flat[off:off + n].view_as(g))
             off += n
     return len(buckets)
+
+
+def broadcast_buffers(tensors, group=None, src=0, bucket_bytes=64 << 20):
+    """Rank `src` (a rank of `group`)'s copy of `tensors` on every rank, in place: DistributedDataParallel's default
+    broadcast_buffers, which the training step uses for the BatchNorm running statistics and counters (each rank's
+    training-mode forward updates them from its own shard).  Tensors of one dtype and device are packed into flat
+    buckets of <= bucket_bytes (one tensor larger than that is a bucket of its own), as all_reduce_gradients packs
+    gradients.  Every rank must pass the same tensors in the
+    same order.  Returns the number of collectives issued (0 without a process group / with one rank)."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return 0
+    root = dist.get_global_rank(group, src) if group is not None else src
+    kinds = {}                                   # BatchNorm interleaves fp32 statistics and int64 counters
+    for t in tensors:
+        kinds.setdefault((t.dtype, t.device), []).append(t)
+    buckets = []
+    for ts in kinds.values():
+        cur, cur_bytes = [], 0
+        for t in ts:
+            nb = t.numel() * t.element_size()
+            if cur and cur_bytes + nb > bucket_bytes:
+                buckets.append(cur)
+                cur, cur_bytes = [], 0
+            cur.append(t)
+            cur_bytes += nb
+        if cur:
+            buckets.append(cur)
+    for b in buckets:
+        flat = torch.cat([t.reshape(-1) for t in b])
+        dist.broadcast(flat, src=root, group=group)
+        off = 0
+        for t in b:
+            n = t.numel()
+            t.copy_(flat[off:off + n].view_as(t))
+            off += n
+    return len(buckets)

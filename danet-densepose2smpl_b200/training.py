@@ -27,6 +27,9 @@ Returns the reference's four dicts: 'losses' (0-dim losses unsqueezed to [1], da
 'visualization' ('iuv_pred': the cleaned maps, detached; 'part_iuv_pred': the cleaned part maps) and 'prediction'
 ('cam', 'shape', 'pose', and in training mode 'vertices' and 'cam_t').
 
+`train_step` is the reference's whole training step around danet_forward: the learning-rate decay (`LRDecay`), the
+pretraining phase, prepare_targets, the loss sum, the backward, the gradient average over ranks and the optimizer step.
+
 `run_danet` walks the lowered estimator and regressor ops of the network graph (danet_b200.estimator.run_estimator,
 danet_b200.regressor.run_branch) on a state dictionary through an op table: `cuda_ops(model)` here, an fp64 torch table
 in the tests.  `danet_forward` checks the arguments, draws the noise and passes the model's state and the CUDA ops."""
@@ -34,6 +37,7 @@ import functools
 import types
 
 import torch
+import torch.distributed as dist
 
 from . import _args
 from .iuvmap import NUM_PARTS, PARTDROP_RATE
@@ -135,3 +139,91 @@ def danet_forward(model, in_dict, *, part_drop=None, center_noise=None, scale_no
     for branch in ("body", "limb"):
         state.update(_model_state(model, branch)[1])
     return run_danet(model.graph, state, in_dict, training, cuda_ops(model), part_drop, noise, rate, hm_w)
+
+
+BN_BUFFERS = ("running_mean", "running_var", "num_batches_tracked")
+
+
+class LRDecay:
+    """The reference's learning-rate decay (train/trainer.py:119-128, configs/danet_default.yaml SOLVER) as it is
+    written: decay_steps_ind starts at 1, and when step_count == steps[decay_steps_ind] every param group's lr becomes
+    param_groups[0]['lr'] * gamma and the index moves on.  A trainer that resumes builds a new one, so the index restarts
+    at 1 there too, as in the reference (where a resume past steps[1] therefore never decays again)."""
+
+    def __init__(self, steps=(0, 30000, 60000), gamma=0.1):
+        self.steps = tuple(int(s) for s in steps)
+        self.gamma = _args.number("danet_b200.training.LRDecay", "gamma", gamma)
+        self.decay_steps_ind = 1
+
+    def __call__(self, optimizer, step_count):
+        """Apply the rule for `step_count`; returns True when it decayed the learning rate."""
+        if self.decay_steps_ind < len(self.steps) and step_count == self.steps[self.decay_steps_ind]:
+            lr_new = optimizer.param_groups[0]["lr"] * self.gamma
+            for param_group in optimizer.param_groups:
+                param_group["lr"] = lr_new
+            self.decay_steps_ind += 1
+            return True
+        return False
+
+
+def train_step(model, optimizer, batch, opt_pose, opt_betas, step_count, *, schedule, pretr_step=5000, fit_valid=None,
+               part_drop=None, center_noise=None, scale_noise=None, partdrop_rate=PARTDROP_RATE, stn_hm_weight=None,
+               group=None):
+    """Trainer.train_step (train/trainer.py:117-244) on the GPU, in the reference's order:
+        1. schedule(optimizer, step_count) (the learning-rate decay, LRDecay); 2. model.train();
+        3. pretrain_mode = step_count <= pretr_step (train/base_trainer.py:70-74);
+        4. danet_b200.targets.prepare_targets(model, batch, opt_pose, opt_betas, fit_valid=) merged into the batch;
+        5. danet_forward; 6. loss_tatal, the sum of the losses from 0 in dict order; 7. optimizer.zero_grad();
+        8. loss_tatal.backward(); 9. with a process group of more than one rank, the gradient average
+           (parallel.all_reduce_gradients); 10. optimizer.step();
+        11. with more than one rank, rank 0's BatchNorm statistics and counters on every rank (parallel.broadcast_buffers),
+            so every rank ends the step with the same model, as DistributedDataParallel's broadcast_buffers gives.
+    batch: the data batch (prepare_targets' keys, 'img', 'pose_3d', 'has_pose_3d' and the estimator's optional
+    annotations; see danet_forward).  opt_pose / opt_betas / fit_valid: the fits the caller looked up (FitsDict).
+    part_drop / center_noise / scale_noise / partdrop_rate / stn_hm_weight: as in danet_forward.  optimizer: any
+    torch.optim optimizer (danet_b200.optim.Adam is the reference's Adam in one pass).
+
+    Returns the reference's (output, losses): output 'pred_vertices', 'opt_vertices', 'pred_cam_t', 'opt_cam_t'
+    (the prediction entries None in pretraining mode) and 'visualization'; losses 'loss_<key>' and 'loss_tatal' as
+    detached device tensors, so that the step never waits for the GPU (call .item() where the values are logged)."""
+    from .parallel import all_reduce_gradients, broadcast_buffers
+    from .targets import prepare_targets
+    where = "danet_b200.training.train_step"
+    if not isinstance(optimizer, torch.optim.Optimizer):
+        raise ValueError("%s: optimizer must be a torch.optim.Optimizer (got %s)" % (where, type(optimizer).__name__))
+    if not callable(schedule):
+        raise ValueError("%s: schedule must be callable as schedule(optimizer, step_count) (e.g. LRDecay())" % where)
+    if not isinstance(batch, dict) or "img" not in batch:
+        raise ValueError("%s: batch must be a dict with 'img'" % where)
+    for name, v in (("step_count", step_count), ("pretr_step", pretr_step)):
+        if isinstance(v, bool) or not isinstance(v, int):
+            raise ValueError("%s: %s must be an int (got %r)" % (where, name, v))
+    schedule(optimizer, step_count)
+    model.train()
+    in_dict = dict(batch)
+    in_dict["pretrain_mode"] = step_count <= pretr_step
+    targets = prepare_targets(model, batch, opt_pose, opt_betas, fit_valid=fit_valid)
+    in_dict.update(targets)
+    ret = danet_forward(model, in_dict, part_drop=part_drop, center_noise=center_noise, scale_noise=scale_noise,
+                        partdrop_rate=partdrop_rate, stn_hm_weight=stn_hm_weight)
+    loss_tatal = 0
+    losses = {}
+    for k, v in ret["losses"].items():
+        loss_tatal += v
+        losses["loss_%s" % k] = v.detach()
+    optimizer.zero_grad()
+    loss_tatal.backward()
+    ranks = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+    if ranks > 1:
+        all_reduce_gradients(model.parameters(), group)
+    optimizer.step()
+    if ranks > 1:
+        broadcast_buffers([b for n, b in model.named_buffers() if n.endswith(BN_BUFFERS)], group)
+    pretrain = in_dict["pretrain_mode"]
+    output = {"pred_vertices": None if pretrain else ret["prediction"]["vertices"].detach(),
+              "opt_vertices": targets["target_verts"],
+              "pred_cam_t": None if pretrain else ret["prediction"]["cam_t"].detach(),
+              "opt_cam_t": targets["opt_cam_t"],
+              "visualization": ret["visualization"]}
+    losses["loss_tatal"] = loss_tatal.detach()
+    return output, losses

@@ -227,6 +227,22 @@ int danet_part_drop_clean_backward(int32_t B, int32_t S, const uint8_t* drop, co
                                    float* grad_parts, danet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Optimizer.  Replaces train/trainer.py:42-44's torch.optim.Adam(lr, weight_decay=0) step (torch's CUDA default,
+ * _multi_tensor_adam with capturable=False, amsgrad=False, maximize=False) bit for bit, in one pass.
+ * ------------------------------------------------------------------------------------------ */
+/* One Adam step of `count` fp32 tensors that share one step count and one set of hyper-parameters.  params, grads,
+ * exp_avgs, exp_avg_sqs and numels are HOST arrays of `count` device pointers / element counts (contiguous tensors;
+ * 16-byte aligned ones take vector accesses, the bits do not depend on it).  The scalars are torch's doubles for step t:
+ * lerp_weight = 1 - beta1, one_minus_beta2 = 1 - beta2, bias_correction2_sqrt = (1 - beta2**t) ** 0.5,
+ * step_size = (lr / (1 - beta1**t)) * -1; each is rounded to fp32 as torch's kernels round them.  Per element:
+ * m = lerp(m, g, w1); v = v * beta2; v = fma(c2, g * g, v); p = fma(s, m / (sqrt(v) / bc2 + eps), p).  Long lists are
+ * split into several launches; no host synchronisation, no copies. */
+int danet_adam_step(int32_t count, float* const* params, const float* const* grads, float* const* exp_avgs,
+                    float* const* exp_avg_sqs, const int64_t* numels, double lerp_weight, double beta2,
+                    double one_minus_beta2, double bias_correction2_sqrt, double eps, double step_size,
+                    danet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * IUV rasteriser.  Replaces utils/renderer.py:207-298 (IUV_Renderer) and the third-party
  * neural_renderer forward pass it calls; optionally fuses utils/iuvmap.py:103-151 (iuv_img2map).
  * ------------------------------------------------------------------------------------------ */
