@@ -981,6 +981,9 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
     DANET_CHECK(pose_kind >= 0 && pose_kind <= 2, "danet_smpl_forward: bad pose_kind %d", pose_kind);
     DANET_CHECK(verts || !(joints || smpl_joints || joints_h36m),
                 "danet_smpl_forward: joint outputs need the verts buffer (picked vertices are read from it)");
+    DANET_CHECK(bodies_per_cta == -1 || bodies_per_cta == 0 || bodies_per_cta == 1 || bodies_per_cta == 2 ||
+                bodies_per_cta == 4 || bodies_per_cta == 8 || bodies_per_cta == 16,
+                "danet_smpl_forward: bodies_per_cta must be -1, 0, 1, 2, 4, 8 or 16 (got %d)", bodies_per_cta);
     cudaStream_t stream = (cudaStream_t)stream_;
     const SmplView& m = h->v;
     const SmplFwdWs ws(h, B, bodies_per_cta, workspace);
@@ -988,13 +991,14 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
     DANET_LAUNCH_CHECK();
     int nb = bodies_per_cta;
     if (nb <= 0) nb = B >= 32 ? 8 : (B >= 4 ? 4 : (B >= 2 ? 2 : 1));      // tools/lbs_sweep.py sweeps it
-    const size_t smem = (size_t)nb * (kPF + kJ * 12 + kTileC + kMaxBetas) * sizeof(float);
+    // shared memory is sized from the blocking a launch instantiates: the GEMM route's fallback always runs 8 bodies
+    // per CTA, whatever the caller's bodies_per_cta
 #define DANET_LBS_LAUNCH(NBV, Bc, off, VP)                                                          \
     do {                                                                                            \
+        const size_t smem = (size_t)NBV * (kPF + kJ * 12 + kTileC + kMaxBetas) * sizeof(float);     \
         static unsigned long long attr_devs = 0;                                                    \
         if (first_use_on_current_device(&attr_devs) != 0) {                                         \
-            DANET_CUDA(cudaFuncSetAttribute(k_smpl_verts<NBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                            (int)((size_t)NBV * (kPF + kJ * 12 + kTileC + kMaxBetas) * sizeof(float)))); \
+            DANET_CUDA(cudaFuncSetAttribute(k_smpl_verts<NBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
         }                                                                                           \
         dim3 grid(m.ntiles, cdiv(Bc, NBV));                                                         \
         k_smpl_verts<NBV><<<grid, kTileV, smem, stream>>>(Bc, betas + (size_t)(off) * m.nbetas, ws.pf + (size_t)(off) * kPF, \
@@ -1030,8 +1034,7 @@ extern "C" int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas,
             case 2:  DANET_LBS_LAUNCH(2, B, 0, nullptr); break;
             case 4:  DANET_LBS_LAUNCH(4, B, 0, nullptr); break;
             case 8:  DANET_LBS_LAUNCH(8, B, 0, nullptr); break;
-            case 16: DANET_LBS_LAUNCH(16, B, 0, nullptr); break;
-            default: DANET_CHECK(false, "danet_smpl_forward: bodies_per_cta must be 0,1,2,4,8,16 (got %d)", nb);
+            case 16: DANET_LBS_LAUNCH(16, B, 0, nullptr); break;        // no other value passes the check on entry
         }
         DANET_LAUNCH_CHECK();
     }

@@ -64,7 +64,10 @@ int danet_smpl_destroy(danet_smpl_t h);
 int64_t danet_smpl_workspace_bytes(danet_smpl_t h, int32_t B);
 /* outputs may be NULL to skip: verts [B,V,3]; joints [B,num_out_joints,3];
  * smpl_joints [B,J,3]; joints_h36m [B,num_h36m,3]; rotmats [B,J,3,3].
- * `bodies_per_cta` 0 = auto (tuning knob: 1,2,4,8,16). */
+ * Batches of 512 bodies or more take the tensor-core route (the blend shapes as a split-fp16 GEMM), smaller ones the
+ * fused fp32 route.  `bodies_per_cta` is the fused route's blocking: 0 = auto, 1, 2, 4, 8 or 16 bodies per CTA; it
+ * does not apply on the tensor-core route.  -1 forces the fused route at any B, with the automatic blocking.  Any other
+ * value is refused before anything is launched, as are joint outputs without verts. */
 int danet_smpl_forward(danet_smpl_t h, int32_t B, const float* betas, const float* pose,
                        int32_t pose_kind, float* verts, float* joints, float* smpl_joints,
                        float* joints_h36m, float* rotmats, void* workspace,
