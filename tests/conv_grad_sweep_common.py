@@ -22,9 +22,9 @@ import math
 import torch
 import torch.nn.functional as F
 
-U = 2.0 ** -22
-U_OUT = 2.0 ** -24
-TINY = 2.0 ** -149
+import fp64_bound as fb
+
+U_SPLIT = 2.0 ** -22
 
 # the 18 network convolutions of body_net, limb_net, limb_reslayer and two HRNet shapes:
 # (name, cin, cout, H, k, stride, groups), channel counts per group, square maps
@@ -139,11 +139,11 @@ def wgrad_geo(case):
 
 
 def _classes():
-    """[(name, predicate(case, geo))]"""
+    """[(name, predicate((case, geo)))]"""
     cl = []
 
     def add(name, fn):
-        cl.append((name, fn))
+        cl.append((name, lambda cg: fn(*cg)))
 
     # filter x stride x map parity; a non-square map for every (k, s)
     for k, s in ((1, 1), (3, 1), (1, 2), (3, 2), (7, 2)):
@@ -206,8 +206,7 @@ CLASSES = _classes()
 def coverage(cases=None):
     """{class name: [indices of the cases in it]}"""
     cases = CASES if cases is None else cases
-    geos = [wgrad_geo(c) for c in cases]
-    return {name: [i for i, (c, g) in enumerate(zip(cases, geos)) if fn(c, g)] for name, fn in CLASSES}
+    return fb.coverage([(c, wgrad_geo(c)) for c in cases], CLASSES)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -277,25 +276,15 @@ def bounds(case, x, w, b, dy):
     A = op.C(ax, aw)
     if b is not None:
         A = A + b.double().abs()[None, :, None, None]
-    out = {"y": U * A + fx * op.C(ox, aw) + fw * op.C(ax, ow),
-           "dx": U * op.Ct(ady, aw) + fdy * op.Ct(ody, aw) + fw * op.Ct(ady, ow),
-           "dW": U * op.Wg(ax, ady) + fdy * op.Wg(ax, ody) + fx * op.Wg(ox, ady)}
+    out = {"y": U_SPLIT * A + fx * op.C(ox, aw) + fw * op.C(ax, ow),
+           "dx": U_SPLIT * op.Ct(ady, aw) + fdy * op.Ct(ody, aw) + fw * op.Ct(ady, ow),
+           "dW": U_SPLIT * op.Wg(ax, ady) + fdy * op.Wg(ax, ody) + fx * op.Wg(ox, ady)}
     res = {}
     for name in ("y", "dx", "dW"):
-        res[name] = (r[name], out[name], U_OUT * r[name].abs() + TINY)
+        res[name] = (r[name], out[name], fb.U24 * r[name].abs() + fb.TINY)
     if b is not None:
-        res["db"] = (r["db"], torch.zeros_like(r["db"]), U_OUT * r["db"].abs() + 2.0 ** -50 * ady.sum(dim=(0, 2, 3)))
+        res["db"] = (r["db"], torch.zeros_like(r["db"]), fb.U24 * r["db"].abs() + 2.0 ** -50 * ady.sum(dim=(0, 2, 3)))
     return res
-
-
-def worst_ratio(got, r, base, floor):
-    """max over the elements of (|got - r| - floor) / base (<= c passes; -inf where nothing is off), and its index.
-    Elements with base = 0 (db) count as infinitely off when they exceed the floor."""
-    excess = (got.double() - r).abs() - floor
-    q = torch.where(excess <= 0, torch.full_like(excess, -math.inf), excess / base)
-    q = torch.where(torch.isnan(q), torch.full_like(q, math.inf), q)
-    i = int(q.argmax())
-    return float(q.flatten()[i]), tuple(int(v) for v in torch.unravel_index(torch.tensor(i), q.shape))
 
 
 # operand magnitudes (x * 2^ex, w * 2^ew, dy * 2^edy; the bias follows y's magnitude 2^(ex + ew)): every fp64 reference

@@ -12,6 +12,8 @@ swizzle (those widths are chosen only for Cin <= 32, one chunk), and a last chun
 at those widths (a chunk is one or two K steps and Cin fills all but the last 8 channels of them)."""
 import ctypes
 
+import fp64_bound as fb
+
 # N, H, W, Cin, Cout, k, stride, wsets, relu, residual (none | f32 | planes), output (f32 | planes | both), bias, precision
 CASES = [
     (2, 12, 10, 16, 16, 1, 1, 1, 0, "none", "f32", 0, "fast"),  # fast NT 16 full
@@ -194,11 +196,11 @@ def report(case):
 
 
 def _classes():
-    """[(name, predicate(case, report))]"""
+    """[(name, predicate((case, report)))]"""
     cl = []
 
     def add(name, fn):
-        cl.append((name, fn))
+        cl.append((name, lambda cr: fn(*cr)))
 
     def prec(p):
         return lambda c: c[12] == p
@@ -285,5 +287,4 @@ CLASSES = _classes()
 def coverage(cases=None):
     """{class name: [indices of the cases in it]}"""
     cases = CASES if cases is None else cases
-    reps = [report(c) for c in cases]
-    return {name: [i for i, (c, r) in enumerate(zip(cases, reps)) if fn(c, r)] for name, fn in CLASSES}
+    return fb.coverage([(c, report(c)) for c in cases], CLASSES)

@@ -16,7 +16,8 @@ The bound: each element of a stage output against its fp64 reference r,
     |got - r| <= C * 2^-24 * M + 2^-24 * |r| + tiny
 
 M is the element's magnitude, computed from absolute values; C is the longest chain of rounded fp32 operations a term
-of the result passes through in the kernel; 2^-24 |r| is the final rounding; tiny = C * 2^-139 is the subnormal floor.
+of the result passes through in the kernel; 2^-24 |r| is the final rounding; tiny = C * 2^-139 is the subnormal floor
+(TINY_HEAD).
 
     k_adj_fwd      M = I + mask * relu(E): 2.  d = 1 / sqrt(colsum): 23 adds, sqrt, divide, and its relative error
                    amplified by sum |M| / |sum M|: held relatively.  A_hat = d_i M_ij d_j: 2.
@@ -62,11 +63,13 @@ import os
 import numpy as np
 import torch
 
+import fp64_bound as fb
 from oracle import gcn_head as og
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-U = 2.0 ** -24
-TINY = 2.0 ** -139
+# the head's own subnormal floor per rounded operation, 2^10 TINY: a rounding in fp32's subnormal range (TINY) can be
+# scaled up by a later factor of its chain, such as invstd <= eps^-1/2 < 2^9 in the BatchNorm kernels
+TINY_HEAD = 2.0 ** 10 * fb.TINY
 EPS, MOM = 1e-5, 0.1
 KDI = [128, 128, 256, 256, 128]
 KDO = [128, 256, 256, 128, 128]
@@ -188,10 +191,6 @@ def _classes():
 
 
 CLASSES = _classes()
-
-
-def uncovered():
-    return [name for name, fn in CLASSES if not any(fn(c) for c in CASES)]
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -637,53 +636,23 @@ def stages(c, inp, got=None, device="cpu", dtype=torch.float64, defect=None):
 # ----------------------------------------------------------------------------------------------------------------------
 # the bound
 # ----------------------------------------------------------------------------------------------------------------------
-def excess(got, st):
-    """max over the elements of (|got - r| - 2^-24 |r| - tiny) / (2^-24 M), the quantity held to <= C ('abs') or 1
-    ('rel', where M already holds C r); +inf where finiteness differs or an exact result is off; -inf when every element
-    is within the floor"""
-    r = st.r
-    g = got.to(r.device, torch.float64).reshape(r.shape)
-    fin = torch.isfinite(r)
-    if not torch.equal(fin, torch.isfinite(g)):
-        return math.inf
+def bound(st):
+    """(scale, floor, limit) of a stage for fp64_bound.worst: an 'abs' stage passes at C units of 2^-24 M, a 'rel' one
+    (M already holds C r) at 1, and an 'exact' one only at equality"""
     if st.kind == "exact":
-        same = (g == r) | (torch.isnan(g) & torch.isnan(r))
-        return -math.inf if bool(same.all()) else math.inf
-    M = st.M.reshape(r.shape)
-    floor = U * r.abs() + TINY * max(st.C, 1)
-    e = ((g - r).abs() - floor)[fin]
-    if e.numel() == 0:
-        return -math.inf
-    q = torch.where(e <= 0, torch.full_like(e, -math.inf), e / (U * M[fin]))
-    q = torch.where(torch.isnan(q), torch.full_like(q, math.inf), q)
-    return float(q.max())
-
-
-def limit(st):
-    return 1.0 if st.kind == "rel" else float(st.C)
-
-
-def ratio(got, st):
-    """the worst |got - r| / (2^-24 M) over the finite elements, what the sweep prints"""
-    if st.kind == "exact":
-        return 0.0
-    r, M = st.r, st.M.reshape(st.r.shape)
-    g = got.to(r.device, torch.float64).reshape(r.shape)
-    fin = torch.isfinite(r) & torch.isfinite(g)
-    e = (g - r).abs()[fin]
-    if e.numel() == 0:
-        return 0.0
-    q = torch.where(e == 0, torch.zeros_like(e), e / (U * M[fin]))
-    return float(q.max())
+        return 0.0, 0.0, 0.0
+    scale, floor = fb.U24 * st.M.reshape(st.r.shape), fb.U24 * st.r.abs() + TINY_HEAD * max(st.C, 1)
+    return scale, floor, 1.0 if st.kind == "rel" else float(st.C)
 
 
 def check(got, S, skip=()):
-    """[(stage, excess, limit)] of the failing stages"""
+    """[(stage, worst, limit)] of the failing stages"""
     bad = []
     for name, st in S.items():
         if name.startswith("_") or name in skip or name not in got:
             continue
-        x = excess(got[name], st)
-        if not x <= limit(st):
-            bad.append((name, x, limit(st)))
+        scale, floor, lim = bound(st)
+        q = fb.worst(got[name], st.r, scale, floor)[0]
+        if not q <= lim:
+            bad.append((name, q, lim))
     return bad

@@ -46,8 +46,7 @@ import math
 import torch
 import torch.nn.functional as F
 
-U = 2.0 ** -24
-TINY = 2.0 ** -149
+from fp64_bound import TINY
 MOM, EPS = 0.1, 1e-5
 
 C_BN_Y = 6
@@ -512,43 +511,8 @@ def relu_mask(y):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# coverage and the bound
+# coverage
 # ----------------------------------------------------------------------------------------------------------------------
 TABLES = {"batch_norm": (BN_CASES, BN_CLASSES), "max_pool2d": (POOL_CASES, POOL_CLASSES),
           "adaptive_avg_pool2d": (AVG_CASES, AVG_CLASSES), "linear": (LIN_CASES, LIN_CLASSES),
           "hr_fuse": (FUSE_CASES, FUSE_CLASSES)}
-
-
-def uncovered():
-    """names of the classes no case of their table is in"""
-    return ["%s: %s" % (op, name) for op, (cases, classes) in TABLES.items() for name, fn in classes
-            if not any(fn(c) for c in cases)]
-
-
-def worst_ratio(got, r, M, C, tiny=TINY):
-    """max over the finite elements of (|got - r| - 2^-24 |r| - tiny) / (2^-24 M) (-inf where every element is within
-    the floor); the test passes when it is <= C.  Where r is not finite, got must be non-finite (+inf otherwise), and
-    where r is finite got must be too."""
-    r, M = r.double(), M.double()
-    g = got.to(r.device).double()
-    fin = torch.isfinite(r)
-    if not torch.equal(fin, torch.isfinite(g)):
-        return math.inf
-    tiny = torch.as_tensor(tiny, dtype=torch.float64, device=r.device)
-    excess = ((g - r).abs() - (U * r.abs() + tiny))[fin]
-    if excess.numel() == 0:
-        return -math.inf
-    q = torch.where(excess <= 0, torch.full_like(excess, -math.inf), excess / (U * M[fin]))
-    q = torch.where(torch.isnan(q), torch.full_like(q, math.inf), q)
-    return float(q.max())
-
-
-def err_ratio(got, r, M):
-    """the worst |got - r| / (2^-24 M) over the finite elements (0 where both are 0), what the sweep prints"""
-    r, M = r.double(), M.double()
-    fin = torch.isfinite(r) & torch.isfinite(got.to(r.device).double())
-    e = (got.to(r.device).double() - r).abs()[fin]
-    if e.numel() == 0:
-        return 0.0
-    q = torch.where(e == 0, torch.zeros_like(e), e / (U * M[fin]))
-    return float(q.max())

@@ -60,8 +60,8 @@ import zlib
 import numpy as np
 import torch
 
-U = 2.0 ** -24
-TINY = 2.0 ** -149
+import fp64_bound as fb
+from fp64_bound import TINY, U24
 EXP_ULP = 2
 C_SL1_G = 2
 C_CE_G = EXP_ULP + 4
@@ -93,24 +93,11 @@ def block_threads(total):
     return 256 if total >= 132 * 2048 * 2 else (128 if total >= 132 * 2048 // 2 else 64)
 
 
-def worst_ratio(got, r, M, C, name="", tiny=TINY):
-    """max over finite r of |got - r| / bound (<= 1 passes); NaN r must be NaN, +-inf r must be equal and finite r
-    finite.  Returns the worst ratio of |got - r| to C * 2^-24 * M + 2^-24 |r| + tiny."""
-    got = torch.as_tensor(got).to(F64).cpu()
-    r = torch.as_tensor(r).to(F64).cpu()
-    M = torch.as_tensor(M).to(F64).cpu().expand_as(r)
-    C = torch.as_tensor(C, dtype=F64).cpu().expand_as(r)
-    nan = torch.isnan(r)
-    assert bool(torch.isnan(got[nan]).all()), "%s: %d NaN references not NaN" % (name, int((~torch.isnan(got[nan])).sum()))
-    inf = torch.isinf(r)
-    assert bool((got[inf] == r[inf]).all()), "%s: infinite references differ" % name
-    fin = torch.isfinite(r)
-    bad = fin & ~torch.isfinite(got)
-    assert not bool(bad.any()), "%s: %d non-finite results where the reference is finite" % (name, int(bad.sum()))
-    if not bool(fin.any()):
-        return 0.0
-    bound = C * U * M + U * r.abs() + (C + 1) * tiny
-    return float(((got - r).abs() / bound)[fin].max())
+def bound(r, M, C):
+    """(scale, floor) of the bound C 2^-24 M + 2^-24 |r| + (C + 1) 2^-149 for fp64_bound.worst, which passes at <= 1:
+    C differs from element to element here, so it goes into the scale"""
+    C = torch.as_tensor(C, dtype=F64, device=r.device)
+    return C * U24 * torch.as_tensor(M, dtype=F64, device=r.device), U24 * r.abs() + (C + 1) * TINY
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -769,7 +756,7 @@ def part_reference(c, p, dt=F64, defect=None):
     isum64 = Isel.to(F64).sum(2)
     bg = (isum32 < 0.5).to(F64)
     flips = (isum32 < 0.5) != (isum64 < 0.5)
-    worst = float(((isum64 - 0.5).abs() / (5 * U * Isel.to(F64).abs().sum(2) + TINY))[flips].max()) if bool(flips.any()) else 0.0
+    worst = float(((isum64 - 0.5).abs() / (5 * U24 * Isel.to(F64).abs().sum(2) + TINY))[flips].max()) if bool(flips.any()) else 0.0
     src = [Um[:, mp].to(F64), Vm[:, mp].to(F64), Isel.to(F64)]
     for k, inb, q in taps(x0, y0, S):
         w = torch.where(inb, fw[k], torch.zeros((), dtype=F64))                # [B,24,HW]
@@ -787,55 +774,55 @@ def part_reference(c, p, dt=F64, defect=None):
 # ----------------------------------------------------------------------------------------------------------------------
 # coverage
 # ----------------------------------------------------------------------------------------------------------------------
-def coverage():
-    """{class: number of cases in it}; every class needs at least one"""
-    b, d, s, q = BODY_CASES, DP_CASES, STN_CASES, PART_CASES
+def _classes():
+    """[(name, predicate)] over CASES: each table's classes see only that table's cases"""
+    b, d, s, q = [], [], [], []
     hw = lambda c: c.N * c.H * c.W
-    cls = {
-        "body N*HW = 135167": [c for c in b if hw(c) == 135167], "body N*HW = 135168": [c for c in b if hw(c) == 135168],
-        "body N*HW = 540671": [c for c in b if hw(c) == 540671], "body N*HW = 540672": [c for c in b if hw(c) == 540672],
-        "body B = 64 global heads": [c for c in b if c.N == 64 and c.C == 25 and c.H == 56 and c.Cann == 15],
-        "body 128-thread block": [c for c in b if block_threads(hw(c)) == 128],
-        "body C = 1": [c for c in b if c.C == 1], "body C = 7": [c for c in b if c.C == 7],
-        "body C = 25": [c for c in b if c.C == 25], "body ann absent": [c for c in b if not c.Cann],
-        "body Cann = 1": [c for c in b if c.Cann == 1], "body Cann = 15": [c for c in b if c.Cann == 15],
-        "body strided rows": [c for c in b if c.pad or c.part], "body part layout": [c for c in b if c.part],
-        **{"body has %s" % h: [c for c in b if c.has == h] for h in ("none", "all", "some", "one", "zero")},
-        "body soft I": [c for c in b if c.I == "soft"], "body one-hot I": [c for c in b if c.I == "onehot"],
-        "body target ties": [c for c in b if c.I == "tie"],
-        **{"body logits 2^%d" % e: [c for c in b if c.scale == e] for e in (0, 4, 10)},
-        "body logit offset 2^14": [c for c in b if c.offset],
-        "body NaN predictions": [c for c in b if c.nonfinite == "nan"],
-        "body +-inf predictions": [c for c in b if c.nonfinite == "inf"],
-        "body leading -inf": [c for c in b if c.nonfinite == "lead_ninf"],
-        "body all-NaN target pixel": [c for c in b if c.nonfinite == "tgt_nan"],
-        "body all--inf target pixel": [c for c in b if c.nonfinite == "tgt_ninf"],
-        **{"dp P = %d" % P: [c for c in d if c.P == P] for P in (1, 31, 196, 256)},
-        "dp HW < 256": [c for c in d if c.S * c.S < 256], "dp HW % 256 != 0, > 256": [c for c in d if c.S * c.S > 256 and c.S * c.S % 256],
-        "dp points on pixel centres": [c for c in d if c.pts in ("centre", "mixed", "pile") and not c.align],
-        "dp last row / column, align False": [c for c in d if c.pts in ("edge", "mixed") and not c.align],
-        "dp last row / column, align True": [c for c in d if c.pts in ("edge", "mixed") and c.align],
-        "dp points outside": [c for c in d if c.pts in ("outside", "mixed")],
-        "dp 256 points on one pixel": [c for c in d if c.pts == "pile" and c.P == 256],
-        "dp point weights 0 / 1 / 2": list(d), "dp fractional labels, 0 and 24": list(d),
-        **{"dp has %s" % h: [c for c in d if c.has == h] for h in ("none", "all", "some", "one", "zero")},
-        "dp Cann = 1": [c for c in d if c.Cann == 1],
-        **{"dp %s" % k: [c for c in d if c.nonfinite == k] for k in ("nan", "inf", "lead_ninf", "coords")},
-        "stn HW < 256": [c for c in s if c.S * c.S < 256], "stn HW > 256": [c for c in s if c.S * c.S > 256],
-        "stn kps_cols 2": [c for c in s if c.cols == 2], "stn kps_cols 3": [c for c in s if c.cols == 3],
-        "stn kps_weight 0": [c for c in s if c.kw == 0 and c.cols == 3], "stn hm_weight 0": [c for c in s if c.hw == 0],
-        "stn joints on / left of / far outside the border": list(s),
-        **{"stn hm %s" % k: [c for c in s if c.hm == k] for k in ("peaked", "const", "offset")},
-        **{"stn %s hm" % k: [c for c in s if c.nonfinite == k] for k in ("nan", "inf", "ninf")},
-        "stn grad_roi == grad_hm": [c for c in s if c.alias],
-        "part S = 2": [c for c in q if c.S == 2], "part S = 56": [c for c in q if c.S == 56],
-        "part align False": [c for c in q if not c.align], "part align True": [c for c in q if c.align],
-        "part general theta": [c for c in q if c.theta == "general"], "part scale 0": [c for c in q if c.theta == "zero"],
-        "part negative scales": [c for c in q if c.theta == "neg"], "part all outside": [c for c in q if c.theta == "out"],
-        "part sum I at 0.5 and one ulp off": [c for c in q if c.half],
-    }
-    for sub in ("u", "v", "i", "a", "uv", "ia", "uia", "va", ""):
-        cls["body needs-grad '%s'" % sub] = [c for c in b if c.need == sub]
-    for sub in ("u", "v", "i", "a", "uv", "ia", "uia", ""):
-        cls["dp needs-grad '%s'" % sub] = [c for c in d if c.need == sub]
-    return {k: len(v) for k, v in cls.items()}
+    b += [("body N*HW = %d" % n, lambda c, n=n: hw(c) == n) for n in (135167, 135168, 540671, 540672)]
+    b += [("body B = 64 global heads", lambda c: c.N == 64 and c.C == 25 and c.H == 56 and c.Cann == 15),
+          ("body 128-thread block", lambda c: block_threads(hw(c)) == 128),
+          ("body C = 1", lambda c: c.C == 1), ("body C = 7", lambda c: c.C == 7),
+          ("body C = 25", lambda c: c.C == 25), ("body ann absent", lambda c: not c.Cann),
+          ("body Cann = 1", lambda c: c.Cann == 1), ("body Cann = 15", lambda c: c.Cann == 15),
+          ("body strided rows", lambda c: c.pad or c.part), ("body part layout", lambda c: c.part)]
+    b += [("body has %s" % h, lambda c, h=h: c.has == h) for h in ("none", "all", "some", "one", "zero")]
+    b += [("body soft I", lambda c: c.I == "soft"), ("body one-hot I", lambda c: c.I == "onehot"),
+          ("body target ties", lambda c: c.I == "tie")]
+    b += [("body logits 2^%d" % e, lambda c, e=e: c.scale == e) for e in (0, 4, 10)]
+    b += [("body logit offset 2^14", lambda c: c.offset),
+          ("body NaN predictions", lambda c: c.nonfinite == "nan"),
+          ("body +-inf predictions", lambda c: c.nonfinite == "inf"),
+          ("body leading -inf", lambda c: c.nonfinite == "lead_ninf"),
+          ("body all-NaN target pixel", lambda c: c.nonfinite == "tgt_nan"),
+          ("body all--inf target pixel", lambda c: c.nonfinite == "tgt_ninf")]
+    d += [("dp P = %d" % P, lambda c, P=P: c.P == P) for P in (1, 31, 196, 256)]
+    d += [("dp HW < 256", lambda c: c.S * c.S < 256), ("dp HW % 256 != 0, > 256", lambda c: c.S * c.S > 256 and c.S * c.S % 256),
+          ("dp points on pixel centres", lambda c: c.pts in ("centre", "mixed", "pile") and not c.align),
+          ("dp last row / column, align False", lambda c: c.pts in ("edge", "mixed") and not c.align),
+          ("dp last row / column, align True", lambda c: c.pts in ("edge", "mixed") and c.align),
+          ("dp points outside", lambda c: c.pts in ("outside", "mixed")),
+          ("dp 256 points on one pixel", lambda c: c.pts == "pile" and c.P == 256),
+          ("dp point weights 0 / 1 / 2", lambda c: True), ("dp fractional labels, 0 and 24", lambda c: True)]
+    d += [("dp has %s" % h, lambda c, h=h: c.has == h) for h in ("none", "all", "some", "one", "zero")]
+    d += [("dp Cann = 1", lambda c: c.Cann == 1)]
+    d += [("dp %s" % k, lambda c, k=k: c.nonfinite == k) for k in ("nan", "inf", "lead_ninf", "coords")]
+    s += [("stn HW < 256", lambda c: c.S * c.S < 256), ("stn HW > 256", lambda c: c.S * c.S > 256),
+          ("stn kps_cols 2", lambda c: c.cols == 2), ("stn kps_cols 3", lambda c: c.cols == 3),
+          ("stn kps_weight 0", lambda c: c.kw == 0 and c.cols == 3), ("stn hm_weight 0", lambda c: c.hw == 0),
+          ("stn joints on / left of / far outside the border", lambda c: True)]
+    s += [("stn hm %s" % k, lambda c, k=k: c.hm == k) for k in ("peaked", "const", "offset")]
+    s += [("stn %s hm" % k, lambda c, k=k: c.nonfinite == k) for k in ("nan", "inf", "ninf")]
+    s += [("stn grad_roi == grad_hm", lambda c: c.alias)]
+    q += [("part S = 2", lambda c: c.S == 2), ("part S = 56", lambda c: c.S == 56),
+          ("part align False", lambda c: not c.align), ("part align True", lambda c: c.align),
+          ("part general theta", lambda c: c.theta == "general"), ("part scale 0", lambda c: c.theta == "zero"),
+          ("part negative scales", lambda c: c.theta == "neg"), ("part all outside", lambda c: c.theta == "out"),
+          ("part sum I at 0.5 and one ulp off", lambda c: c.half)]
+    b += [("body needs-grad '%s'" % n, lambda c, n=n: c.need == n) for n in ("u", "v", "i", "a", "uv", "ia", "uia", "va", "")]
+    d += [("dp needs-grad '%s'" % n, lambda c, n=n: c.need == n) for n in ("u", "v", "i", "a", "uv", "ia", "uia", "")]
+    return [(name, lambda c, t=t, fn=fn: type(c) is t and fn(c))
+            for t, cl in ((Body, b), (Dp, d), (Stn, s), (Part, q)) for name, fn in cl]
+
+
+CASES = BODY_CASES + DP_CASES + STN_CASES + PART_CASES
+CLASSES = _classes()

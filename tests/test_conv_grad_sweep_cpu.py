@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import conv_grad_sweep_common as S
+import fp64_bound as fb
 
 
 def test_every_class_has_a_case():
@@ -96,7 +97,7 @@ def test_bound_holds_for_the_scaled_split(ex, ew, edy):
         x, w, b, dy = S.scaled(x, w, b, dy, ex, ew, edy)
         got, bnd = _emulate(case, x, w, b, dy, True), S.bounds(case, x, w, b, dy)
         for name in got:
-            q, at = S.worst_ratio(got[name], *bnd[name])
+            q, at = fb.worst(got[name], *bnd[name])
             assert q <= 1.0, (name, q, at, case, (ex, ew, edy))
 
 
@@ -108,10 +109,10 @@ def test_bound_breaks_for_the_unscaled_split(ex):
         x, w, b, dy = S.scaled(x, w, b, dy, ex, 0, 0)
         got, bnd = _emulate(case, x, w, b, dy, False), S.bounds(case, x, w, b, dy)
         for name in ("y", "dW"):
-            q, _ = S.worst_ratio(got[name], *bnd[name])
+            q, _ = fb.worst(got[name], *bnd[name])
             assert q > 4.0, (name, q, case, ex)
         ok = _emulate(case, x, w, b, dy, True)
-        assert S.worst_ratio(ok["y"], *bnd["y"])[0] <= 1.0
+        assert fb.worst(ok["y"], *bnd["y"])[0] <= 1.0
 
 
 def test_split_exponent():

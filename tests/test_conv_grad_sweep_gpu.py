@@ -14,6 +14,7 @@ import pytest
 import torch
 
 import conv_grad_sweep_common as S
+import fp64_bound as fb
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
@@ -47,7 +48,8 @@ def check(case, x, w, b, dy, what="", got=None, select=None):
             g, r, base, floor = (select[name](t) for t in (g, r, base, floor))
         assert torch.isfinite(g).all(), "%s has NaN / inf at %s: %s %s" % (
             name, tuple(int(v) for v in (~torch.isfinite(g)).nonzero()[0]), what, case)
-        q, at = S.worst_ratio(g, r, base, floor)
+        assert torch.isfinite(r).all(), (name, "a non-finite reference", what, case)
+        q, at = fb.worst(g, r, base, floor)
         print("RATIO %s %.4f %s %s" % (name, q, what, case))
         assert q <= C, "%s off by %.3g x the bound at %s (got %r, want %r): %s %s" % (
             name, q / C, at, float(g[at]), float(r[at]), what, case)

@@ -23,11 +23,12 @@ import pytest
 import torch
 
 from conv_sweep_common import CASES, base, out_hw, report
+import fp64_bound as fb
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
-U = {"exact": 2.0 ** -22, "fast": 2.0 ** -10}
+U_MMA = {"exact": 2.0 ** -22, "fast": 2.0 ** -10}
 FLOOR = 2.0 ** -25
 U_PLANES = {"exact": 2.0 ** -22, "fast": 2.0 ** -11}
 C = {"exact": 3.0, "fast": 2.0}
@@ -59,14 +60,11 @@ def _reference(case, x, w, b, res):
     return r, A, Ws
 
 
-def _ratio(y, view, prec, r, A, Ws, res_planes=False):
+def _worst(y, view, prec, r, A, Ws, res_planes=False):
     """the worst error of one output view in units of the bound's c (<= C[prec] passes), and where"""
-    u_out, f_out = (2.0 ** -24, 0.0) if view == "f32" else (U_PLANES[prec], FLOOR)
+    u_out, f_out = (fb.U24, 0.0) if view == "f32" else (U_PLANES[prec], FLOOR)
     assert torch.isfinite(y).all(), "%s output has NaN / inf (unwritten or overflowed elements)" % view
-    excess = (y.double() - r).abs() - u_out * r.abs() - f_out
-    q = excess / (U[prec] * A + FLOOR * (Ws + (1.0 if res_planes else 0.0)) + 1e-300)
-    i = int(q.argmax())
-    return float(q.flatten()[i]), tuple(int(v) for v in torch.unravel_index(torch.tensor(i), q.shape))
+    return fb.worst(y, r, U_MMA[prec] * A + FLOOR * (Ws + (1.0 if res_planes else 0.0)), u_out * r.abs() + f_out)
 
 
 def _run(case, x, w, b, res):
@@ -87,7 +85,7 @@ def _check(case, x, w, b, res, out=None, what=""):
     for view in ("f32", "planes"):
         if view not in out:
             continue
-        q, at = _ratio(out[view], view, prec, r, A, Ws, res_planes=case[9] == "planes")
+        q, at = _worst(out[view], view, prec, r, A, Ws, res_planes=case[9] == "planes")
         print("RATIO %s %s %.3f %s %s" % (prec, view, q, what, case))
         assert q <= C[prec], ("%s view off by %.2f x the %s bound at (n, oh, ow, co) = %s" % (view, q / C[prec], prec, at),
                               what, case, report(case))
@@ -124,8 +122,8 @@ def test_long_sums_of_non_negative_data_are_not_biased(case):
     r, A, Ws = _reference(case, x, w, b, res)
     _check(case, x, w, b, res, out=out, what="uniform")
     mean = float(((out["f32"].double() - r) / A).mean())
-    print("BIAS %.4f u %s" % (mean / U["exact"], case))
-    assert abs(mean) <= C_BIAS * U["exact"], ("mean signed error %.3f u" % (mean / U["exact"]), case, report(case))
+    print("BIAS %.4f u %s" % (mean / U_MMA["exact"], case))
+    assert abs(mean) <= C_BIAS * U_MMA["exact"], ("mean signed error %.3f u" % (mean / U_MMA["exact"]), case, report(case))
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -183,14 +181,14 @@ def test_outputs_beyond_the_planes_range(prec):
     torch.cuda.synchronize()
     out = collect(outs)
     r, A, Ws = _reference(case, x, w, b, None)
-    q, at = _ratio(out["f32"], "f32", prec, r, A, Ws)
+    q, at = _worst(out["f32"], "f32", prec, r, A, Ws)
     assert q <= C[prec], (q, at)
     over = out["f32"].abs() >= 65520.0                            # rn_f16 overflows from here
     assert over.any() and (r.abs() > 65504).float().mean() > 0.01
     assert (out["hi"][over].float().abs() >= 65504.0).all()       # no finite value of the wrong magnitude
     inside = out["f32"].abs() < 65504.0
     err = (out["planes"].double() - r).abs()[inside]
-    lim = (C[prec] * (U[prec] * A + FLOOR * Ws) + U_PLANES[prec] * r.abs() + FLOOR)[inside]
+    lim = (C[prec] * (U_MMA[prec] * A + FLOOR * Ws) + U_PLANES[prec] * r.abs() + FLOOR)[inside]
     assert (err <= lim).all()
 
 
@@ -250,7 +248,7 @@ def _check_impulses(shape, prec, images=None):
                 want[n, oh // s, ow // s] += w[n % G, (r * k + c) * Cin + ci].double()
                 tap_at[(n, oh // s, ow // s)] = (r, c, ci)
     out = _run(case, x, w, b, None)
-    for view, u in (("f32", U[prec]), ("planes", U[prec] + U_PLANES[prec])):
+    for view, u in (("f32", U_MMA[prec]), ("planes", U_MMA[prec] + U_PLANES[prec])):
         y = out[view].double()
         tol = torch.zeros_like(want)
         for (n, oh, ow) in tap_at:
@@ -403,7 +401,7 @@ def test_output_offsets_past_4_gib(case):
         got = {"f32": y.view(-1, Cout)[idx].cpu(),
                "planes": yh.view(-1, Cout)[idx].float().cpu() + (yl.view(-1, Cout)[idx].float().cpu() if exact else 0.0)}
         for view in got:
-            q, at = _ratio(got[view], view, prec, r, A, Ws)
+            q, at = _worst(got[view], view, prec, r, A, Ws)
             assert q <= C[prec], (view, q, at, int(idx[at[0]]))
     finally:
         del y, yh, yl, x, xp

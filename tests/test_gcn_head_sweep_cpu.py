@@ -8,6 +8,7 @@ import os
 import pytest
 import torch
 
+import fp64_bound as fb
 import gcn_head_sweep_common as gs
 from oracle import gcn_head as og
 
@@ -17,7 +18,7 @@ COMPOSE = [c for c in gs.CASES if c.B <= 16 and not c.nonfinite and c.adj != "na
 
 
 def test_every_class_has_a_case():
-    assert gs.uncovered() == []
+    assert fb.uncovered(gs.CASES, gs.CLASSES) == []
 
 
 def _autograd(c, inp):
@@ -161,6 +162,7 @@ def test_clean_emulation_stays_well_inside(c):
     for name, st in S.items():
         if name.startswith("_") or st.kind == "exact":
             continue
-        lim = gs.limit(st) / (2 if st.kind == "rel" or st.C <= 7 else 4)
-        x = gs.excess(got[name], st)
+        scale, floor, lim = gs.bound(st)
+        lim = lim / (2 if st.kind == "rel" or st.C <= 7 else 4)
+        x = fb.worst(got[name], st.r, scale, floor)[0]
         assert x <= lim, (name, x, lim)

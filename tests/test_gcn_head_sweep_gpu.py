@@ -7,6 +7,7 @@ import ctypes
 import pytest
 import torch
 
+import fp64_bound as fb
 import gcn_head_sweep_common as gs
 from oracle import gcn_head as og
 
@@ -85,7 +86,7 @@ def test_case_stages_and_bits(c):
     di = _dev(inp)
     got = run_c(c, di, float("nan"))
     S = gs.stages(c, inp, got, device=DEV)
-    worst = {n: gs.ratio(got[n], st) for n, st in S.items() if not n.startswith("_") and n in got}
+    worst = {n: fb.err_ratio(got[n], st.r, gs.bound(st)[0]) for n, st in S.items() if not n.startswith("_") and n in got}
     top = sorted(worst.items(), key=lambda kv: -kv[1])[:4]
     print("%s worst |err|/(2^-24 M): %s" % (gs.case_id(c), ", ".join("%s %.3g" % kv for kv in top)))
     bad = gs.check(got, S)

@@ -9,13 +9,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import fp64_bound as fb
 import layers_sweep_common as S
 
 SMALL = 200000                       # cases up to this many elements are emulated on the CPU
 
 
 def test_every_class_is_covered():
-    missing = S.uncovered()
+    missing = ["%s: %s" % (op, name) for op, (cases, classes) in S.TABLES.items() for name in fb.uncovered(cases, classes)]
     assert not missing, "uncovered classes: " + "; ".join(missing)
 
 
@@ -269,6 +270,11 @@ def emulate_fuse_dt(dz, f, bad_stride=False):
 BN_EMU = [c for c in S.BN_CASES if c.N * c.C * c.H * c.W <= SMALL and not c.nonfinite]
 
 
+def _worst(got, r, M, tiny=fb.TINY):
+    """the excess over the floor in units of 2^-24 M: <= C passes"""
+    return fb.worst(got, r, fb.U24 * M, fb.U24 * r.abs() + tiny)[0]
+
+
 def _bn_ratios(c, defect=None):
     p = S.make_bn(c)
     got = emulate_bn(c, p, defect)
@@ -277,7 +283,7 @@ def _bn_ratios(c, defect=None):
     out = {}
     for k, (r, M, tiny) in ref.items():
         if k != "dr":
-            out[k] = (S.worst_ratio(got[k], r, M, S.BN_C[k], tiny), S.BN_C[k])
+            out[k] = (_worst(got[k], r, M, tiny), S.BN_C[k])
     return out
 
 
@@ -305,7 +311,7 @@ def _pool_case_ratio(c, skip_fourth):
     x, dy = S.make_pool(c)
     dx, idx = emulate_pool_dx(x, dy, skip_fourth)
     r, M, _ = S.pool_backward_reference(idx, dy, c.H, c.W)
-    return S.worst_ratio(dx, r, M, S.C_POOL_DX)
+    return _worst(dx, r, M)
 
 
 def _avg_ratios(c, bad):
@@ -314,14 +320,14 @@ def _avg_ratios(c, bad):
     HW = c.H * c.W
     xd = x.double()
     r = (dy.double() / HW).expand_as(xd)
-    return (S.worst_ratio(y, xd.mean((2, 3), keepdim=True), xd.abs().mean((2, 3), keepdim=True), S.c_avg_y(HW)),
-            S.worst_ratio(dx, r, r.abs(), S.C_AVG_DX))
+    return (_worst(y, xd.mean((2, 3), keepdim=True), xd.abs().mean((2, 3), keepdim=True)),
+            _worst(dx, r, r.abs()))
 
 
 def _lin_ratio(c, drop):
     x, w, b, a, dy = S.make_lin(c)
     r, M = S.lin_reference(x, w, b, a, dy)["y"]
-    return S.worst_ratio(emulate_linear_y(x, w, b, a, drop), r, M, S.c_lin_y(c.In))
+    return _worst(emulate_linear_y(x, w, b, a, drop), r, M)
 
 
 def _fuse_ratios(c, bad):
@@ -331,7 +337,7 @@ def _fuse_ratios(c, bad):
     out = []
     for f in c.factors:
         r, M = S.fuse_backward_reference(dz, f)
-        out.append((S.worst_ratio(emulate_fuse_dt(dz, f, bad), r, M, S.c_fuse_dx(f)), S.c_fuse_dx(f)))
+        out.append((_worst(emulate_fuse_dt(dz, f, bad), r, M), S.c_fuse_dx(f)))
     return out
 
 

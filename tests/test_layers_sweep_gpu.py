@@ -9,6 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import fp64_bound as fb
 import layers_sweep_common as S
 
 pytestmark = pytest.mark.gpu
@@ -38,10 +39,10 @@ def report(name, ratios):
     print("%s  %s" % (name, "  ".join("%s %.2f" % kv for kv in ratios.items())))
 
 
-def hold(name, got, r, M, C, tiny=S.TINY):
-    q = S.worst_ratio(got, r, M, C, tiny)
+def hold(name, got, r, M, C, tiny=fb.TINY, finiteness_only=False):
+    q = fb.worst(got, r, fb.U24 * M, fb.U24 * r.abs() + tiny, finiteness_only)[0]
     assert q <= C, "%s: worst excess %.3g units of 2^-24 M over the bound's %d" % (name, q, C)
-    return S.err_ratio(got, r, M)
+    return fb.err_ratio(got, r, fb.U24 * M)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -77,7 +78,7 @@ def test_batch_norm(c):
         assert torch.equal(torch.isnan(got["y"]), torch.isnan(z)), "ReLU output: NaN pattern differs from relu(z)"
         flips = (mask != (z > 0)) & ~torch.isnan(z)
         r_y, M_y, _ = ref["y"]
-        assert bool((z[flips].abs() <= 2 * S.C_BN_Y * S.U * M_y[flips] + S.TINY).all()), "ReLU mask flips away from 0"
+        assert bool((z[flips].abs() <= 2 * S.C_BN_Y * fb.U24 * M_y[flips] + fb.TINY).all()), "ReLU mask flips away from 0"
     ratios = {}
     for k, (r, M, tiny) in ref.items():
         assert got[k] is not None and got[k].dtype == torch.float32 and got[k].shape == r.shape, k
@@ -85,7 +86,9 @@ def test_batch_norm(c):
             fin = torch.isfinite(r)
             assert torch.equal(got[k][fin].double(), r[fin]) and torch.equal(torch.isnan(got[k]), torch.isnan(r)), k
             continue
-        ratios[k] = hold(k, got[k], r, M, S.BN_C[k], tiny)
+        # a channel whose x holds +inf: the reference's correction pass makes its mean inf - inf = NaN, while the op
+        # keeps the +inf torch's batch_norm gives in the running mean (N4C3_7x7_train_relu_m1_s1_nonfinitex)
+        ratios[k] = hold(k, got[k], r, M, S.BN_C[k], tiny, finiteness_only=k == "rm")
     for k in ("dx", "dw", "db", "dr"):
         if k not in ref:
             assert k not in got or got[k] is None, k

@@ -12,13 +12,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import fp64_bound as fb
 import loss_sweep_common as S
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_every_class_is_covered():
-    missing = [k for k, n in S.coverage().items() if n == 0]
+    missing = fb.uncovered(S.CASES, S.CLASSES)
     assert not missing, "classes with no case: %s" % ", ".join(missing)
 
 
@@ -213,7 +214,7 @@ def check_all(got, ref, where):
     worst = {}
     for k, val in got.items():
         r, M, C = ref[k]
-        worst[k] = S.worst_ratio(torch.from_numpy(np.asarray(val)), r, M, C, "%s %s" % (where, k))
+        worst[k] = fb.worst(torch.from_numpy(np.asarray(val)), r, *S.bound(r, M, C))[0]
         assert worst[k] <= 1.0, "%s %s: error %.3g of the bound" % (where, k, worst[k])
     return worst
 
@@ -274,7 +275,7 @@ def test_part_host_walk_within_bound(hostlibs, c):
     p = S.make_part(c)
     r, M, C, flips, worst = S.part_reference(c, p)
     assert worst <= 1.0, "a background decision differs from fp64 away from 0.5"
-    q = S.worst_ratio(torch.from_numpy(host_part(hostlibs[1], c, p)), r, M, C, S.part_id(c))
+    q = fb.worst(torch.from_numpy(host_part(hostlibs[1], c, p)), r, *S.bound(r, M, C))[0]
     assert q <= 1.0
     if c.theta == "out":
         assert float(r.abs().max()) == 0.0
@@ -324,7 +325,7 @@ def _emu_ratio(kind, c, defect):
         if bool((torch.isfinite(got) != fin).any()) or bool((torch.isnan(got) != torch.isnan(r)).any()):
             worst.append((float("inf"), 1.0))
             continue
-        e = ((got - r).abs() - S.U * r.abs() - S.TINY).clamp(min=0) / (S.U * torch.as_tensor(M).to(S.F64).expand_as(r))
+        e = ((got - r).abs() - fb.U24 * r.abs() - fb.TINY).clamp(min=0) / (fb.U24 * torch.as_tensor(M).to(S.F64).expand_as(r))
         e = torch.where(fin, e.nan_to_num(0, float("inf"), 0), torch.zeros((), dtype=S.F64))
         k_ = int(e.argmax())
         worst.append((float(e.view(-1)[k_]), float(Ct.reshape(-1)[k_])))

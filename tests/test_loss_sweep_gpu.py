@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+import fp64_bound as fb
 import loss_sweep_common as S
 
 pytestmark = pytest.mark.gpu
@@ -31,7 +32,7 @@ def hold(name, got, ref):
     out = {}
     for k, val in got.items():
         r, M, C = ref[k]
-        out[k] = S.worst_ratio(val.cpu(), r, M, C, "%s %s" % (name, k))
+        out[k] = fb.worst(val.cpu(), r, *S.bound(r, M, C))[0]
         assert out[k] <= 1.0, "%s %s: error %.3g of the bound" % (name, k, out[k])
     report(name, out)
 
@@ -199,7 +200,7 @@ def test_part(c):
     torch.cuda.synchronize()
     r, M, C, flips, worst = S.part_reference(c, p)
     assert worst <= 1.0
-    q = S.worst_ratio(out.cpu(), r, M, C, S.part_id(c))
+    q = fb.worst(out.cpu(), r, *S.bound(r, M, C))[0]
     report(S.part_id(c), {"out": q, "bg flips": flips})
     assert q <= 1.0
     same_bits(out, Lm.part_iuv_targets([U, V, I], th, align_corners=c.align), "op")

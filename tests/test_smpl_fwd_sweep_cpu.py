@@ -11,12 +11,12 @@ import torch
 
 from oracle import lbs as olbs
 from oracle import lbs_grad
+import fp64_bound as fb
 import smpl_fwd_sweep_common as sc
 
 
 def test_every_class_is_covered():
-    cov = sc.coverage()
-    missing = [name for name, idx in cov.items() if not idx]
+    missing = fb.uncovered(sc.CASES, sc.CLASSES)
     assert not missing, "uncovered classes: %s" % missing
 
 
@@ -50,8 +50,8 @@ def test_rodrigues_magnitude_bounds_an_fp32_evaluation():
                     s * z + c1 * (x * y), one + c1 * (-(z * z) - x * x), s * (-x) + c1 * (y * z),
                     s * (-y) + c1 * (x * z), s * x + c1 * (y * z), one + c1 * (-(y * y) - x * x)], 1).reshape(-1, 3, 3)
     M = sc.rodrigues_magnitude(a)
-    excess = np.abs(got - R) - sc.U * np.abs(R)
-    q = np.where(excess <= 0, -np.inf, excess / np.maximum(sc.U * M, 1e-300))
+    excess = np.abs(got - R) - fb.U24 * np.abs(R)
+    q = np.where(excess <= 0, -np.inf, excess / np.maximum(fb.U24 * M, 1e-300))
     print("fp32 rodrigues: worst ratio %.3g (C_AA = %d)" % (q.max(), sc.C_AA))
     assert q.max() <= sc.C_AA / 2
 
@@ -176,9 +176,9 @@ def _case_data(i):
     return m, inp, sc.reference(c, m, inp, with_h36m=c.out != "no_h36m")
 
 
-def _ratio(got, ref):
+def _worst(got, ref):
     """the worst q / C over the outputs (<= 1 passes), and the output"""
-    qs = {k: sc.worst_ratio(got[k].reshape(r.shape), r, M, slack) / C for k, (r, M, slack, C) in ref.items()}
+    qs = {k: fb.worst(got[k], r, fb.U24 * M, fb.U24 * r.abs() + fb.TINY + slack)[0] / C for k, (r, M, slack, C) in ref.items()}
     k = max(qs, key=qs.get)
     return qs[k], k
 
@@ -187,7 +187,7 @@ def test_manual_forward_meets_the_bound():
     worst = {}
     for i, c in enumerate(sc.CASES):
         m, inp, ref = _case_data(i)
-        q, k = _ratio(manual_forward(c, m, inp), ref)
+        q, k = _worst(manual_forward(c, m, inp), ref)
         worst[sc.route(c)] = max(worst.get(sc.route(c), -np.inf), q)
         assert q <= 1.0, (sc.case_id(c), k, q)
     print("fp64 restatement: worst error / bound per route %s" % worst)
@@ -198,7 +198,7 @@ def test_bound_catches_mutant(mutant):
     worst, where = -np.inf, None
     for i, c in enumerate(sc.CASES):
         m, inp, ref = _case_data(i)
-        q, k = _ratio(manual_forward(c, m, inp, mutant=mutant), ref)
+        q, k = _worst(manual_forward(c, m, inp, mutant=mutant), ref)
         if q > worst:
             worst, where = q, "%s %s" % (sc.case_id(c), k)
     print("mutant %s: worst error / bound %.3g at %s" % (mutant, worst, where))
@@ -233,7 +233,7 @@ def test_float32_restatement_meets_a_quarter_of_the_bound():
             continue
         m, inp, _ = _case_data(i)
         ref = sc.reference(c, m, inp, with_h36m=c.out != "no_h36m", gemm=False)
-        q, k = _ratio(_float32_forward(c, m, inp), ref)
+        q, k = _worst(_float32_forward(c, m, inp), ref)
         worst = max(worst, q)
         assert q <= 0.25, (sc.case_id(c), k, q)
     print("float32 restatement: worst error / bound %.3g (<= 1/4)" % worst)

@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from oracle import lbs as olbs
+import fp64_bound as fb
 import smpl_fwd_sweep_common as sc
 
 pytestmark = pytest.mark.gpu
@@ -63,7 +64,7 @@ def test_case_meets_the_bound(case):
     fails = []
     for name, (r, M, slack, C) in ref.items():
         g = got[name][idx].reshape(r.shape)
-        q, e = sc.worst_ratio(g, r, M, slack), sc.err_ratio(g, r, M)
+        q, e = fb.worst(g, r, fb.U24 * M, fb.U24 * r.abs() + fb.TINY + slack)[0], fb.err_ratio(g, r, fb.U24 * M)
         key = (sc.skin_path(case), name)
         _WORST[key] = max(_WORST.get(key, -np.inf), q / C)
         print("%s %s: worst |err| / (2^-24 M) = %.3g, beyond the floor and slack %.3g (C = %d)"
@@ -211,8 +212,8 @@ def test_mpjpe_meets_the_bound(regime):
     D = np.abs(p[:, olbs.H36M_TO_J14]) + np.abs(p[:, :1]) + np.abs(g)
     M = np.sqrt((D ** 2).sum(-1)).mean(-1)
     err = np.abs(got - r)
-    q = (err - sc.U * np.abs(r) - sc.TINY) / (sc.U * M)
-    print("mpjpe %s: worst |err| / (2^-24 M) = %.3g (C = %d)" % (regime, (err / (sc.U * M)).max(), C_MPJPE))
+    q = (err - fb.U24 * np.abs(r) - fb.TINY) / (fb.U24 * M)
+    print("mpjpe %s: worst |err| / (2^-24 M) = %.3g (C = %d)" % (regime, (err / (fb.U24 * M)).max(), C_MPJPE))
     assert (q <= C_MPJPE).all(), q.max()
     if regime == "exact_match":
         assert (got == 0).all()

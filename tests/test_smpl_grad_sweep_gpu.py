@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from oracle import lbs as olbs
+import fp64_bound as fb
 import smpl_grad_sweep_common as sc
 
 pytestmark = pytest.mark.gpu
@@ -51,8 +52,8 @@ def test_case_meets_the_bound(case):
     ref = sc.reference(mdl, sc.subset(inp, idx), device=DEV)
     for route, got in (("backward_lbs", _backward_lbs(smpl, mdl, inp)), ("autograd", _autograd(smpl, inp))):
         got = [g[idx] for g in got]
-        q = max(sc.worst_ratio(g, r, M) for g, (r, M) in zip(got, ref))
-        e = max(sc.err_ratio(g, r, M) for g, (r, M) in zip(got, ref))
+        q = max(fb.worst(g, r, fb.U24 * M, fb.U24 * r.abs() + fb.TINY)[0] for g, (r, M) in zip(got, ref))
+        e = max(fb.err_ratio(g, r, fb.U24 * M) for g, (r, M) in zip(got, ref))
         print("%s %s: worst |err| / (2^-24 M) = %.3g (C = %d)" % (sc.case_id(case), route, e, sc.C))
         assert q <= sc.C, (route, q)
 
